@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- the driver-facing benchmark of the RetinaNet inference hot path (see DESIGN.md).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload full|postproc]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload full|postproc] [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
 
 One JSON line on rank 0.  A "step" is one pass of the hot path over one batch of synthetic input:
@@ -33,11 +33,12 @@ def _peaks():
         d = json.load(open(p))
         return {"hbm": d["hbm_gbs"], "tensor": d["bf16_tflops"], "tensor_sustained": d.get("bf16_tflops_sustained"),
                 "source": "measured"}
-    return {"hbm": 6650.0, "tensor": 1590.0, "tensor_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense FP16 989 TFLOP/s -- not reached figures
+    return {"hbm": 3350.0, "tensor": 989.0, "tensor_sustained": None, "source": "H100 SXM data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index, self.rows, self.proc = index, [], None
@@ -64,6 +65,7 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        self.proc.wait()
         sm, mx, reasons, power = [], None, set(), []
         for (t, line) in self.rows:
             f = [x.strip() for x in line.split(",")]
@@ -120,10 +122,11 @@ class FullWorkload:
         sd = make_state_dict(backbone, 80, na, rotated, seed=0)
         model = Model(backbone, classes=80, rotated_bbox=rotated)
 
-        def gpu_logits(s):   # probe: 2 images through the CUDA engine
-            model.load_state_dict(s).cuda(device.index)
-            return model.forward_heads(self.dev_x[:2], sigmoid=False)[0]
-        self.sd = synth.calibrate_cls_head(sd, gpu_logits)
+        # calibrated on the fp32 CPU oracle over a fixed probe (as the reference arm does): the weights, hence the inputs
+        # of every step, do not depend on the build under test
+        from oracle import model_ref
+        probe = torch.randn((1, 3, 256, 384), generator=torch.Generator().manual_seed(3))
+        self.sd = synth.calibrate_cls_head(sd, lambda s: model_ref.forward_heads(s, backbone, probe, sigmoid=False)[0])
         self.model = model.load_state_dict(self.sd).cuda(device.index)
         if os.environ.get("ODTK_BENCH_CUDA_GRAPH", "1") != "0":
             self.model.enable_cuda_graph()
@@ -252,17 +255,11 @@ class FullWorkload:
                 "weights": "random init (seed 0), BatchNorm folded, class head calibrated to ~0.56% scores > 0.05",
                 "cuda_graph": getattr(self.model, "_graphs", None) is not None,
                 "detections_in_last_step": n_det,
-                "l2": "activations of a step (GBs) exceed the 126 MB L2; input batch %.0f MB" % (self.h2d_bytes / 1e6)}
+                "l2": "activations of a step (GBs) exceed the 50 MB L2; input batch %.0f MB" % (self.h2d_bytes / 1e6)}
 
-    PROFILE = "r02_layer_table.json"
-
-    def _profiled_traffic(self):
-        if not (self.backbone == "ResNet50FPN" and self.batch == 32 and not self.rotated):
-            return None
-        try:
-            return int(json.load(open(os.path.join(ROOT, "profiles", self.PROFILE)))["summary"]["conv_dram_bytes"])
-        except (OSError, KeyError, ValueError):
-            return None
+    def outputs(self):
+        """What the timed step returned: detections per image (scores [B, D], boxes [B, D, 4|6], classes [B, D])."""
+        return dict(zip(("scores", "boxes", "classes"), self.out))
 
     def roofline(self, lib, peaks, steps):
         ms, n = _prof_get(lib, 3)
@@ -281,13 +278,11 @@ class FullWorkload:
                           "algorithmic_bytes_per_step": int(sum(l["bytes"] for l in self.trace)),
                           "note": "sum over the step's launches of max(FLOPs/tensor peak, operand+output bytes/HBM peak): "
                                   "the bound of layer-by-layer execution; frac_of_step = ideal / measured ms_per_step"}
-        return {"kernel": "conv_gemm_kernel + bottleneck_tail_kernel + stem_pool_kernel (tcgen05, all %d conv launches of a step)" % (n // steps), "bound": "tensor",
+        return {"kernel": "conv_gemm_kernel (wgmma, all %d conv launches of a step)" % (n // steps), "bound": "tensor",
                 "achieved": round(achieved, 1), "peak": peak, "unit": "TFLOP/s", "frac": round(achieved / peak, 4),
-                # dram__bytes_read.sum + dram__bytes_write.sum summed over the conv launches of ONE step, from the
-                # committed ncu capture of this workload (tools/capture_step.py -> profiles/r02_layer_table.json)
-                "traffic": self._profiled_traffic(),
-                "traffic_note": "bytes per step (all conv launches), from profiles/%s (ncu, same workload)" % self.PROFILE,
-                "peak_source": peaks["source"] + " (MEASURED_PEAKS.json bf16_tflops_sustained: kernel timed inside a long step)",
+                "traffic": None,
+                "traffic_note": "DRAM bytes per step: not measured",
+                "peak_source": peaks["source"],
                 "avg_launch_ms": round(ms / n, 5), "launches_timed": n,
                 "algorithmic_flops_per_step": int(self.flops_per_step),
                 "conv_share_of_step": None}
@@ -427,7 +422,11 @@ class PostprocWorkload:
     def config(self):
         return {"workload": self.name, "images_per_gpu": self.batch, "top_n": 1000, "detections": 100,
                 "threshold": 0.05, "nms": 0.5, "batches_in_flight": max(1, self.nstreams),
-                "l2": "inputs (%.0f MB per step per GPU) exceed the 126 MB L2" % (self.h2d_bytes / 1e6)}
+                "l2": "inputs (%.0f MB per step per GPU) exceed the 50 MB L2" % (self.h2d_bytes / 1e6)}
+
+    def outputs(self):
+        """What the timed step returned: detections per image (scores [B, D], boxes [B, D, 4|6], classes [B, D])."""
+        return dict(zip(("scores", "boxes", "classes"), self.out))
 
     def roofline(self, lib, peaks, steps):
         ms, n = _prof_get(lib, 0)
@@ -438,8 +437,7 @@ class PostprocWorkload:
         achieved = bytes_per_launch / (avg_ms * 1e-3) / 1e9
         return {"kernel": "score_filter_kernel", "bound": "hbm", "achieved": round(achieved, 1),
                 "peak": peaks["hbm"], "unit": "GB/s", "frac": round(achieved / peaks["hbm"], 4),
-                # ncu --set full capture of this kernel at batch 8 (profiles/r01_score_filter_ncu_summary.json)
-                "traffic": 497508352 if (self.batch == 8 and not self.rotated) else None, "peak_source": peaks["source"] + " (MEASURED_PEAKS.json hbm_gbs, burst copy)",
+                "traffic": None, "peak_source": peaks["source"],
                 "avg_launch_ms": round(avg_ms, 5), "launches_timed": n,
                 "algorithmic_bytes_per_launch": int(bytes_per_launch),
                 "note": "one launch per step streams the scores of all 5 levels of the batch"}
@@ -517,6 +515,20 @@ def postproc_sub(device, peaks, lib, rotated=False, batch=8, steps=30):
             "note": "per-kernel times come from event-bracketed launches of the one-batch-at-a-time loop", "roofline": roof}
 
 
+def dump_outputs(arrays, out_dir, limit=64 << 20):
+    """Every array as out_dir/<name>.npy in float32; an array larger than its share of `limit` bytes is replaced by a
+    fixed, seeded sample of its flattened elements (the same positions in every run)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = limit // max(1, len(arrays)) // 4
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.size > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=share // 2, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -530,6 +542,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-postproc", action="store_true", help="skip the decode+NMS sub-measurement of the default line")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (float32; rank 0)")
     ap.add_argument("--config", default=None, choices=sorted(CONFIGS),
                     help="BASELINE.json matrix presets: " + ", ".join("%s = %s" % kv for kv in sorted(CONFIGS.items())))
     args = ap.parse_args()
@@ -603,6 +617,8 @@ def main():
         # pass 1: the measured value (no per-kernel events in the stream)
         ms, t0, t1 = timed(wl.step, args.steps, profile=False)
         clocks = sampler.stop(t0, t1) if rank == 0 else None
+        if args.dump_outputs and rank == 0:
+            dump_outputs(wl.outputs(), args.dump_outputs)
         # pass 2: same steps with the dominant kernel bracketed by CUDA events (roofline numbers)
         ms_prof, _, _ = timed(getattr(wl, "step_profile", wl.step), args.steps, profile=True)
         roof = wl.roofline(lib, peaks, args.steps)
@@ -686,7 +702,7 @@ def main():
 def reference_arm(args, rank, world):
     """The reference's CPU implementation of the path on this box's host cores.  /root/reference (Python) cannot travel to
     the GPU box, so this is the oracle port: oracle/model_ref.py (the same torch CPU convolutions nn.Conv2d runs) +
-    oracle decode/nms.  Protocol (BASELINE.md section 3): --warmup untimed and EXACTLY --steps timed single-image passes
+    oracle decode/nms.  Protocol: --warmup untimed and EXACTLY --steps timed single-image passes
     (one image of the configured workload per step: a bounded sample), a fixed thread count, the MEDIAN pass time is
     the reported step time.  Rank 0 only; other ranks exit 0."""
     if rank != 0:

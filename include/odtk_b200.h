@@ -1,5 +1,5 @@
 /*
- * odtk_b200.h -- C ABI of the B200-native RetinaNet inference hot path.
+ * odtk_b200.h -- C ABI of the H100-native RetinaNet inference hot path.
  *
  * Drop-in boundary for NVIDIA/retinanet-examples (ODTK).  Every entry point is
  * plain C: raw device pointers, sizes, a cudaStream_t passed as void*.  No torch,
@@ -30,17 +30,17 @@ extern "C" {
 #define ODTK_OK 0
 #define ODTK_E_INVALID (-1)     /* bad argument (null pointer, size <= 0, ...)      */
 #define ODTK_E_WORKSPACE (-2)   /* workspace too small (reference: utils.h:55-57)    */
-#define ODTK_E_UNSUPPORTED (-3) /* size outside what the sm_100a kernels handle     */
+#define ODTK_E_UNSUPPORTED (-3) /* size outside what the sm_90a kernels handle     */
 #define ODTK_E_CUDA (-4)        /* a CUDA runtime / driver call failed               */
 
 typedef void *odtk_stream_t; /* cudaStream_t */
 
-/* Limits of the sm_100a kernels (documented deviations from "any size"). */
+/* Limits of the sm_90a kernels (documented deviations from "any size"). */
 #define ODTK_MAX_TOP_N 4096      /* decode: top_n                                   */
 #define ODTK_MAX_NMS_COUNT 6144  /* nms: candidates per image                       */
 #define ODTK_MAX_DETECTIONS 1024 /* nms: detections_per_im                          */
 
-/* Library identification: returns a static string "odtk_b200 <version> sm_100a". */
+/* Library identification: returns a static string "odtk_b200 <version> sm_90a". */
 const char *odtk_b200_version(void);
 
 /* ---- decode -------------------------------------------------------------------
@@ -63,7 +63,7 @@ long long odtk_decode_rotate(int batch, const void *const *inputs, void *const *
                              const float *anchors, size_t num_anchor_floats, float score_thresh,
                              int top_n, void *workspace, size_t workspace_size, odtk_stream_t stream);
 
-/* Extended decode (B200-native addition): same maths, but the three outputs are
+/* Extended decode (H100-native addition): same maths, but the three outputs are
  * written at element offset out_offset of rows that are out_stride entries long,
  * so that the five pyramid levels land directly in the [B, 5*top_n] buffers the
  * reference builds with torch.cat (odtk/model.py:164).  nbox = 4 or 6.          */
@@ -73,7 +73,7 @@ long long odtk_decode_ex(int batch, const void *const *inputs, void *const *outp
                          int top_n, int nbox, size_t out_stride, size_t out_offset, void *workspace,
                          size_t workspace_size, odtk_stream_t stream);
 
-/* All pyramid levels of the whole batch in three launches (B200-native addition; the
+/* All pyramid levels of the whole batch in three launches (H100-native addition; the
  * reference calls decode once per level, odtk/model.py:153-161, and torch.cat's the
  * results, :164).  Level l writes columns [out_offset + l*top_n, +top_n) of the
  * [B, out_stride] outputs.  anchors in odtk_level_t is a HOST pointer (4*A floats). */
@@ -90,7 +90,7 @@ long long odtk_decode_levels(int batch, int num_levels, const odtk_level_t *leve
                              int nbox, void *const *outputs, size_t out_stride, size_t out_offset,
                              void *workspace, size_t workspace_size, odtk_stream_t stream);
 
-/* Fused class-head path (B200-native): the last class-head convolution appends its above-threshold
+/* Fused class-head path (H100-native): the last class-head convolution appends its above-threshold
  * scores straight to the decode workspace (odtk_conv2d with out_mode ODTK_OUT_CANDIDATES and the level's
  * sink) instead of writing the dense [B, A*C, H, W] score map that odtk_decode_levels would stream
  * through again.  odtk_decode_fused_begin lays out `workspace` (query the size with workspace == NULL)
@@ -143,7 +143,7 @@ long long odtk_nms_ex(int batch, const void *const *inputs, void *const *outputs
                       int32_t *out_index, void *workspace, size_t workspace_size,
                       odtk_stream_t stream);
 
-/* nms + gather (B200-native).  As odtk_nms_ex, plus:
+/* nms + gather (H100-native).  As odtk_nms_ex, plus:
  *   packed (device [B, D, 2 + nbox] fp32, may be NULL): the detections as (score, box..., class) rows -- the layout that
  *     travels between ranks; outputs may then be NULL.
  *   gather (may be NULL): image-wise sharded inference (odtk/infer.py:98-102 all_gathers the per-rank results).  Here
@@ -168,7 +168,7 @@ long long odtk_nms_gather(int batch, const void *const *inputs, void *const *out
                           odtk_stream_t stream);
 int odtk_gather_wait(const odtk_gather_t *gather, int batch, odtk_stream_t stream);
 
-/* ---- iou (rotated target assignment, SURVEY.md section 8f row 2) ---------------------------
+/* ---- iou (rotated target assignment) ---------------------------
  * Replaces odtk::cuda::iou (csrc/cuda/nms_iou.h:33-35, nms_iou.cu:324-387), the kernel behind
  * odtk._C.iou (csrc/extensions.cpp:47-67,200).
  *   inputs  = { boxes [num_boxes, 4 corners, (x, y)], anchors [num_anchors, 4, 2] }  fp32
@@ -202,8 +202,8 @@ typedef struct {
   void *y;
   int n, h, width, cin, cout, ksize, relu /* 0 none, 1 ReLU, 2 ReLU6 (NHWC fp16 output only) */, out_mode, ldy, ldr;
   int stride;           /* 0/1, or 2: stride-2 conv (pad ksize/2); y is [n, (h-1)/2+1, (width-1)/2+1, ...] */
-  const void *bias_op;  /* optional: bias packed by odtk_conv_pack_bias ([cout, 64] fp16).  When given, the
-                           bias is added by ONE extra K block on the tensor core instead of in the epilogue */
+  const void *bias_op;  /* optional: bias packed by odtk_conv_pack_bias ([cout, 64] fp16).  Accepted for ABI
+                           compatibility and not read: the sm_90a kernel adds the fp32 bias in its epilogue */
   const odtk_cand_sink_t *sink; /* out_mode ODTK_OUT_CANDIDATES: where the candidates go (host struct)       */
   int groups;           /* 0 / 1 dense; > 1: grouped 3x3 (ResNeXt, odtk/backbones/fpn.py:85-91): cin == cout, a group never
                            straddles a 64-channel chunk, w is [cout, 9*64] with the group's weights at the columns of
@@ -219,8 +219,9 @@ typedef struct {
 } odtk_conv_t;
 int odtk_conv2d(const odtk_conv_t *desc, odtk_stream_t stream);
 /* Introspection (tests): the kernel variant the last odtk_conv2d / odtk_stem_conv call of the calling host thread
- * launched.  mode: 0 GEMM rows (1x1), 1 shifted box per tap, 3 stride 2, 4 halo (3x3 s1), 5 raw-window stem;
- * cluster: 0 single CTAs, 1 2-CTA multicast pairs, 2 cta_group::2 pairs.  res_mma: 1 residual tile as one I * R
+ * launched.  mode: 0 GEMM rows (1x1), 1 shifted box per tap (3x3, odd-size stride 2), 2 stem, 3 even-size stride 2;
+ * bn: N tile (64 or 128); grid: persistent CTAs.  cluster, npatch, tile_t, b_resident, bias_mma, res_mma, tma_store and
+ * up_mma are always 0 on sm_90a (kept for ABI stability).  res_mma: 1 residual tile as one I * R
  * product, 2 residual chunks through the pipeline stages (R_j * I64), 0 residual (if any) added in the epilogue.  */
 typedef struct {
   int mode, cluster, bn, num_m_tiles, num_n_tiles, nstages, npatch, tile_t, b_resident, bias_mma, res_mma, tma_store;
@@ -247,8 +248,8 @@ int odtk_peer_free(void *ptr);
 /* Tail of a stride-1 ResNet bottleneck block in ONE kernel (torchvision Bottleneck.forward behind
  * odtk/backbones/resnet.py:24-39; the reference runs it as two cuDNN convolutions + an elementwise add):
  *     y = relu( conv1x1( relu( conv3x3(x, w2) + b2 ), w3 ) + b3 + residual )
- * The [n, h, width, c1] output of the 3x3 never leaves the SM (it is rounded to fp16 exactly as the two-kernel route
- * stores it), and the tensor-bound 3x3 runs under the HBM time of the 1x1 expansion.  c1 in {64, 128}; c2 % 128 == 0,
+ * The [n, h, width, c1] output of the 3x3 never leaves the SM: it is rounded to fp16 exactly as a separate 3x3 launch
+ * stores it and becomes the shared-memory A operand of the 1x1.  c1 in {64, 128}; c2 % 128 == 0,
  * c2 <= 512; x: NHWC fp16 [n, h, width, c1]; w2: fp16 [c1, 9*c1] (tap-major, channel-minor); w3: fp16 [c2, c1];
  * b2 / b3: fp32 or NULL; residual, y: NHWC fp16 [n, h, width, c2]; relu: applied to y.                          */
 typedef struct {
@@ -284,7 +285,7 @@ int odtk_lower_conv(const void *x, void *out, int n, int h, int w, int c, int ks
 int odtk_pad_input(const void *x, void *y, int n, int h, int w, odtk_stream_t stream);
 int odtk_stem_conv(const void *xp, const void *w, const float *bias, void *y, int n, int h, int width,
                    int cout, int relu, odtk_stream_t stream);
-/* Stem + max-pool fused (B200-native): 7x7/2 convolution + bias (folded BatchNorm) + ReLU + 3x3/2 pad-1 max-pool in one
+/* Stem + max-pool fused (H100-native): 7x7/2 convolution + bias (folded BatchNorm) + ReLU + 3x3/2 pad-1 max-pool in one
  * kernel; the [n, h/2, w/2, 64] stem activation is never written.  xp, w as for odtk_stem_conv; cout must be 64;
  * y: NHWC fp16 [n, (h/2 - 1)/2 + 1, (w/2 - 1)/2 + 1, 64].  Bit-identical to odtk_stem_conv followed by
  * odtk_maxpool3x3s2 (the same fp16 values are pooled).                                                        */
@@ -320,12 +321,12 @@ long long odtk_focal_loss(const float *logits, const float *target, const float 
                           size_t workspace_size, odtk_stream_t stream);
 
 /* Smooth L1 (odtk/loss.py:27-31; box loss of Model._compute_loss, odtk/model.py:201-205), same fused
- * forward + backward + masked-sum form as odtk_focal_loss.  SURVEY.md section 8f, row 1.            */
+ * forward + backward + masked-sum form as odtk_focal_loss.                                           */
 long long odtk_smooth_l1_loss(const float *pred, const float *target, const float *mask, long long n,
                               float beta, float grad_scale, float *loss_elem, float *loss_sum, float *grad,
                               void *workspace, size_t workspace_size, odtk_stream_t stream);
 
-/* Model._compute_loss in ONE launch (odtk/model.py:186-210; SURVEY.md section 8f, row 1): over all pyramid levels, focal
+/* Model._compute_loss in ONE launch (odtk/model.py:186-210): over all pyramid levels, focal
  * loss of the class logits against class-index targets with the (depth >= 0) mask, smooth L1 of the box deltas with the
  * (depth > 0) mask, per-level foreground counts clamp(min=1) summed, both losses divided by that sum -- and, when the
  * grad pointers are given, the gradients of the two NORMALISED losses w.r.t. the head outputs.  Deterministic (integer
@@ -343,7 +344,7 @@ long long odtk_retina_loss(int batch, int num_levels, const odtk_loss_level_t *l
                            int nbox, float alpha, float gamma, float beta, float *out, void *workspace,
                            size_t workspace_size, odtk_stream_t stream);
 
-/* ---- anchor target assignment (SURVEY.md section 8f, row 2) --------------------------------------------
+/* ---- anchor target assignment --------------------------------------------
  * Replaces snap_to_anchors (odtk/box.py:134-186) + box2delta (:67-78) as called per image and level by
  * Model._extract_targets (odtk/model.py:167-184), for the whole batch in one launch.
  *   targets [B, G, 5] fp32 device: x, y, w, h, class; rows with class <= -1 are padding (the reference
@@ -353,14 +354,14 @@ long long odtk_retina_loss(int batch, int num_levels, const odtk_loss_level_t *l
  *   cls_target [B, A, C, H, W] dense one-hot, may be NULL;  box_target [B, A, 4, H, W];
  *   depth [B, A, 1, H, W]: -1 ignored (iou_bg <= IoU < iou_fg), 0 background, class + 1 foreground;
  *   cls_index [B, A, H, W] int32, may be NULL: class, -1 background, -2 ignored -- the class-index
- *   target layout odtk_focal_loss consumes (B200-native: the dense one-hot never has to exist).
+ *   target layout odtk_focal_loss consumes (H100-native: the dense one-hot never has to exist).
  * An image without valid rows yields zeros everywhere (odtk/box.py:140-143) and cls_index -1.         */
 int odtk_snap_to_anchors(const float *targets, int batch, int max_boxes, int height, int width, int stride,
                          const float *anchors, int num_anchors, int num_classes, float iou_bg, float iou_fg,
                          float *cls_target, float *box_target, float *depth, int *cls_index,
                          odtk_stream_t stream);
 
-/* ---- input side of `odtk infer` (SURVEY.md section 8f, row 3) ---------------------------------------
+/* ---- input side of `odtk infer` ---------------------------------------
  * Replaces the per-image tensor maths of CocoDataset.__getitem__ (odtk/data.py:113-123): uint8 HWC
  * [n,h,w,3] -> /255 -> (x - mean)/std -> zero padding to [hs, ws] (a multiple of the model stride),
  * written straight into the zero-padded NHWC4 fp16 buffer [n, hs+6, ws+8, 4] that odtk_stem_conv
@@ -368,7 +369,7 @@ int odtk_snap_to_anchors(const float *targets, int batch, int max_boxes, int hei
 int odtk_preprocess_u8(const void *x, void *y, int n, int h, int w, int hs, int ws, const float *mean,
                        const float *std, odtk_stream_t stream);
 
-/* ---- per-kernel timing (B200-native addition; the reference has only a wall-clock
+/* ---- per-kernel timing (H100-native addition; the reference has only a wall-clock
  * Profiler without CUDA sync, odtk/utils.py:140-167) ------------------------------
  * When enabled, every launch of a tagged kernel is bracketed by CUDA events on the
  * launching stream.  Tags: 0 score filter, 1 select+decode, 2 nms, 3 conv, 4 loss / target

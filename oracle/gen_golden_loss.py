@@ -1,4 +1,4 @@
-"""Fixture for the fused training loss (SURVEY.md section 8f row 1): the UNMODIFIED reference Model._compute_loss
+"""Fixture for the fused training loss: the UNMODIFIED reference Model._compute_loss
 (odtk/model.py:186-210: _extract_targets -> snap_to_anchors per image and level, FocalLoss, SmoothL1Loss, masks,
 foreground counts, normalisation) and its autograd gradients w.r.t. the head tensors, on seeded random heads / targets.
     python oracle/gen_golden_loss.py  ->  tests/golden/compute_loss.npz          TEST INFRASTRUCTURE ONLY."""

@@ -1,4 +1,4 @@
-"""Fixtures for the rotated training-side target assignment (SURVEY.md section 8f row 2), made in the build container:
+"""Fixtures for the rotated training-side target assignment, made in the build container:
     python oracle/gen_golden_rotated.py  ->  tests/golden/snap_rotated.npz
 TEST INFRASTRUCTURE ONLY.
 

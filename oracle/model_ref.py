@@ -34,7 +34,7 @@ def _conv(sd, p, x, stride=1, padding=0, groups=1):
 
 # ---- fp16-emulating mode ------------------------------------------------------------------------------------------
 # The product path stores activations and weights in fp16 and accumulates in fp32 (what "fp16" means for the reference
-# too: apex AMP O2 / a TensorRT FP16 engine, SURVEY.md App. B item 10).  With fp16=True this oracle performs the SAME
+# too: apex AMP O2 / a TensorRT FP16 engine).  With fp16=True this oracle performs the SAME
 # roundings -- BatchNorm folded into the weights in fp32, weights rounded to fp16 once, every layer's output (after bias,
 # residual / upsample add and ReLU, all in fp32) rounded to fp16, head outputs kept in fp32 -- so that what remains
 # between it and the CUDA path is fp32 summation order (plus the rare 1-ulp fp16 rounding flip it causes): the conv
@@ -107,8 +107,8 @@ def features(sd, backbone, x, fp16=False):
                 out = _cb(sd, p + "conv2", p + "bn2", out, 1, 1, fp16)
             if (p + "downsample.0.weight") in sd:
                 identity = _cb(sd, p + "downsample.0", p + "downsample.1", x, stride, 0, fp16)
-                # the product path computes the stride-1 projection of layer1's first bottleneck block inside the fused
-                # block kernel (bottleneck.cu) and adds it in fp32; every other projected identity is stored in fp16
+                # the product path computes the stride-1 projection of layer1's first bottleneck block in the fp32
+                # accumulator of the fused block kernel's 1x1 (bottleneck.cu); every other projected identity is stored in fp16
                 if not (block == "bottleneck" and stride == 1 and backbone not in GROUPS):
                     identity = _q(identity, fp16)
             x = _q(F.relu(out + identity), fp16)

@@ -8,7 +8,7 @@
  * Nothing in the product package may import, link or call this file.
  *
  * Each function cites the reference file:line it follows.  Where the
- * reference's CUDA and CPU paths disagree (SURVEY.md App. B) the CUDA
+ * reference's CUDA and CPU paths disagree the CUDA
  * semantics are followed with IEEE arithmetic and stable ordering.
  *
  * Pinning status: decode / nms are pinned by fixtures generated from the

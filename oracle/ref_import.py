@@ -4,7 +4,7 @@ TEST INFRASTRUCTURE ONLY.  Used by oracle/gen_golden.py (fixture generation) and
 not-gpu tests that re-validate the oracle whenever /root/reference is mounted.  It cannot
 travel to the GPU box; nothing under -m gpu, smoke() or bench.py may call it.
 
-Shims (SURVEY.md section 8c): a stub `odtk._C` (the compiled extension is absent) and
+Shims: a stub `odtk._C` (the compiled extension is absent) and
 `torchvision.models.{resnet,mobilenet}.model_urls` (removed in torchvision >= 0.13).
 """
 import collections

@@ -7,7 +7,7 @@
 // /root/reference by oracle/Makefile into oracle/_ref/libodtk_ref.so; no
 // reference source is copied into this repository.  The result is (a) the GPU
 // oracle the -m gpu parity tests pin against and (b) the "reference csrc/cuda
-// plugins recompiled for sm_100a" comparator of BASELINE.json configs[1]/[4].
+// plugins recompiled for sm_90a" comparator of BASELINE.json configs[1]/[4].
 #include <cuda_runtime.h>
 #include <vector>
 #include "decode.h"

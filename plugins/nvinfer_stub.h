@@ -1,5 +1,5 @@
 // nvinfer_stub.h -- the handful of TensorRT types odtk_b200_plugin.h touches, for compile-checking the plugin-shaped
-// wrappers in an image without TensorRT (this one: `import tensorrt` / <NvInfer.h> are absent, SURVEY.md section 2).
+// wrappers in an image without TensorRT (this one: `import tensorrt` / <NvInfer.h> are absent).
 // NOT TensorRT: with the real SDK define ODTK_B200_HAVE_NVINFER and this file is never included.
 #pragma once
 #include <cstddef>

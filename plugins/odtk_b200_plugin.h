@@ -1,10 +1,10 @@
-// odtk_b200_plugin.h -- TensorRT-plugin-shaped wrappers over the C ABI of the B200 hot path (include/odtk_b200.h).
+// odtk_b200_plugin.h -- TensorRT-plugin-shaped wrappers over the C ABI of the H100 hot path (include/odtk_b200.h).
 //
-// SURVEY.md section 8(f) row 4.  The reference's TensorRT plugins are thin shells around odtk::cuda::decode / nms: their
+// The reference's TensorRT plugins are thin shells around odtk::cuda::decode / nms: their
 // configurePlugin() reads the geometry off the input descriptors, getWorkspaceSize() is the size query of the same
 // function, enqueue() is the call itself (csrc/plugins/DecodePlugin.h:141-161,177-191; DecodeRotatePlugin.h; NMSPlugin.h:120-138;
 // NMSRotatePlugin.h).  The C ABI keeps exactly that contract (two-phase workspace, caller-owned buffers, stream
-// argument, no host synchronisation), so a plugin backed by the sm_100a kernels is the same three methods over
+// argument, no host synchronisation), so a plugin backed by the sm_90a kernels is the same three methods over
 // odtk_decode / odtk_decode_rotate / odtk_nms / odtk_nms_rotate.  The classes below are those three methods, with the
 // TensorRT signatures, independent of the TensorRT base class: a maintainer derives
 //     class DecodePlugin : public nvinfer1::IPluginV2DynamicExt, private odtk_b200::DecodeBackend { ... }

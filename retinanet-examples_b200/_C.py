@@ -1,7 +1,7 @@
 """Mirror of the reference's compiled extension module `odtk._C` (csrc/extensions.cpp:184-201):
 `decode`, `nms` with the same signatures, argument meaning, shapes, dtypes and error behaviour
 (RuntimeError on non-CUDA / non-contiguous input, extensions.cpp:42-44), implemented by the
-sm_100a kernels behind the C ABI; `iou` (extensions.cpp:47-67) likewise.  `Engine` (TensorRT) is outside the hot path."""
+sm_90a kernels behind the C ABI; `iou` (extensions.cpp:47-67) likewise.  `Engine` (TensorRT) is outside the hot path."""
 import ctypes
 
 import torch
@@ -62,7 +62,7 @@ def decode(cls_head, box_head, anchors, scale, score_thresh, top_n, rotated=Fals
 
 
 def decode_levels(cls_heads, box_heads, anchors, scales, score_thresh, top_n, rotated=False):
-    """All pyramid levels of the batch in three launches (B200-native addition, see
+    """All pyramid levels of the batch in three launches (H100-native addition, see
     odtk_decode_levels in include/odtk_b200.h).  cls_heads / box_heads: lists of per-level
     tensors as for `decode`; anchors: list of flat per-level lists; scales: per-level strides.
     Returns [scores [B, L*top_n], boxes [B, L*top_n, 4|6], classes [B, L*top_n]] == the torch.cat

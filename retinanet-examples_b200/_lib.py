@@ -9,7 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("ODTK_B200_LIB", os.path.join(_HERE, "libodtk_b200.so"))  # override: A/B builds
 
 ODTK_OK = 0
-_ERRORS = {-1: "invalid argument", -2: "workspace is too small", -3: "size not supported by the sm_100a kernels",
+_ERRORS = {-1: "invalid argument", -2: "workspace is too small", -3: "size not supported by the sm_90a kernels",
            -4: "CUDA runtime error"}
 
 _c_vpp = ctypes.POINTER(ctypes.c_void_p)

@@ -1,6 +1,6 @@
 """Host-side mirror of the reference's odtk/box.py for the inference hot path: anchor tables
 (setup-time, CPU) and the decode / nms / nms_rotated dispatchers, which here ALWAYS run the
-sm_100a kernels (the reference dispatches to odtk._C when torch.cuda.is_available(),
+sm_90a kernels (the reference dispatches to odtk._C when torch.cuda.is_available(),
 odtk/box.py:262,315,373, and otherwise to a CPU fallback -- this package has no fallback)."""
 import math
 
@@ -137,7 +137,7 @@ def snap_to_anchors(boxes, size, stride, anchors, num_classes, device, anchor_io
     return cls_target[0], box_target[0], depth[0]
 
 
-# ---- rotated-box target assignment (SURVEY.md section 8f row 2; reference odtk/box.py:80-96,189-252, odtk/utils.py:33-80) ----
+# ---- rotated-box target assignment (reference odtk/box.py:80-96,189-252, odtk/utils.py:33-80) ----
 def rotate_boxes(boxes, points=False):
     """Target boxes (xmin, ymin, width, height, theta) -> (boxes_axis [G, 6] = (x1, y1, x2, y2, sin, cos),
     boxes_rotated [G, 8] = the four rotated corners ordered tl, tr, br, bl).  Reference: odtk/utils.py:33-80."""
@@ -173,7 +173,7 @@ def box2delta_rotated(boxes, anchors):
 def snap_to_anchors_rotated(boxes, size, stride, anchors, num_classes, device, anchor_ious):
     """'Snap target boxes (x, y, w, h, a) to anchors' -- odtk/box.py:192-252, same signature and results.
     boxes [G, 6] (x, y, w, h, theta, class) of ONE image; anchors = (anchors_axis [A, 4], anchors_rotated [A, 8]) from
-    generate_anchors_rotated; size = [W*stride, H*stride].  The A*H*W x G polygon IoUs run on the sm_100a kernel
+    generate_anchors_rotated; size = [W*stride, H*stride].  The A*H*W x G polygon IoUs run on the sm_90a kernel
     (_C.iou -> odtk_iou); the arg-max / delta / scatter bookkeeping are the reference's own tensor expressions on the
     device.  Returns (cls_target [A, C, H, W], box_target [A, 6, H, W], depth [A, 1, H, W])."""
     anchors_axis, anchors_rotated = anchors

@@ -1,678 +1,290 @@
-// bottleneck.cu -- the tail of a ResNet bottleneck block in ONE kernel (torchvision Bottleneck.forward, stride 1:
-//     y = relu( conv3_1x1( relu( conv2_3x3(x) + b2 ) ) + b3 + identity )        (BatchNorm folded into w / b)
-// used by odtk/backbones/resnet.py:24-39 through layer1 / layer2).  The reference runs conv2 and conv3 as two cuDNN
-// calls; so did this repo (conv.cu modes 4 and 0).  At 800 x 1280 the 1x1 expansion is HBM-bound (it reads the identity
-// and writes the block output, 4 x C1 channels each) while the 3x3 in front of it is tensor-bound: fused, the 3x3 runs
-// UNDER the expansion's memory time and its [N, H, W, C1] output never touches HBM.
+// bottleneck.cu -- the tail of a stride-1 ResNet bottleneck block in ONE kernel on the Hopper tensor cores (sm_90a):
 //
-//   tile      8 rows x 16 columns of pixels per CTA (accumulator row m -> (m % 8, m / 8)), CTA PAIRS (cta_group::2, M = 256)
-//   GEMM1     3x3: the halo patch [18 columns][10-row pitch][64 ch] of a 64-channel chunk is loaded once (one 4-D TMA box,
-//             hardware zero fill == padding); the nine taps are nine shifted SWIZZLE_128B views of it (as conv.cu mode 4).
-//             Accumulator acc1[2] (C1 <= 128 TMEM columns each).
-//   ep1       epilogue warps: acc1 + b2 -> ReLU -> fp16 -> shared memory, written directly in the K-major SWIZZLE_128B
-//             layout of a UMMA A operand ("y1").
-//   GEMM2     1x1: for every 128-channel output tile n2: acc2[n2 & 1] = y1 * W3[n2]^T.
-//   GEMM3     (optional, C1 = 64) the NEXT block's conv1: z = relu(y * W1n^T + b1n) -- the block output chunks the epilogue
-//             has just written in place in the identity slots are already A operands; issued one tile late, behind the next
-//             tile's 3x3, into a third accumulator (columns 128 .. 255); removes the widest read of the next block.
-//   ep2       the identity chunks [128 px x 64 ch] arrive by TMA (4-D box straight from the NHWC tensor, 128B-swizzled rows
-//             = pixels) in a ring of 16 KB slots; each epilogue thread adds ITS pixel's 128 bytes to acc2 + b3, applies
-//             ReLU and writes the fp16 result back IN PLACE; the slot's 4 KB quarter of the warp is then the source of a
-//             cp.async.bulk.tensor store (4-D box, edges clipped by the TMA unit).  No staging slabs, no extra pass.
+//     mid = relu(conv3x3(x, W2) + b2)                       GEMM1: 9 * C1/64 K blocks, A = shifted TMA boxes of x
+//     y   = act(mid * W3^T + b3 + identity)                  GEMM2: per 128-channel output tile, A = mid from shared memory
+//     z   = relu(y * Wn^T + bn)          (optional)          GEMM3: the next block's conv1, A = y from shared memory
 //
-//   warp 0 TMA producer (patches + weights), warp 3 TMA producer of the identity chunks (the HBM stream that bounds the
-//   kernel: its own ring, never blocked behind a weight slot), warp 1 MMA issuer (leader CTA of the pair), warp 2 TMEM
-//   allocator + bias loader, warps 4-11 epilogue.  The issue order is software-pipelined, G1(t+1) before G2(t): the tensor
-//   pipe works on the next tile's 3x3 while the epilogue turns acc1(t) into y1(t).  C1 = 64: both weight matrices stay
-//   resident in shared memory (52 KB per CTA); C1 = 128: they stream through a ring of 8 KB blocks (L2 hits).
-//   The halo patch keeps only the 8 + 2 pixel rows a tile reads (10-slot pitch, 8-row-group stride 1280 B: the 128-byte
-//   swizzle follows the absolute shared-memory address for the TMA write and the UMMA read alike).
+// identity is the residual tensor, or -- first block of layer1 -- xproj * Wproj^T, one more K block of GEMM2's
+// accumulator.  `mid` never leaves the SM: GEMM1's epilogue rounds it to fp16 (exactly what a separate 3x3 launch would
+// store) and writes it into shared memory in the 128-byte-swizzled K-major layout of a wgmma A operand; GEMM2 reads it
+// from there.  GEMM3 reads the fp16 block output the same way instead of re-loading it from HBM.
+//
+//   warpgroup 0     TMA producer (one thread): x boxes + W2 blocks, then W3 (+ xproj / Wproj) blocks per output tile,
+//                   then Wn blocks, through one ring of full / empty mbarrier stages -- in the order the consumers use them.
+//   warpgroups 1-2  64 pixels of the 128-pixel tile each: wgmma.mma_async, fp32 accumulators in registers, epilogues.
+//                   Every A row a warpgroup reads from shared memory it wrote itself, so a 128-thread named barrier
+//                   (plus fence.proxy.async: generic-proxy stores -> async-proxy wgmma reads) is the only hand-over.
 #include <cuda.h>
 #include <cuda_fp16.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include <mutex>
 
 #include "common.cuh"
+#include "conv.cuh"
 #include "prof.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 128 + 32 * kEpiWarps;
-constexpr int kNPatch = 2;
-constexpr int kRSlot = 16384;                  // identity chunk: 128 pixels x 64 channels
-constexpr int kMaxRSlots = 6;
-constexpr int kWSlot = 8192;                   // streamed weight block: this CTA's 64 rows x 64 K
-constexpr int kMaxWSlots = 8;
-constexpr int kBiasBytes = 3072;               // b2 (<= 128 fp32) + b3 (<= 512 fp32) + b_next (<= 128 fp32)
-constexpr int kBarBytes = 512;
-constexpr int kTmemCols = 512;
-constexpr int kSmemMax = 232448;               // 227 KB
-
-// Optional in-kernel wait profile (build with -DODTK_BT_PROF, tools only): cycles each role of CTA 0 spends in its waits.
-#ifdef ODTK_BT_PROF
-__device__ unsigned long long g_bt_prof[32];
-#define BT_WAIT(cat, bar, par) do { const long long t0_ = clock64(); mbar_wait(bar, par); if (blockIdx.x == 0 && lane == 0) atomicAdd(&g_bt_prof[cat], (unsigned long long)(clock64() - t0_)); } while (0)
-#define BT_T0(name) const long long name = clock64()
-#define BT_ADD(cat, name) do { if (blockIdx.x == 0 && lane == 0 && warp == 4) atomicAdd(&g_bt_prof[cat], (unsigned long long)(clock64() - name)); } while (0)
-#define BT_TOTAL_BEGIN() const long long tt0_ = clock64()
-#define BT_TOTAL_END(cat) do { if (blockIdx.x == 0 && lane == 0) atomicAdd(&g_bt_prof[cat], (unsigned long long)(clock64() - tt0_)); } while (0)
-#else
-#define BT_WAIT(cat, bar, par) mbar_wait(bar, par)
-#define BT_T0(name)
-#define BT_ADD(cat, name)
-#define BT_TOTAL_BEGIN()
-#define BT_TOTAL_END(cat)
-#endif
-
-struct BtBars {
-  uint64_t pfull[kNPatch], pempty[kNPatch];
-  uint64_t wfull[kMaxWSlots], wempty[kMaxWSlots];
-  uint64_t rfull[kMaxRSlots], rempty[kMaxRSlots];
-  uint64_t acc1_full[2], acc1_empty[2];
-  uint64_t acc2_full[2], acc2_empty[2];
-  uint64_t y1_full[2], y1_empty[2], wres_full;
-  uint64_t xfull[2], xempty[2];
-  uint64_t ycf[kMaxRSlots];              // GEMM3: the block output chunk in this slot is written (8 epilogue warps of the pair)
-  uint64_t acc3_full, acc3_empty;          // projection mode: the block input tile (A operand of the identity GEMM)
-  uint32_t tmem_base;
-};
-static_assert(sizeof(BtBars) <= kBarBytes, "barrier block too small");
+constexpr int kThreads = 384;
+constexpr int kStageBytes = 2 * 16384;   // A: 128 rows x 128 B; B: up to 128 rows x 128 B
+constexpr int kMaxStages = 6;
+constexpr int kSmemLimit = 227 * 1024;
+constexpr int kChunk = 16384;            // one 64-channel chunk of a [128 pixels][C] operand in shared memory
 
 struct BtParams {
-  int N, H, W, C1, C2;
-  int tiles_h, tiles_w, total_tiles;
-  int ppitch;            // pixel slots per patch column: 16, or 10 (only the 8 + 2 rows a tile reads)
-  int patch_slot;        // bytes between patch buffers (1024-aligned)
-  int w_resident;        // C1 == 64: W2 / W3 halves stay in shared memory (52 KB); else they stream through the weight ring
-  int nw, nr;            // weight / identity ring depths
-  int relu;
-  int g3_late;           // issue GEMM3(t) behind G1(t+2) instead of right behind G2(t)
-  int n3;                // > 0: GEMM3 -- the NEXT block's 1x1 conv1 (C2 -> n3 channels, + bias + ReLU) computed from the block
-                         // output while its chunks still sit in the identity slots; z: [N, H, W, n3]
-  __half *z;
-  const float *b_next;
-  int proj;              // identity = 1x1 projection of a 64-channel block input, computed here (first block of layer1)
-  const float *b2, *b3;
+  int N, H, W, C2, TH, TW, tiles_h, tiles_w, total_tiles, nstages, relu, proj;
+  int mid_off, ysm_off;                  // byte offsets of the mid / block-output operands in shared memory
+  const float *b2, *b3, *bn;
+  const __half *residual;
+  __half *y, *z;
 };
 
-// halo view (conv.cu make_desc_halo): 8-row groups (8 consecutive pixels of a patch column) `sbo` bytes apart
-__device__ __forceinline__ uint64_t bt_desc_halo(uint32_t saddr, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+struct Ring {
+  int stage = 0;
+  uint32_t phase = 0;
+  int n;
+  __device__ void next() { if (++stage == n) { stage = 0; phase ^= 1u; } }
+};
+
+__device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void sts32(uint32_t saddr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory"); }
+// (row, col) of a [128][64 k] 128B-swizzled K-major chunk: the 16-byte unit (col / 8) is XOR-ed with row % 8
+__device__ __forceinline__ uint32_t swz_off(int row, int col) {
+  return (uint32_t)(row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2);
+}
+__device__ __forceinline__ uint32_t h2u(__half2 h) { return *reinterpret_cast<uint32_t *>(&h); }
+
+template <int N>
+__device__ __forceinline__ void mma_block(float (&acc)[N / 2], uint64_t da, uint64_t db, bool first) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; k++) Wgmma<N>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (first && k == 0) ? 0 : 1);
+  wgmma_commit();
 }
 
+template <int C1, int N3>
 __global__ void __launch_bounds__(kThreads, 1)
 bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW2,
-                       const __grid_constant__ CUtensorMap tmW3, const __grid_constant__ CUtensorMap tmR,
-                       const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmWd,
-                       const __grid_constant__ CUtensorMap tmW1,
+                       const __grid_constant__ CUtensorMap tmW3, const __grid_constant__ CUtensorMap tmXp,
+                       const __grid_constant__ CUtensorMap tmWp, const __grid_constant__ CUtensorMap tmWn,
                        const __grid_constant__ BtParams p) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  // layout (every region 1024-aligned): patches | weights (resident, or ring) | identity ring | y1 | bias | barriers
-  const int kc1 = p.C1 >> 6;                         // 64-channel chunks of the 3x3's input == of y1
-  const int n2tiles = p.C2 >> 7;
-  const uint32_t w2_block = (uint32_t)(p.C1 >> 1) * 128u;    // this CTA's half of the rows of one W2 block (tap, chunk)
-  const int nb1 = 9 * kc1;                           // W2 blocks per tile, linear index b = chunk * 9 + tap
-  unsigned char *spatch = smem;
-  unsigned char *sw = spatch + kNPatch * p.patch_slot;
-  const uint32_t w_bytes = p.w_resident ? (uint32_t)nb1 * w2_block + (uint32_t)(n2tiles * kc1) * kWSlot + (p.proj ? (uint32_t)n2tiles * kWSlot : 0u) + (uint32_t)(2 * n2tiles) * (uint32_t)(p.n3 >> 1) * 128u
-                                        : (uint32_t)p.nw * kWSlot;
-  const uint32_t w1_off = (uint32_t)nb1 * w2_block + (uint32_t)(n2tiles * kc1) * kWSlot + (p.proj ? (uint32_t)n2tiles * kWSlot : 0u);   // resident W1n blocks
-  unsigned char *sres = sw + w_bytes;
-  unsigned char *sx = sres + p.nr * kRSlot;          // projection mode: 2 slots for the block-input tile
-  unsigned char *sy1 = sx + (p.proj ? 2 * kRSlot : 0);
-  float *sbias = reinterpret_cast<float *>(sy1 + 2 * kc1 * 16384);    // y1 is double-buffered: ep1(t+1) does not wait for GEMM2(t)
-  BtBars *bars = reinterpret_cast<BtBars *>(reinterpret_cast<unsigned char *>(sbias) + kBiasBytes);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-  const int crank = (int)cluster_ctarank();
-  const uint32_t patch_bytes = 18u * (uint32_t)p.ppitch * 128u;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmX) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW2) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW3) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmR) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmY) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kNPatch; s++) { mbar_init(&bars->pfull[s], 1); mbar_init(&bars->pempty[s], 1); }
-    for (int s = 0; s < kMaxWSlots; s++) { mbar_init(&bars->wfull[s], 1); mbar_init(&bars->wempty[s], 1); }
-    for (int s = 0; s < kMaxRSlots; s++) { mbar_init(&bars->rfull[s], 1); mbar_init(&bars->rempty[s], p.n3 ? 5 : 4); mbar_init(&bars->ycf[s], 2 * 4); }
-    mbar_init(&bars->acc3_full, 1); mbar_init(&bars->acc3_empty, 2 * kEpiWarps);   // a slot is consumed by the 4 epilogue warps of one column half
-    for (int b = 0; b < 2; b++) {
-      mbar_init(&bars->acc1_full[b], 1); mbar_init(&bars->acc1_empty[b], 2 * kEpiWarps);   // one arrival per epilogue warp of the pair
-      mbar_init(&bars->acc2_full[b], 1); mbar_init(&bars->acc2_empty[b], 2 * kEpiWarps);
-      mbar_init(&bars->y1_full[b], 2 * kEpiWarps); mbar_init(&bars->y1_empty[b], 1);
-    }
-    mbar_init(&bars->wres_full, 1);
-    for (int s = 0; s < 2; s++) { mbar_init(&bars->xfull[s], 1); mbar_init(&bars->xempty[s], 1); }
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + p.ysm_off + (N3 ? (p.C2 / 64) * kChunk : 0));
+  uint64_t *empty = full + kMaxStages;
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0), tid = threadIdx.x & 127;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < p.nstages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8 /* one per consumer warp */); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-    for (int i = lane; i < p.C1; i += 32) sbias[i] = p.b2 ? p.b2[i] : 0.0f;
-    for (int i = lane; i < p.C2; i += 32) sbias[128 + i] = p.b3 ? p.b3[i] : 0.0f;
-    for (int i = lane; i < p.n3; i += 32) sbias[640 + i] = p.b_next ? p.b_next[i] : 0.0f;
-  }
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
+  __syncthreads();
   grid_dep_launch_dependents();
-  grid_dep_wait();                // (the prologue above touched only constants: weights' descriptors, biases)
-  const uint32_t tmem_base = bars->tmem_base;
-
-  // work: pairs of consecutive tiles; the pair's second tile may be padding (odd total): computed, never stored
-  const int npairs = (p.total_tiles + 1) >> 1;
-  const int c_first = (int)(blockIdx.x >> 1), c_step = (int)(gridDim.x >> 1);
-  const int per_img = p.tiles_h * p.tiles_w;
-  auto tile_of = [&](int pair, int &img, int &h0, int &w0) -> bool {
-    int t = 2 * pair + crank;
-    const bool real = t < p.total_tiles;
-    if (!real) t = p.total_tiles - 1;
-    img = t / per_img;
-    const int rr = t - img * per_img;
-    h0 = (rr / p.tiles_w) * 8;
-    w0 = (rr % p.tiles_w) * 16;
-    return real;
+  grid_dep_wait();
+  constexpr int KC1 = C1 / 64;
+  const int n2tiles = p.C2 / 128, per_img = p.tiles_h * p.tiles_w;
+  auto origin = [&](int tile, int &img, int &h0, int &w0) {
+    img = tile / per_img;
+    const int r = tile - img * per_img;
+    h0 = (r / p.tiles_w) * p.TH;
+    w0 = (r % p.tiles_w) * p.TW;
   };
 
-  if (warp == 0) {
-    // ============================ TMA producer: patches + weights ============================
-    int ws = 0, pb = 0;
-    uint32_t wph = 0, pphase = 0;
-    if (p.w_resident && elect_one()) {
-      const uint32_t lbar = mapa_rank(smem_u32(&bars->wres_full), 0);
-      if (crank == 0) mbar_arrive_expect_tx(&bars->wres_full, 2u * w_bytes);
-      for (int i = 0; i < nb1; i++) {
-        const int kc = i / 9, tap = i - 9 * kc;
-        tma2_load_2d(sw + i * w2_block, &tmW2, lbar, tap * p.C1 + kc * 64, crank * (p.C1 >> 1));
-      }
-      for (int n2 = 0; n2 < n2tiles; n2++)
-        for (int kc = 0; kc < kc1; kc++)
-          tma2_load_2d(sw + nb1 * w2_block + (n2 * kc1 + kc) * kWSlot, &tmW3, lbar, kc * 64, n2 * 128 + crank * 64);
-      if (p.proj)
-        for (int n2 = 0; n2 < n2tiles; n2++)
-          tma2_load_2d(sw + nb1 * w2_block + (n2tiles * kc1 + n2) * kWSlot, &tmWd, lbar, 0, n2 * 128 + crank * 64);
-      if (p.n3)   // next block's conv1: [n3, C2], this CTA's half of the rows, one 64-channel K block per output chunk
-        for (int c = 0; c < 2 * n2tiles; c++)
-          tma2_load_2d(sw + w1_off + c * ((p.n3 >> 1) * 128), &tmW1, lbar, c * 64, crank * (p.n3 >> 1));
-    }
-    auto produce_g1 = [&](int pair) {
+  if (wg == 0) {
+    // ===================================== TMA producer =====================================
+    if (tid != 0) return;
+    Ring ring;
+    ring.n = p.nstages;
+    const uint32_t a_bytes = (uint32_t)(p.TH * p.TW * 128);
+    auto slot = [&](uint32_t bytes) -> unsigned char * {
+      mbar_wait(&empty[ring.stage], ring.phase ^ 1u);
+      mbar_arrive_expect_tx(&full[ring.stage], bytes);
+      return smem + ring.stage * kStageBytes;
+    };
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       int img, h0, w0;
-      tile_of(pair, img, h0, w0);
-      for (int kc = 0; kc < kc1; kc++) {
-        BT_WAIT(7, &bars->pempty[pb], pphase ^ 1u);
-        if (elect_one()) {
-          if (crank == 0) mbar_arrive_expect_tx(&bars->pfull[pb], 2u * patch_bytes);
-          tma2_load_4d(spatch + pb * p.patch_slot, &tmX, mapa_rank(smem_u32(&bars->pfull[pb]), 0), kc * 64, h0 - 1, w0 - 1, img);
-        }
-        if (++pb == kNPatch) { pb = 0; pphase ^= 1u; }
-        if (p.w_resident) continue;
+      origin(tile, img, h0, w0);
+      for (int kb = 0; kb < KC1; kb++)
         for (int tap = 0; tap < 9; tap++) {
-          BT_WAIT(8, &bars->wempty[ws], wph ^ 1u);
-          if (elect_one()) {
-            if (crank == 0) mbar_arrive_expect_tx(&bars->wfull[ws], 2u * w2_block);
-            tma2_load_2d(sw + ws * kWSlot, &tmW2, mapa_rank(smem_u32(&bars->wfull[ws]), 0), tap * p.C1 + kc * 64, crank * (p.C1 >> 1));
-          }
-          if (++ws == p.nw) { ws = 0; wph ^= 1u; }
+          unsigned char *s = slot(a_bytes + C1 * 128);
+          tma_load_4d(s, &tmX, &full[ring.stage], kb * 64, w0 + tap % 3 - 1, h0 + tap / 3 - 1, img);
+          tma_load_2d(s + 16384, &tmW2, &full[ring.stage], (tap * KC1 + kb) * 64, 0);
+          ring.next();
         }
-      }
-    };
-    auto produce_g2 = [&]() {
-      if (p.w_resident) return;
-      for (int n2 = 0; n2 < n2tiles; n2++)
-        for (int kc = 0; kc < kc1; kc++) {
-          BT_WAIT(8, &bars->wempty[ws], wph ^ 1u);
-          if (elect_one()) {
-            if (crank == 0) mbar_arrive_expect_tx(&bars->wfull[ws], 2u * (uint32_t)kWSlot);
-            tma2_load_2d(sw + ws * kWSlot, &tmW3, mapa_rank(smem_u32(&bars->wfull[ws]), 0), kc * 64, n2 * 128 + crank * 64);
-          }
-          if (++ws == p.nw) { ws = 0; wph ^= 1u; }
+      for (int n2 = 0; n2 < n2tiles; n2++) {
+        for (int kb = 0; kb < KC1; kb++) {
+          unsigned char *s = slot(128 * 128);
+          tma_load_2d(s + 16384, &tmW3, &full[ring.stage], kb * 64, n2 * 128);
+          ring.next();
         }
-    };
-    BT_TOTAL_BEGIN();
-    if (c_first < npairs) produce_g1(c_first);
-    for (int pair = c_first; pair < npairs; pair += c_step) {
-      if (pair + c_step < npairs) produce_g1(pair + c_step);
-      produce_g2();
-    }
-    BT_TOTAL_END(9);
-  } else if (warp == 3) {
-    // ============================ TMA producer: the identity stream (HBM) ============================
-    int rs = 0;
-    uint32_t rph = 0;
-    BT_TOTAL_BEGIN();
-    int xs = 0;
-    uint32_t xph = 0;
-    for (int pair = c_first; pair < npairs; pair += c_step) {
-      int img, h0, w0;
-      tile_of(pair, img, h0, w0);
-      if (p.proj) {                                  // one 64-channel tile of the block input per tile (pair protocol: the MMA reads both CTAs')
-        mbar_wait(&bars->xempty[xs], xph ^ 1u);
-        if (elect_one()) {
-          if (crank == 0) mbar_arrive_expect_tx(&bars->xfull[xs], 2u * (uint32_t)kRSlot);
-          tma2_load_4d(sx + xs * kRSlot, &tmR, mapa_rank(smem_u32(&bars->xfull[xs]), 0), 0, h0, w0, img);
-        }
-        if (++xs == 2) { xs = 0; xph ^= 1u; }
-        continue;
-      }
-      for (int c = 0; c < 2 * n2tiles; c++) {
-        BT_WAIT(10, &bars->rempty[rs], rph ^ 1u);
-        if (elect_one()) {                            // this CTA's own barrier: the two identity streams of a pair are independent
-          mbar_arrive_expect_tx(&bars->rfull[rs], (uint32_t)kRSlot);
-          tma_load_4d(sres + rs * kRSlot, &tmR, &bars->rfull[rs], c * 64, h0, w0, img);
-        }
-        if (++rs == p.nr) { rs = 0; rph ^= 1u; }
-      }
-    }
-    BT_TOTAL_END(11);
-  } else if (warp == 1) {
-    // ===================================== MMA issuer (leader CTA) ===========================
-    if (crank == 0) {
-      const uint32_t idesc1 = (1u << 4) | ((uint32_t)(p.C1 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      const uint32_t idesc2 = (1u << 4) | ((uint32_t)(128 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-      const uint32_t w_s = smem_u32(sw), patch_s = smem_u32(spatch), y1_s = smem_u32(sy1);
-      const uint32_t sbo = (uint32_t)p.ppitch * 128u;
-      int ws = 0, pb = 0;
-      uint32_t wph = 0, pphase = 0;
-      int it1 = 0, it2 = 0, u2 = 0;                  // G1 / G2 invocation counters, acc2 use counter
-      int xs = 0;
-      uint32_t xph = 0;
-      const uint32_t x_s = smem_u32(sx), res_s3 = smem_u32(sres);
-      if (p.w_resident) mbar_wait(&bars->wres_full, 0);
-      tc_fence_after();
-      auto issue_g1 = [&]() {
-        const int buf = it1 & 1;
-        BT_WAIT(0, &bars->acc1_empty[buf], ((uint32_t)(it1 >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * p.C1);   // acc1[2] at columns 0 / C1 (C1 = 64: columns 128 .. 255 stay free for GEMM3's accumulator)
-        for (int kc = 0; kc < kc1; kc++) {
-          BT_WAIT(1, &bars->pfull[pb], pphase);
-          tc_fence_after();
-          const uint32_t pbase = patch_s + (uint32_t)(pb * p.patch_slot);
-          for (int tap = 0; tap < 9; tap++) {
-            uint32_t wb;
-            if (p.w_resident) wb = w_s + (uint32_t)(kc * 9 + tap) * w2_block;
-            else {
-              BT_WAIT(2, &bars->wfull[ws], wph);
-              tc_fence_after();
-              wb = w_s + (uint32_t)(ws * kWSlot);
-            }
-            const int r = tap / 3, s3 = tap - 3 * r;
-            const uint64_t da = bt_desc_halo(pbase + (uint32_t)(s3 * p.ppitch + r) * 128u, sbo);
-            const uint64_t db = make_desc_kmajor(wb, 128);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 4; k++) tc_mma2_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc1, (kc | tap | k) ? 1u : 0u);
-              if (!p.w_resident) tc_commit2_mc(&bars->wempty[ws], (uint16_t)3);
-              if (tap == 8) tc_commit2_mc(&bars->pempty[pb], (uint16_t)3);
-            }
-            if (!p.w_resident) { if (++ws == p.nw) { ws = 0; wph ^= 1u; } }
-          }
-          if (++pb == kNPatch) { pb = 0; pphase ^= 1u; }
-        }
-        if (elect_one()) tc_commit2_mc(&bars->acc1_full[buf], (uint16_t)3);
-        it1++;
-      };
-      auto issue_g2 = [&]() {
-        const int yb = it2 & 1;
-        BT_WAIT(3, &bars->y1_full[yb], (uint32_t)(it2 >> 1) & 1u);
-        if (p.proj) mbar_wait(&bars->xfull[xs], xph);
-        tc_fence_after();
-        for (int n2 = 0; n2 < n2tiles; n2++, u2++) {
-          const int buf = u2 & 1;
-          BT_WAIT(4, &bars->acc2_empty[buf], ((uint32_t)(u2 >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + 256u + (uint32_t)(buf * 128);
-          for (int kc = 0; kc < kc1; kc++) {
-            uint32_t wb;
-            if (p.w_resident) wb = w_s + (uint32_t)nb1 * w2_block + (uint32_t)(n2 * kc1 + kc) * kWSlot;
-            else {
-              BT_WAIT(2, &bars->wfull[ws], wph);
-              tc_fence_after();
-              wb = w_s + (uint32_t)(ws * kWSlot);
-            }
-            const uint64_t da = make_desc_kmajor(y1_s + (uint32_t)(yb * kc1 + kc) * 16384u, 128);
-            const uint64_t db = make_desc_kmajor(wb, 128);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 4; k++) tc_mma2_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc2, (kc | k) ? 1u : 0u);
-              if (!p.w_resident) tc_commit2_mc(&bars->wempty[ws], (uint16_t)3);
-            }
-            if (!p.w_resident) { if (++ws == p.nw) { ws = 0; wph ^= 1u; } }
-          }
-          if (p.proj && elect_one()) {               // + identity: block-input tile x Wd[n2]^T into the same accumulator
-            const uint64_t da = make_desc_kmajor(x_s + (uint32_t)(xs * kRSlot), 128);
-            const uint64_t db = make_desc_kmajor(w_s + (uint32_t)nb1 * w2_block + (uint32_t)(n2tiles * kc1 + n2) * kWSlot, 128);
-#pragma unroll
-            for (int k = 0; k < 4; k++) tc_mma2_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc2, 1u);
-          }
-          if (elect_one()) tc_commit2_mc(&bars->acc2_full[buf], (uint16_t)3);
-        }
-        if (elect_one()) tc_commit2_mc(&bars->y1_empty[yb], (uint16_t)3);
         if (p.proj) {
-          if (elect_one()) tc_commit2_mc(&bars->xempty[xs], (uint16_t)3);
-          if (++xs == 2) { xs = 0; xph ^= 1u; }
+          unsigned char *s = slot(a_bytes + 128 * 128);
+          tma_load_4d(s, &tmXp, &full[ring.stage], 0, w0, h0, img);
+          tma_load_2d(s + 16384, &tmWp, &full[ring.stage], 0, n2 * 128);
+          ring.next();
         }
-        it2++;
-      };
-      BT_TOTAL_BEGIN();
-      int it3 = 0;
-      auto issue_g3 = [&]() {
-          // GEMM3: z = y * W1n^T over the block output chunks the epilogue has just written in place into the identity
-          // slots (K-major, 128-byte swizzle: already an A operand); a slot goes back to its producer when these MMAs AND
-          // the chunk's bulk stores have read it
-          const uint32_t idesc3 = (1u << 4) | ((uint32_t)(p.n3 >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-          mbar_wait(&bars->acc3_empty, ((uint32_t)it3 & 1u) ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_z = tmem_base + 128u;
-          for (int c = 0; c < 2 * n2tiles; c++) {
-            const int cidx = 2 * n2tiles * it3 + c, slot = cidx % p.nr;
-            mbar_wait(&bars->ycf[slot], (uint32_t)(cidx / p.nr) & 1u);
-            tc_fence_after();
-            if (elect_one()) {
-              const uint64_t da = make_desc_kmajor(res_s3 + (uint32_t)(slot * kRSlot), 128);
-              const uint64_t db = make_desc_kmajor(w_s + w1_off + (uint32_t)c * (uint32_t)((p.n3 >> 1) * 128), 128);
-#pragma unroll
-              for (int k = 0; k < 4; k++) tc_mma2_f16(tmem_z, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc3, (c | k) ? 1u : 0u);
-              tc_commit2_mc(&bars->rempty[slot], (uint16_t)3);
-            }
-          }
-          if (elect_one()) tc_commit2_mc(&bars->acc3_full, (uint16_t)3);
-        it3++;
-      };
-      // order on the tensor pipe: G1(t+1), [G3(t-1)], G2(t): GEMM3 of a tile is issued one step late (g3_late), behind the
-      // next tile's 3x3, so that the pipe has work while the epilogue writes the block output the GEMM3 reads
-      if (c_first < npairs) issue_g1();
-      bool g3_pending = false;
-      for (int pair = c_first; pair < npairs; pair += c_step) {
-        if (pair + c_step < npairs) issue_g1();
-        if (g3_pending) { issue_g3(); g3_pending = false; }
-        issue_g2();
-        if (p.n3) { if (p.g3_late) g3_pending = true; else issue_g3(); }
       }
-      if (g3_pending) issue_g3();
-      BT_TOTAL_END(6);
+      if (N3)
+        for (int kb = 0; kb < p.C2 / 64; kb++) {
+          unsigned char *s = slot(N3 * 128);
+          tma_load_2d(s + 16384, &tmWn, &full[ring.stage], kb * 64, 0);
+          ring.next();
+        }
     }
-  } else if (warp >= 4) {
-    // ===================================== epilogue ==========================================
-    const int q = warp & 3, sg = (warp - 4) >> 2;
-    const int row = q * 32 + lane;                   // accumulator row == pixel (row % 8, row / 8) of the tile
-    const uint32_t y1_s = smem_u32(sy1), sb_s = smem_u32(sbias);
-    const uint32_t lbar_acc1e0 = mapa_rank(smem_u32(&bars->acc1_empty[0]), 0), lbar_acc1e1 = mapa_rank(smem_u32(&bars->acc1_empty[1]), 0);
-    const uint32_t lbar_acc2e0 = mapa_rank(smem_u32(&bars->acc2_empty[0]), 0), lbar_acc2e1 = mapa_rank(smem_u32(&bars->acc2_empty[1]), 0);
-    const uint32_t lbar_y1f0 = mapa_rank(smem_u32(&bars->y1_full[0]), 0), lbar_y1f1 = mapa_rank(smem_u32(&bars->y1_full[1]), 0);
-    const int cols1 = p.C1 >> 1;                     // columns of acc1 this warp converts: [sg * cols1, +cols1)
-    // ---- ep1: acc1 + b2 -> ReLU -> fp16 -> y1 (K-major, 128-byte swizzle: the A operand of GEMM2) ----
-    auto ep1 = [&](int it) {
-      const int buf = it & 1;
-      BT_WAIT(12, &bars->acc1_full[buf], (uint32_t)(it >> 1) & 1u);
-      BT_WAIT(13, &bars->y1_empty[buf], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * p.C1 + sg * cols1);
-      const uint32_t yrow = y1_s + (uint32_t)(buf * kc1) * 16384u + (uint32_t)((row >> 3) * 1024 + (row & 7) * 128);
-      uint32_t v[2][16];
-      const int nch = cols1 >> 4;                    // 16-column chunks: 2 (C1 = 64) or 4 (C1 = 128)
-      tc_ld16(taddr, v[0]);
-#pragma unroll
-      for (int cc = 0; cc < 4; cc++) {
-        if (cc < nch) {
-          tc_ld_wait();
-          if (cc + 1 < nch) tc_ld16(taddr + (uint32_t)((cc + 1) * 16), v[(cc + 1) & 1]);
-          const int col0 = sg * cols1 + cc * 16;     // first of the 16 channels of this chunk
-          float f[16];
-#pragma unroll
-          for (int j4 = 0; j4 < 4; j4++) {
-            const float4 b = lds128f(sb_s + (uint32_t)((col0 + j4 * 4) * 4));
-            f[4 * j4] = __uint_as_float(v[cc & 1][4 * j4]) + b.x;
-            f[4 * j4 + 1] = __uint_as_float(v[cc & 1][4 * j4 + 1]) + b.y;
-            f[4 * j4 + 2] = __uint_as_float(v[cc & 1][4 * j4 + 2]) + b.z;
-            f[4 * j4 + 3] = __uint_as_float(v[cc & 1][4 * j4 + 3]) + b.w;
-          }
-          uint4 o0, o1;
-          __half2 *q0 = reinterpret_cast<__half2 *>(&o0), *q1 = reinterpret_cast<__half2 *>(&o1);
-          const __half2 z = __float2half2_rn(0.0f);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            q0[j] = __hmax2(__floats2half2_rn(f[2 * j], f[2 * j + 1]), z);
-            q1[j] = __hmax2(__floats2half2_rn(f[8 + 2 * j], f[8 + 2 * j + 1]), z);
-          }
-          const int kc = col0 >> 6, unit = (col0 & 63) >> 3;
-          const uint32_t base = yrow + (uint32_t)kc * 16384u;
-          sts128(base + (uint32_t)(((unit) ^ (row & 7)) << 4), o0);
-          sts128(base + (uint32_t)(((unit + 1) ^ (row & 7)) << 4), o1);
-        }
-      }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy writes -> visible to the tensor core
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {                               // ONE arrival per warp: 512 remote arrivals per barrier serialise on it
-        mbar_arrive_remote(buf ? lbar_acc1e1 : lbar_acc1e0);
-        mbar_arrive_remote(buf ? lbar_y1f1 : lbar_y1f0);
-      }
-    };
-    int u2 = 0;
-    int held = -1;                                   // identity slot this warp's last bulk store still reads from
-    const uint32_t res_s = smem_u32(sres);
-    // ---- ep2: per 128-channel output tile: acc2 + b3 + identity -> ReLU -> fp16, in place in the identity slot -> store ----
-    auto ep2 = [&](int pair) {
-      int img, h0, w0;
-      const bool real = tile_of(pair, img, h0, w0);
-      for (int n2 = 0; n2 < n2tiles; n2++, u2++) {
-        const int buf = u2 & 1;
-        const int cidx = 2 * u2 + sg;                // running index of the identity chunk this warp consumes
-        const int slot = cidx % p.nr;
-        BT_T0(ta_);
-        if (held >= 0) {                             // hand the previous slot back once its store has read it
-          if (lane == 0) {
-            asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            if (!p.proj) mbar_arrive(&bars->rempty[held]);   // (projection mode: the slots are this warp's private staging)
-          }
-          held = -1;
-        }
-        BT_ADD(17, ta_);
-        BT_WAIT(14, &bars->acc2_full[buf], (uint32_t)(u2 >> 1) & 1u);
-        if (!p.proj) BT_WAIT(15, &bars->rfull[slot], (uint32_t)(cidx / p.nr) & 1u);
-        tc_fence_after();
-        BT_T0(tb_);
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + 256u + (uint32_t)(buf * 128 + sg * 64);
-        const uint32_t srow = res_s + (uint32_t)(slot * kRSlot + row * 128);   // this thread's pixel: 64 channels, 128B-swizzled
-        uint32_t v[2][16];
-        tc_ld16(taddr, v[0]);
-#pragma unroll
-        for (int cc = 0; cc < 4; cc++) {
-          const uint32_t a0 = srow + (uint32_t)(((2 * cc) ^ (row & 7)) << 4), a1 = srow + (uint32_t)(((2 * cc + 1) ^ (row & 7)) << 4);
-          uint4 r0 = make_uint4(0u, 0u, 0u, 0u), r1 = r0;
-          if (!p.proj) { r0 = lds128(a0); r1 = lds128(a1); }
-          tc_ld_wait();
-          if (cc < 3) tc_ld16(taddr + (uint32_t)((cc + 1) * 16), v[(cc + 1) & 1]);
-          const int col0 = n2 * 128 + sg * 64 + cc * 16;
-          float f[16];
-#pragma unroll
-          for (int j4 = 0; j4 < 4; j4++) {
-            const float4 b = lds128f(sb_s + (uint32_t)((128 + col0 + j4 * 4) * 4));
-            f[4 * j4] = __uint_as_float(v[cc & 1][4 * j4]) + b.x;
-            f[4 * j4 + 1] = __uint_as_float(v[cc & 1][4 * j4 + 1]) + b.y;
-            f[4 * j4 + 2] = __uint_as_float(v[cc & 1][4 * j4 + 2]) + b.z;
-            f[4 * j4 + 3] = __uint_as_float(v[cc & 1][4 * j4 + 3]) + b.w;
-          }
-          const __half2 *x0 = reinterpret_cast<const __half2 *>(&r0), *x1 = reinterpret_cast<const __half2 *>(&r1);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            const float2 a = __half22float2(x0[j]), b = __half22float2(x1[j]);
-            f[2 * j] += a.x; f[2 * j + 1] += a.y; f[8 + 2 * j] += b.x; f[8 + 2 * j + 1] += b.y;
-          }
-          uint4 o0, o1;
-          __half2 *q0 = reinterpret_cast<__half2 *>(&o0), *q1 = reinterpret_cast<__half2 *>(&o1);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            q0[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-            q1[j] = __floats2half2_rn(f[8 + 2 * j], f[8 + 2 * j + 1]);
-          }
-          if (p.relu) {
-            const __half2 z = __float2half2_rn(0.0f);
-#pragma unroll
-            for (int j = 0; j < 4; j++) { q0[j] = __hmax2(q0[j], z); q1[j] = __hmax2(q1[j], z); }
-          }
-          sts128(a0, o0);
-          sts128(a1, o1);
-        }
-        BT_ADD(18, tb_);
-        BT_T0(tc_);
-        tc_fence_before();
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        BT_ADD(19, tc_);
-        BT_T0(td_);
-        if (lane == 0) {
-          if (p.n3) mbar_arrive_remote(mapa_rank(smem_u32(&bars->ycf[slot]), 0));   // GEMM3 may read this warp's quarter of the chunk
-          mbar_arrive_remote(buf ? lbar_acc2e1 : lbar_acc2e0);   // the accumulator has been read: hand it back (one arrival per warp)
-          if (real) {
-            // 32 pixels = 8 rows x 4 columns of the tile = this warp's 4 KB quarter of the slot; pixels outside the image
-            // are clipped by the TMA unit
-            asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-                         ::"l"(&tmY), "r"(res_s + (uint32_t)(slot * kRSlot + q * 4096)), "r"(n2 * 128 + sg * 64), "r"(h0), "r"(w0 + 4 * q), "r"(img)
-                         : "memory");
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-        }
-        held = slot;
-        __syncwarp();
-        BT_ADD(20, td_);
-      }
-    };
-    // ---- ep3 (GEMM3): acc3 + b_next -> ReLU -> fp16 -> z, 16-byte stores straight from registers (a quarter of y's bytes) ----
-    auto ep3 = [&](int pair, int t) {
-      int img, h0, w0;
-      const bool real = tile_of(pair, img, h0, w0);
-      mbar_wait(&bars->acc3_full, (uint32_t)t & 1u);
-      tc_fence_after();
-      const int cols3 = p.n3 >> 1;                   // this warp's columns of acc3: [sg * cols3, +cols3)
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + 128u + (uint32_t)(sg * cols3);
-      const int hh = h0 + (row & 7), ww = w0 + (row >> 3);
-      const bool inside = real && hh < p.H && ww < p.W;
-      __half *zrow = p.z + (((long long)img * p.H + hh) * p.W + ww) * p.n3 + sg * cols3;
-      uint32_t v[2][16];
-      const int nch = cols3 >> 4;
-      tc_ld16(taddr, v[0]);
-#pragma unroll
-      for (int cc = 0; cc < 4; cc++) {
-        if (cc < nch) {
-          tc_ld_wait();
-          if (cc + 1 < nch) tc_ld16(taddr + (uint32_t)((cc + 1) * 16), v[(cc + 1) & 1]);
-          const int col0 = sg * cols3 + cc * 16;
-          float f[16];
-#pragma unroll
-          for (int j4 = 0; j4 < 4; j4++) {
-            const float4 b = lds128f(sb_s + (uint32_t)((640 + col0 + j4 * 4) * 4));
-            f[4 * j4] = __uint_as_float(v[cc & 1][4 * j4]) + b.x;
-            f[4 * j4 + 1] = __uint_as_float(v[cc & 1][4 * j4 + 1]) + b.y;
-            f[4 * j4 + 2] = __uint_as_float(v[cc & 1][4 * j4 + 2]) + b.z;
-            f[4 * j4 + 3] = __uint_as_float(v[cc & 1][4 * j4 + 3]) + b.w;
-          }
-          uint4 o0, o1;
-          __half2 *q0 = reinterpret_cast<__half2 *>(&o0), *q1 = reinterpret_cast<__half2 *>(&o1);
-          const __half2 z2 = __float2half2_rn(0.0f);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            q0[j] = __hmax2(__floats2half2_rn(f[2 * j], f[2 * j + 1]), z2);
-            q1[j] = __hmax2(__floats2half2_rn(f[8 + 2 * j], f[8 + 2 * j + 1]), z2);
-          }
-          if (inside) {
-            *reinterpret_cast<uint4 *>(zrow + cc * 16) = o0;
-            *reinterpret_cast<uint4 *>(zrow + cc * 16 + 8) = o1;
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(mapa_rank(smem_u32(&bars->acc3_empty), 0));
-    };
-    // software pipeline, mirrored by the MMA warp: ep1(t+1) (feeds GEMM2(t+1)) before ep2(t)
-    int it = 0, t3 = 0;
-    BT_TOTAL_BEGIN();
-    if (c_first < npairs) ep1(it++);
-    for (int pair = c_first; pair < npairs; pair += c_step) {
-      if (pair + c_step < npairs) ep1(it++);
-      ep2(pair);
-      if (p.n3) ep3(pair, t3++);
-    }
-    if (held >= 0 && lane == 0) {
-      asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-      if (!p.proj) mbar_arrive(&bars->rempty[held]);
-    }
-    if (warp == 4) { BT_TOTAL_END(16); }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    return;
   }
 
-  tc_fence_before();
-  cluster_sync_all();   // no CTA may leave while its peer can still write to it / read its shared memory
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
+  // ===================================== MMA + epilogues ====================================
+  const int cw = wg - 1, warp = tid >> 5, lane = tid & 31, q = lane & 3;
+  const uint32_t mid_s = smem_u32(smem + p.mid_off), ysm_s = smem_u32(smem + p.ysm_off);
+  const uint32_t rows = (uint32_t)(cw * 64 * 128);   // this warpgroup's 64 rows inside a [128][64] operand chunk
+  Ring ring;
+  ring.n = p.nstages;
+  int prev = -1;
+  // one K block: wait for its stage, issue its 4 MMAs, and release the PREVIOUS block's stage once at most this
+  // block's MMAs are in flight
+  auto consumed = [&]() {
+    wgmma_wait<1>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    prev = ring.stage;
+    ring.next();
+  };
+  auto drain = [&]() {
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+    prev = -1;
+  };
+  float acc1[C1 / 2];
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    int img, h0, w0;
+    origin(tile, img, h0, w0);
+    // ---- GEMM1: the 3x3 ----
+    for (int kb = 0; kb < 9 * KC1; kb++) {
+      mbar_wait(&full[ring.stage], ring.phase);
+      const uint32_t sa = smem_u32(smem + ring.stage * kStageBytes);
+      mma_block<C1>(acc1, wgmma_desc(sa + rows, 128), wgmma_desc(sa + 16384, 128), kb == 0);
+      consumed();
+    }
+    drain();
+    // pixel of each of this thread's two accumulator rows
+    int prow[2];
+    long long pix[2];
+    bool valid[2];
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+      prow[i] = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;
+      const int dh = prow[i] / p.TW, dw = prow[i] - dh * p.TW, h = h0 + dh, w = w0 + dw;
+      valid[i] = prow[i] < p.TH * p.TW && h < p.H && w < p.W;
+      pix[i] = ((long long)img * p.H + h) * p.W + w;
+    }
+    named_sync(1 + cw);   // the previous tile's GEMM2 / GEMM3 of every warp of this warpgroup read `mid` / `ysm`
+    // ---- epilogue 1: mid = fp16(relu(acc1 + b2)) -> the A operand of GEMM2 ----
+#pragma unroll
+    for (int j = 0; j < C1 / 8; j++) {
+      const int col = 8 * j + 2 * q;
+      const float b0 = p.b2 ? __ldg(p.b2 + col) : 0.0f, b1 = p.b2 ? __ldg(p.b2 + col + 1) : 0.0f;
+#pragma unroll
+      for (int i = 0; i < 2; i++) {
+        const __half2 v = __hmax2(__floats2half2_rn(acc1[4 * j + 2 * i] + b0, acc1[4 * j + 2 * i + 1] + b1), __float2half2_rn(0.0f));
+        sts32(mid_s + (uint32_t)((col >> 6) * kChunk) + swz_off(prow[i], col), h2u(v));
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    named_sync(1 + cw);
+    // ---- GEMM2 per 128-channel output tile, + identity, epilogue 2 ----
+    for (int n2 = 0; n2 < n2tiles; n2++) {
+      float acc2[64];
+      for (int kb = 0; kb < KC1; kb++) {
+        mbar_wait(&full[ring.stage], ring.phase);
+        const uint32_t sa = smem_u32(smem + ring.stage * kStageBytes);
+        mma_block<128>(acc2, wgmma_desc(mid_s + (uint32_t)(kb * kChunk) + rows, 128), wgmma_desc(sa + 16384, 128), kb == 0);
+        consumed();
+      }
+      if (p.proj) {
+        mbar_wait(&full[ring.stage], ring.phase);
+        const uint32_t sa = smem_u32(smem + ring.stage * kStageBytes);
+        mma_block<128>(acc2, wgmma_desc(sa + rows, 128), wgmma_desc(sa + 16384, 128), false);
+        consumed();
+      }
+      drain();
+#pragma unroll
+      for (int j = 0; j < 16; j++) {
+        const int col = n2 * 128 + 8 * j + 2 * q;
+        const float b0 = p.b3 ? __ldg(p.b3 + col) : 0.0f, b1 = p.b3 ? __ldg(p.b3 + col + 1) : 0.0f;
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+          float v0 = acc2[4 * j + 2 * i] + b0, v1 = acc2[4 * j + 2 * i + 1] + b1;
+          if (!p.proj && valid[i]) {
+            const float2 r = __half22float2(*reinterpret_cast<const __half2 *>(p.residual + pix[i] * p.C2 + col));
+            v0 += r.x; v1 += r.y;
+          }
+          __half2 y = __floats2half2_rn(v0, v1);
+          if (p.relu) y = __hmax2(y, __float2half2_rn(0.0f));
+          if (valid[i]) *reinterpret_cast<__half2 *>(p.y + pix[i] * p.C2 + col) = y;
+          if (N3) sts32(ysm_s + (uint32_t)((col >> 6) * kChunk) + swz_off(prow[i], col), h2u(y));
+        }
+      }
+    }
+    if constexpr (N3 > 0) {
+      // ---- GEMM3: the next block's conv1 from the fp16 block output ----
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      named_sync(1 + cw);
+      float acc3[N3 / 2];
+      for (int kb = 0; kb < p.C2 / 64; kb++) {
+        mbar_wait(&full[ring.stage], ring.phase);
+        const uint32_t sa = smem_u32(smem + ring.stage * kStageBytes);
+        mma_block<N3>(acc3, wgmma_desc(ysm_s + (uint32_t)(kb * kChunk) + rows, 128), wgmma_desc(sa + 16384, 128), kb == 0);
+        consumed();
+      }
+      drain();
+#pragma unroll
+      for (int j = 0; j < N3 / 8; j++) {
+        const int col = 8 * j + 2 * q;
+        const float b0 = p.bn ? __ldg(p.bn + col) : 0.0f, b1 = p.bn ? __ldg(p.bn + col + 1) : 0.0f;
+#pragma unroll
+        for (int i = 0; i < 2; i++)
+          if (valid[i])
+            *reinterpret_cast<__half2 *>(p.z + pix[i] * N3 + col) =
+                __hmax2(__floats2half2_rn(acc3[4 * j + 2 * i] + b0, acc3[4 * j + 2 * i + 1] + b1), __float2half2_rn(0.0f));
+      }
+    }
   }
 }
 
-// ---------------------------------------------------------------------------------- host
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-bool bt_encode(CUtensorMap *m, const void *base, int rank, const uint64_t *dims, const uint64_t *strides, const uint32_t *box) {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return false;
-    fn = (EncodeTiledFn)ptr;
-  }
-  cuuint64_t gdim[5], gstr[5];
-  cuuint32_t bx[5], es[5];
-  for (int i = 0; i < rank; i++) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i < rank - 1; i++) gstr[i] = strides[i];
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr, bx, es,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-struct BtDevice { bool ready; };
-BtDevice g_bt_dev[64];
-std::mutex g_bt_mu;
-
-const BtDevice *bt_device(cudaStream_t stream) {
+template <int C1, int N3>
+int launch(int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap *tm, const BtParams &p) {
+  static std::mutex mu;
+  static bool ready[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return nullptr;
-  std::lock_guard<std::mutex> lk(g_bt_mu);
-  BtDevice &d = g_bt_dev[dev];
-  if (d.ready) return &d;
-  if (cudaFuncSetAttribute(bottleneck_tail_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax) != cudaSuccess) return nullptr;
-  d.ready = true;
-  return &d;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return ODTK_E_CUDA;
+  {
+    std::lock_guard<std::mutex> lk(mu);
+    if (!ready[dev]) {
+      if (cudaFuncSetAttribute(bottleneck_tail_kernel<C1, N3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit) != cudaSuccess)
+        return ODTK_E_CUDA;
+      ready[dev] = true;
+    }
+  }
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = (size_t)smem_bytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = odtk_pdl_on() ? 1 : 0;
+  {
+    OdtkProfScope prof(ODTK_PROF_CONV, stream);
+    cudaLaunchKernelEx(&cfg, bottleneck_tail_kernel<C1, N3>, tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 
 }  // namespace
-
-#ifdef ODTK_BT_PROF
-extern "C" int odtk_bt_prof_read(unsigned long long *out, int reset) {
-  if (cudaDeviceSynchronize() != cudaSuccess) return ODTK_E_CUDA;
-  if (cudaMemcpyFromSymbol(out, g_bt_prof, sizeof(unsigned long long) * 32) != cudaSuccess) return ODTK_E_CUDA;
-  if (reset) { unsigned long long z[32] = {0}; cudaMemcpyToSymbol(g_bt_prof, z, sizeof z); }
-  return ODTK_OK;
-}
-#endif
 
 extern "C" int odtk_bottleneck_tail(const odtk_bneck_t *d, odtk_stream_t stream_) {
   if (!d || !d->x || !d->w2 || !d->w3 || !d->y) return ODTK_E_INVALID;
@@ -684,105 +296,62 @@ extern "C" int odtk_bottleneck_tail(const odtk_bneck_t *d, odtk_stream_t stream_
   if ((d->c1 != 64 && d->c1 != 128) || d->c2 % 128 != 0 || d->c2 <= 0 || d->c2 > 512) return ODTK_E_UNSUPPORTED;
   if (((uintptr_t)d->x | (uintptr_t)d->w2 | (uintptr_t)d->w3 | (uintptr_t)d->residual | (uintptr_t)d->y | (uintptr_t)d->xproj | (uintptr_t)d->wproj) & 15) return ODTK_E_INVALID;
   if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const BtDevice *ds = bt_device(stream);
-  if (!ds) return ODTK_E_CUDA;
   BtParams p;
   memset(&p, 0, sizeof p);
-  p.N = d->n; p.H = d->h; p.W = d->width; p.C1 = d->c1; p.C2 = d->c2;
-  p.tiles_h = (d->h + 7) / 8; p.tiles_w = (d->width + 15) / 16;
+  p.N = d->n; p.H = d->h; p.W = d->width; p.C2 = d->c2;
+  choose_patch(d->h, d->width, p.TH, p.TW);
+  p.tiles_h = (d->h + p.TH - 1) / p.TH;
+  p.tiles_w = (d->width + p.TW - 1) / p.TW;
   const long long total = (long long)d->n * p.tiles_h * p.tiles_w;
-  if (total >= (1ll << 30)) return ODTK_E_UNSUPPORTED;
+  if (total >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
   p.total_tiles = (int)total;
-  static int pitch = -1, nr_cap = -1;
-  if (pitch < 0) {
-    const char *e = getenv("ODTK_BNECK_PITCH"); pitch = (e && atoi(e) == 16) ? 16 : 10;
-    const char *r = getenv("ODTK_BNECK_NR"); nr_cap = r ? atoi(r) : 4;   // measured (B200, layer_bench): 4 slots 388 / 262 us (C1 = 64 / 128), 6 slots 418 / 300
-    if (nr_cap < 2 || nr_cap > kMaxRSlots) nr_cap = kMaxRSlots;
-  }
-  p.ppitch = pitch;
-  p.patch_slot = (18 * pitch * 128 + 1023) / 1024 * 1024;
-  p.w_resident = d->c1 == 64;
-  p.proj = proj ? 1 : 0;
-  p.n3 = n3; p.z = (__half *)d->z; p.b_next = d->b_next;
-  { static int late = -1; if (late < 0) { const char *e = getenv("ODTK_BNECK_G3_LATE"); late = e ? atoi(e) : 1; } p.g3_late = late; }   // measured: 491.6 vs 552.1 us per launch
-  const int kc1 = d->c1 / 64, n2tiles = d->c2 / 128;
-  const int w_resident_bytes = 9 * kc1 * (d->c1 / 2) * 128 + n2tiles * kc1 * kWSlot + (proj ? n2tiles * kWSlot : 0) + 2 * n2tiles * (n3 / 2) * 128;
-  if (p.w_resident && w_resident_bytes > 88 * 1024) p.w_resident = 0;
-  if (n3 && !p.w_resident) return ODTK_E_UNSUPPORTED;
-  if (proj && !p.w_resident) return ODTK_E_UNSUPPORTED;
-  const int fixed = 1024 + kNPatch * p.patch_slot + 2 * kc1 * 16384 + kBiasBytes + kBarBytes + (proj ? 2 * kRSlot : 0);
-  // shared-memory budget: identity ring as deep as it gets (it carries the HBM stream), then the weight ring
-  static int nw_min = -1;
-  if (nw_min < 0) { const char *e = getenv("ODTK_BNECK_NW"); nw_min = e ? atoi(e) : 4; if (nw_min < 2 || nw_min > kMaxWSlots) nw_min = 4; }
-  p.nw = p.w_resident ? 0 : nw_min;
-  int left = kSmemMax - fixed - (p.w_resident ? w_resident_bytes : p.nw * kWSlot);
-  p.nr = left / kRSlot;
-  if (p.nr > nr_cap) p.nr = nr_cap;
-  if (proj && p.nr > 2) p.nr = (p.nr >= 4) ? 4 : 2;   // projection mode: the slots are the epilogue's private staging (even count)
-  if (p.nr < 2) return ODTK_E_UNSUPPORTED;
-  left -= p.nr * kRSlot;
-  if (!p.w_resident) { p.nw += left / kWSlot; if (p.nw > kMaxWSlots) p.nw = kMaxWSlots; }
-  const int smem_bytes = fixed + (p.w_resident ? w_resident_bytes : p.nw * kWSlot) + p.nr * kRSlot;
-  p.relu = d->relu;
-  p.b2 = d->b2; p.b3 = d->b3;
+  p.relu = d->relu; p.proj = proj;
+  p.b2 = d->b2; p.b3 = d->b3; p.bn = d->b_next;
+  p.residual = (const __half *)d->residual; p.y = (__half *)d->y; p.z = (__half *)d->z;
+  // shared memory: stages | mid [128][C1] | block output [128][C2] (GEMM3 only) | barriers
+  const int mid_bytes = (d->c1 / 64) * kChunk, ysm_bytes = n3 ? (d->c2 / 64) * kChunk : 0;
+  int nst = (kSmemLimit - 1024 - 256 - mid_bytes - ysm_bytes) / kStageBytes;
+  if (nst > kMaxStages) nst = kMaxStages;
+  if (nst < 2) return ODTK_E_UNSUPPORTED;
+  p.nstages = nst;
+  p.mid_off = nst * kStageBytes;
+  p.ysm_off = p.mid_off + mid_bytes;
+  const int smem_bytes = 1024 + p.ysm_off + ysm_bytes + 2 * kMaxStages * 8;
   const uint64_t C1 = (uint64_t)d->c1, C2 = (uint64_t)d->c2, H = (uint64_t)d->h, W = (uint64_t)d->width, N = (uint64_t)d->n;
-  CUtensorMap tmX, tmW2, tmW3, tmR, tmY, tmWd, tmW1;
+  CUtensorMap tm[6];
   {
-    uint64_t dims[4] = {C1, H, W, N}, str[3] = {W * C1 * 2, C1 * 2, H * W * C1 * 2};
-    uint32_t box[4] = {64, (uint32_t)p.ppitch, 18, 1};
-    if (!bt_encode(&tmX, d->x, 4, dims, str, box)) return ODTK_E_CUDA;
+    uint64_t dims[4] = {C1, W, H, N}, str[3] = {C1 * 2, W * C1 * 2, H * W * C1 * 2};
+    uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+    if (!encode_map(&tm[0], d->x, 4, dims, str, box)) return ODTK_E_CUDA;
   }
   {
     uint64_t dims[2] = {9 * C1, C1}, str[1] = {9 * C1 * 2};
-    uint32_t box[2] = {64, (uint32_t)(d->c1 / 2)};
-    if (!bt_encode(&tmW2, d->w2, 2, dims, str, box)) return ODTK_E_CUDA;
+    uint32_t box[2] = {64, (uint32_t)d->c1};
+    if (!encode_map(&tm[1], d->w2, 2, dims, str, box)) return ODTK_E_CUDA;
   }
   {
     uint64_t dims[2] = {C1, C2}, str[1] = {C1 * 2};
-    uint32_t box[2] = {64, 64};
-    if (!bt_encode(&tmW3, d->w3, 2, dims, str, box)) return ODTK_E_CUDA;
+    uint32_t box[2] = {64, 128};
+    if (!encode_map(&tm[2], d->w3, 2, dims, str, box)) return ODTK_E_CUDA;
   }
-  {
-    uint64_t dims[4] = {C2, H, W, N}, str[3] = {W * C2 * 2, C2 * 2, H * W * C2 * 2};
-    uint32_t boxR[4] = {64, 8, 16, 1}, boxY[4] = {64, 8, 4, 1};
-    if (!bt_encode(&tmY, d->y, 4, dims, str, boxY)) return ODTK_E_CUDA;
-    if (!proj && !bt_encode(&tmR, d->residual, 4, dims, str, boxR)) return ODTK_E_CUDA;
-  }
-  tmWd = tmW3;
-  tmW1 = tmW3;
-  if (n3) {   // next block's conv1 weights [n3, C2]: this CTA's half of the rows, 64-channel K blocks
-    uint64_t dimsW[2] = {C2, (uint64_t)n3}, strW[1] = {C2 * 2};
-    uint32_t boxW[2] = {64, (uint32_t)(n3 / 2)};
-    if (!bt_encode(&tmW1, d->w_next, 2, dimsW, strW, boxW)) return ODTK_E_CUDA;
-  }
-  if (proj) {   // identity = xproj [n, h, width, 64] x wproj [c2, 64]^T, computed by the kernel
-    uint64_t dims[4] = {64, H, W, N}, str[3] = {W * 64 * 2, 64 * 2, H * W * 64 * 2};
-    uint32_t boxR[4] = {64, 8, 16, 1};
-    if (!bt_encode(&tmR, d->xproj, 4, dims, str, boxR)) return ODTK_E_CUDA;
+  tm[3] = tm[0]; tm[4] = tm[2]; tm[5] = tm[2];
+  if (proj) {   // identity = xproj [n, h, width, 64] x wproj [c2, 64]^T: one more K block per output tile
+    uint64_t dims[4] = {64, W, H, N}, str[3] = {64 * 2, W * 64 * 2, H * W * 64 * 2};
+    uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
     uint64_t dimsW[2] = {64, C2}, strW[1] = {64 * 2};
-    uint32_t boxW[2] = {64, 64};
-    if (!bt_encode(&tmWd, d->wproj, 2, dimsW, strW, boxW)) return ODTK_E_CUDA;
+    uint32_t boxW[2] = {64, 128};
+    if (!encode_map(&tm[3], d->xproj, 4, dims, str, box) || !encode_map(&tm[4], d->wproj, 2, dimsW, strW, boxW)) return ODTK_E_CUDA;
+  }
+  if (n3) {
+    uint64_t dims[2] = {C2, (uint64_t)n3}, str[1] = {C2 * 2};
+    uint32_t box[2] = {64, (uint32_t)n3};
+    if (!encode_map(&tm[5], d->w_next, 2, dims, str, box)) return ODTK_E_CUDA;
   }
   const int sms = odtk_sm_count();
-  const int npairs = (p.total_tiles + 1) / 2;
-  int clusters = sms / 2;
-  if (clusters > npairs) clusters = npairs;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)(2 * clusters));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = (size_t)smem_bytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = odtk_pdl_on() ? 2 : 1;
-  {
-    OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    cudaLaunchKernelEx(&cfg, bottleneck_tail_kernel, tmX, tmW2, tmW3, tmR, tmY, tmWd, tmW1, p);
-  }
-  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+  const int grid = p.total_tiles < sms ? p.total_tiles : sms;
+  cudaStream_t stream = (cudaStream_t)stream_;
+  if (d->c1 == 128) return launch<128, 0>(grid, smem_bytes, stream, tm, p);
+  if (n3 == 64) return launch<64, 64>(grid, smem_bytes, stream, tm, p);
+  if (n3 == 128) return launch<64, 128>(grid, smem_bytes, stream, tm, p);
+  return launch<64, 0>(grid, smem_bytes, stream, tm, p);
 }

@@ -1,4 +1,4 @@
-// common.cuh -- small device/host helpers shared by the sm_100a kernels.
+// common.cuh -- small device/host helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -20,9 +20,9 @@ extern int g_odtk_sm_budget;
 static inline int odtk_sm_count_device() {
   static int cache[64];
   int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
   if (dev >= 0 && dev < 64 && cache[dev] > 0) return cache[dev];
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
   if (dev >= 0 && dev < 64) cache[dev] = n;
   return n;
 }

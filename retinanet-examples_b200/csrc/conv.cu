@@ -1,45 +1,30 @@
-// conv.cu -- im2col-free implicit-GEMM convolution on the 5th-gen tensor cores (sm_100a).
+// conv.cu -- im2col-free implicit-GEMM convolution on the Hopper tensor cores (sm_90a, wgmma).
 //
 // Replaces the cuDNN convolutions behind nn.Conv2d in the reference's Model.forward
 // (odtk/model.py:57-68,130-135, odtk/backbones/fpn.py:45-61, torchvision resnet blocks): the
 // reference ships no convolution kernel of its own.  One persistent, warp-specialised kernel:
 //
-//   D[pixels, Cout] = sum over taps (r,s) and 64-channel chunks of  A_tap[pixels, 64] * W[Cout, 64]^T
+//   D[pixels, Cout] = sum over 64-channel chunks and taps (r,s) of  A_tap[pixels, 64] * W[Cout, 64]^T
 //
-//   warp 0   TMA producer (converged warp, one elect.sync lane issues): cp.async.bulk.tensor loads of the
-//            activation operand straight from the NHWC tensor (the hardware zero-fills out-of-bounds
-//            rows/columns == conv padding: no im2col, no border code) and of the weight blocks (2-D map
-//            over [Cout, taps*Cin]) into swizzled shared memory guarded by full/empty mbarriers.
-//   warp 1   MMA issuer (converged warp, one elect.sync lane issues): tcgen05.mma kind::f16, M = 128
-//            (cta_group::1) or 256 across a CTA pair (cta_group::2), N <= 256, K = 16, fp32 accumulation
-//            in TMEM; tcgen05.commit releases the stage and, after the last K block, hands the
-//            accumulator to the epilogue.  Bias = one extra K block (A = ones); bottleneck residual =
-//            D += I * R with the residual tile as an MN-major B operand.
-//   warp 2   TMEM allocator (512 columns = two accumulator buffers, so the epilogue of tile i
-//            overlaps the MMAs of tile i+1).
-//   warps 4-11 epilogue: tcgen05.ld the accumulator (one output pixel per thread), FPN nearest-upsample
-//            add + ReLU, fp16 NHWC store (TMA bulk store for the wide 1x1 layers) -- or, for the last
-//            convolution of a head, (sigmoid +) fp32 NCHW store in the layout the reference's decode entry
-//            point expects -- or, class head on the inference path, sigmoid + threshold + candidate append
-//            straight into the decode workspace (ODTK_OUT_CANDIDATES).
+//   warpgroup 0     TMA producer (one thread issues): cp.async.bulk.tensor loads of the activation operand straight
+//                   from the NHWC tensor (the hardware zero-fills out-of-bounds rows/columns == conv padding: no
+//                   im2col, no border code) and of the weight blocks (2-D map over [Cout, taps*Cin]) into swizzled
+//                   shared memory, guarded by full/empty mbarriers.
+//   warpgroups 1-2  MMA + epilogue, 64 accumulator rows (output pixels) each: wgmma.mma_async m64nNk16 (N = BN = 64
+//                   or 128), fp32 accumulation in registers; the stage is released as soon as the next K block's
+//                   MMAs are in flight.  The epilogue works on the registers: + bias, + residual / FPN nearest-
+//                   upsample, ReLU / ReLU6, fp16 NHWC store -- or, for the last convolution of a head, (sigmoid +)
+//                   fp32 NCHW in the layout the reference's decode entry point expects -- or, class head on the
+//                   inference path, sigmoid + threshold + candidate append straight into the decode workspace.
 //
 // A-operand modes (ConvParams::mode):
-//   0  1x1: 2-D [pixels, Cin] map (plain GEMM rows).
-//   4  3x3 stride 1, "halo": the input patch of a 16x8 / 8x16 pixel tile is loaded ONCE per 64-channel
-//      chunk ([18][16-pixel pitch][64 ch], one 4-D box) and the nine taps are nine shifted UMMA views of
-//      it (make_desc_halo); weights stream behind it, or stay resident when they all fit.
-//   1  3x3 stride 1, one SHIFTED 4-D box per tap (fallback for shapes the fixed halo tiles fit badly).
+//   0  1x1: 2-D [pixels, Cin] map (plain GEMM rows); optionally followed by K blocks of a second operand pair
+//      (the projected identity of a bottleneck block: y = mid * W3^T + xproj * Wproj^T).
+//   1  3x3 stride 1: one SHIFTED 4-D box per tap over a TH x TW pixel patch; a tile table maps the tiles of a
+//      pyramid atlas.  Stride 2 on odd sizes: element-strided boxes (s2).
 //   3  stride-2 1x1 / 3x3 on even sizes: parity-split 5-D view {2C, W/2, 2, H/2, N}.
-//   5  7x7 stride-2 stem, "raw window": the zero-padded NHWC4 image patch is read by the tensor core as an
-//      un-swizzled K-major operand whose 16-byte row pitch is the distance between neighbouring windows
-//      (make_desc_raw); weights resident.   2 = the older overlapping-window 5-D TMA map (fallback).
-// Stride-2 3x3 / 1x1 on odd sizes use element-strided TMA boxes (mode 1 with s2); only Cin % 64 != 0 callers (RGB stems other
-// than the fused 7x7) are first lowered to GEMM rows by layers.cu and run as mode 0.
-// Round 2: 128- and 256-wide 3x3 layers, deep 1x1 layers and narrow head outputs run as cta_group::2 CTA pairs; one launch
-// covers all five pyramid levels through a tile table (pyramid atlas); the candidate epilogue overlaps each slot
-// reservation with the next chunk; ReLU6 (relu == 2); kernels are launched with programmatic stream serialization
-// (griddepcontrol) so that a kernel's prologue runs under its predecessor's tail; remote barrier arrives are one per warp
-// with CTA-scope release.  The stride-1 bottleneck tails of layer1 / layer2 and the stem run in bottleneck.cu / stem.cu.
+//   2  7x7 stride-2 stem: overlapping-window 5-D map of the zero-padded NHWC4 image, 64-byte swizzle.
+// Only Cin % 64 != 0 callers (RGB stems other than the 7x7) are first lowered to GEMM rows by layers.cu and run as mode 0.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -53,935 +38,242 @@
 #include "conv.cuh"
 #include "prof.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int kMaxStages = 16;   // narrow-N layers stream small weight blocks: depth, not bytes, hides the L2 latency
-constexpr int kPipeBytes = 4 * (128 * 128 + 256 * 128);   // pipeline region: 4 stages at BN = 256, up to 8 at small BN
-#ifndef ODTK_EPI_WARPS
-#define ODTK_EPI_WARPS 8   /* measured on B200: 8 warps (168 regs, no spills) 1137 img/s vs 16 warps (96 regs, spills) 961 */
-#endif
-constexpr int kEpiWarps = ODTK_EPI_WARPS;                 // 4 per TMEM lane quarter; each takes every 4th 64-column segment
-constexpr int kABytes = 128 * 128;          // 128 rows x 64 fp16
-constexpr int kBBytesMax = 256 * 128;       // up to 256 rows x 64 fp16
-constexpr int kSlabRowBytes = 128;            // 64 fp16, no padding: 16-byte units are XOR-swizzled with (row & 7)
-constexpr int kSlabBytes = 32 * kSlabRowBytes; // per epilogue warp
-constexpr int kBarrierBytes = 512;
-constexpr int kSmemBytes = kPipeBytes + 1024 /*align slack*/ + kBarrierBytes + kEpiWarps * kSlabBytes;
-constexpr int kThreads = 128 + 32 * kEpiWarps;
-constexpr int kTmemCols = 512;
-constexpr int kAccStride = 256;             // columns between the two accumulator buffers
-
-// Halo mode: view of the patch [18][16 pixels][64 ch] (pixel pitch 128 B, patch-row pitch 2048 B) shifted by a tap.
-// 8-row groups (8 consecutive pixels) are 2048 B apart; the 128-byte swizzle phase of the first row is
-// (start >> 7) & 7: the tensor core derives it from the absolute shared-memory address, exactly as the TMA unit did
-// when it wrote the patch, so the base-offset field [49,52) stays 0 (setting it shifts the phase twice: measured).
-constexpr int kPatchBytes = 18 * 16 * 128;
-__device__ __forceinline__ uint64_t make_desc_halo(uint32_t saddr, int use_boff) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(2048 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  if (use_boff) d |= (uint64_t)((saddr >> 7) & 7u) << 49;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Stem "raw window" mode: the A operand is read straight out of the zero-padded NHWC4 image patch in shared memory.
-// Un-swizzled K-major canonical layout ((8,m),(8,2k)) : ((16 B, SBO),(1, LBO)): the 8 rows of a core matrix are 16 B
-// apart -- exactly the distance between the windows of neighbouring output pixels (stride 2 x 4 channels x 2 B) -- the
-// next 16-byte K chunk of a row is LBO = 16 B further (= chunk 0 of the next pixel: the windows overlap), and the next
-// group of 8 output pixels (one output row down) is SBO = two patch rows further.
-constexpr int kStemPatchW = 24;                         // padded pixels per patch row: 2*8 + 6, rounded to the 16-byte pair
-constexpr int kStemPatchRowBytes = kStemPatchW * 8;     // 192
-constexpr int kStemPatchBytes = 37 * kStemPatchRowBytes;  // 2*16 + 5 rows
-constexpr int kStemPatchSlot = 8192;
+constexpr int kThreads = 384;
+constexpr int kMaxStages = 8;
+constexpr int kPipeBytes = 192 * 1024;   // 6 stages at BN = 128 (32 KB each), 8 at BN = 64
+constexpr int kSmemBytes = kPipeBytes + 1024 /*align slack*/ + 256 /*barriers*/;
 
 struct Barriers {
   uint64_t full[kMaxStages];
   uint64_t empty[kMaxStages];
-  uint64_t patch_full[3], patch_empty[3];
-  uint64_t tmem_full[2];
-  uint64_t tmem_empty[2];
-  uint64_t res_full, res_empty, ident_full;   // residual-on-the-tensor-core path
-  uint32_t tmem_base;
 };
-
-static_assert(sizeof(Barriers) <= kBarrierBytes, "barrier block too small");
+static_assert(sizeof(Barriers) <= 256, "barrier block too small");
 
 // ---------------------------------------------------------------------------------- kernel
-template <int CPW, bool UPS, int CL>   // CL: 0 = single CTAs; 1 = 2-CTA cluster, weight tile multicast; 2 = 2-CTA cluster, cta_group::2 MMA (M = 256 per pair, each CTA holds half of the weight tile); CPW: 16-column chunks per epilogue segment (1, 2, 4 for BN <= 64, 128, 256); UPS: FPN upsample-add
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmOnes,
-                 const __grid_constant__ CUtensorMap tmBias, const __grid_constant__ CUtensorMap tmRes,
-                 const __grid_constant__ CUtensorMap tmIdent, const __grid_constant__ ConvParams p) {
+                 const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+                 const __grid_constant__ ConvParams p) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  Barriers *bars = reinterpret_cast<Barriers *>(smem + kPipeBytes + kEpiWarps * kSlabBytes);
-  constexpr bool CL2 = (CL == 1), TWO = (CL == 2), CLUSTER = (CL != 0);
-  const int kStages = p.nstages, kStageBytes = kABytes + (TWO ? p.BN >> 1 : p.BN) * 128;   // per-layer pipeline geometry
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;   // provably warp-uniform
+  Barriers *bars = reinterpret_cast<Barriers *>(smem + kPipeBytes);
+  const int kStages = p.nstages, rb = p.row_bytes;
+  const int stage_bytes = (128 + BN) * rb;
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0), tid = threadIdx.x & 127;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    if (p.tma_store) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; s++) { mbar_init(&bars->full[s], 1); mbar_init(&bars->empty[s], CL2 ? 2 : 1); }
-    for (int b = 0; b < 2; b++) { mbar_init(&bars->tmem_full[b], 1); mbar_init(&bars->tmem_empty[b], (TWO ? 2 : 1) * kEpiWarps /* one arrival per epilogue warp */); }
-    mbar_init(&bars->res_full, 1); mbar_init(&bars->res_empty, 1); mbar_init(&bars->ident_full, 1);
-    for (int s = 0; s < 3; s++) { mbar_init(&bars->patch_full[s], 1); mbar_init(&bars->patch_empty[s], 1); }
+    for (int s = 0; s < kStages; s++) { mbar_init(&bars->full[s], 1); mbar_init(&bars->empty[s], 8 /* one per consumer warp */); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    if (TWO) {   // both CTAs of the pair issue the paired allocation from the same warp id
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)),
-                   "r"(kTmemCols));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::);
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)),
-                   "r"(kTmemCols));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-    }
-  }
-  tc_fence_before();
-  if (CLUSTER) cluster_sync_all(); else __syncthreads();   // peer barriers must exist before any multicast / remote arrive
-  tc_fence_after();
+  __syncthreads();
   grid_dep_launch_dependents();   // the next kernel's CTAs may take the SMs this grid frees (they wait for our completion)
   grid_dep_wait();                // everything above ran under the previous kernel's tail; its outputs are visible from here
-  const uint32_t tmem_base = bars->tmem_base;
 
   const int total_tiles = p.num_m_tiles * p.num_n_tiles;
-  // work items: single tiles, or -- in a 2-CTA cluster -- pairs of consecutive M tiles on the same N tile (both CTAs
-  // run the same K loop in lockstep and each loads half of the weight tile for both)
-  const int crank = CLUSTER ? (int)cluster_ctarank() : 0;
-  const int mpairs = (p.num_m_tiles + 1) >> 1;
-  const int w_first = CLUSTER ? (int)(blockIdx.x >> 1) : (int)blockIdx.x;
-  const int w_step = CLUSTER ? (int)(gridDim.x >> 1) : (int)gridDim.x;
-  const int w_total = CLUSTER ? mpairs * p.num_n_tiles : total_tiles;
-  auto work_tile = [&](int wi, int &m_tile, int &n_tile) -> bool {   // returns false for the padding tile of an odd pair
-    // N fastest: the CTAs that run concurrently share their input rows (one DRAM read, L2 hits for the other N
-    // tiles); the weights of all N tiles stay L2-resident anyway
-    if (CLUSTER) {
-      const int pair = wi / p.num_n_tiles;
-      n_tile = wi - pair * p.num_n_tiles;
-      m_tile = 2 * pair + crank;
-      if (m_tile >= p.num_m_tiles) { m_tile = p.num_m_tiles - 1; return false; }
-      return true;
+  const int per_img = p.tile_tab ? p.tab_tiles : p.tiles_h * p.tiles_w;
+  const int kb_main = p.taps * p.kblocks_per_tap, kb_all = kb_main + p.kblocks2;
+  // tile origin: N fastest, so that the CTAs running at the same time share their input rows (one DRAM read, L2 hits)
+  auto tile_origin = [&](int tile, int &m_tile, int &n_tile, int &img, int &h0, int &w0, int &hlim, int &wlim) {
+    m_tile = tile / p.num_n_tiles;
+    n_tile = tile - m_tile * p.num_n_tiles;
+    img = 0; h0 = 0; w0 = 0; hlim = p.H; wlim = p.W;
+    if (p.mode != 0) {
+      img = m_tile / per_img;
+      const int r = m_tile - img * per_img;
+      h0 = (r / p.tiles_w) * p.TH;
+      w0 = (r % p.tiles_w) * p.TW;
+      if (p.tile_tab) { const int4 e = __ldg(p.tile_tab + r); h0 = e.x; w0 = e.y; hlim = e.z; wlim = e.w; }
     }
-    m_tile = wi / p.num_n_tiles;
-    n_tile = wi - m_tile * p.num_n_tiles;
-    return true;
   };
-  const int kblocks = p.taps * p.kblocks_per_tap;
-  const uint32_t a_bytes = (p.mode == 0) ? (uint32_t)(128 * p.row_bytes) : (uint32_t)(p.TH * p.TW * p.row_bytes);
-  const uint32_t b_bytes = (uint32_t)((TWO ? p.BN >> 1 : p.BN) * p.row_bytes);   // weight bytes landing in THIS CTA per K block
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================================== TMA producer =====================================
-    {   // whole warp converged; one elected lane arms the barriers and issues the TMA loads
-      int stage = 0;
-      uint32_t phase = 0, rphase = 0;
-      // res_mma: 2 stages | 64 KB residual tile | 32 KB identity.  up_mma: 3 stages | 32 KB source-pixel tile | 16 KB U
-      unsigned char *sres = smem + (p.up_mma ? 3 : 2) * (kABytes + kBBytesMax);
-      unsigned char *sident = sres + (p.up_mma ? 2 : 4) * kABytes;
-      if (p.res_mma && elect_one()) {
-        mbar_arrive_expect_tx(&bars->ident_full, 2u * kABytes);
-        tma_load_2d(sident, &tmIdent, &bars->ident_full, 0, 0);
-        tma_load_2d(sident + kABytes, &tmIdent, &bars->ident_full, 64, 0);
-      }
-      if (p.up_mma && elect_one()) {
-        mbar_arrive_expect_tx(&bars->ident_full, (uint32_t)kABytes);
-        tma_load_2d(sident, &tmIdent, &bars->ident_full, 0, 0);
-      }
-      if (p.mode == 5) {
-        // ---- stem, raw-window mode: the 28 KB of weights stay resident; one 7 KB image patch per tile ----
-        unsigned char *sw = smem + kMaxStages * kStemPatchSlot;
-        if (elect_one()) {
-          mbar_arrive_expect_tx(&bars->ident_full, 7u * (uint32_t)(p.BN * 64));
-          for (int r = 0; r < 7; r++) tma_load_2d(sw + r * (p.BN * 64), &tmB, &bars->ident_full, r * 32, 0);
-        }
-        const int per_img = p.tiles_h * p.tiles_w;
-        for (int tile = w_first; tile < w_total; tile += w_step) {
-          const int img = tile / per_img, rr = tile - img * per_img;
-          const int h0 = (rr / p.tiles_w) * 16, w0 = (rr % p.tiles_w) * 8;
+    if (tid != 0) return;
+    const uint32_t a_bytes = (uint32_t)((p.mode == 0 ? 128 : p.TH * p.TW) * rb), b_bytes = (uint32_t)(BN * rb);
+    const int kelems = rb >> 1;   // K elements per block: 64 (SW128) or 32 (SW64)
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      int m_tile, n_tile, img, h0, w0, hlim, wlim;
+      tile_origin(tile, m_tile, n_tile, img, h0, w0, hlim, wlim);
+      const int n0 = n_tile * BN;
+      // K order: 64-channel chunk outer, tap inner
+      for (int kb = 0; kb < p.kblocks_per_tap; kb++) {
+        const int kch = p.grouped ? n0 : kb * 64;   // input-channel coordinate: grouped convs read their own chunk only
+        for (int tap = 0; tap < p.taps; tap++) {
+          const int dy = tap / p.kw - p.pad, dx = tap % p.kw - p.pad;
           mbar_wait(&bars->empty[stage], phase ^ 1u);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&bars->full[stage], (uint32_t)kStemPatchBytes);
-            // patch rows as whole 192-byte runs of the padded image row (3-D map); the older 4-D map fetched the same
-            // bytes as 12 separate 16-byte pixel pairs per row (444 TMA rows per tile: request-bound)
-            if (p.stem_rows) tma_load_3d(smem + stage * kStemPatchSlot, &tmA, &bars->full[stage], 8 * w0, 2 * h0, img);
-            else             tma_load_4d(smem + stage * kStemPatchSlot, &tmA, &bars->full[stage], 0, w0, 2 * h0, img);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-      } else if (p.mode == 4) {
-        // ---- halo mode: one patch load per (tile, 64-channel chunk), nine weight blocks behind it ----
-        unsigned char *sones = smem + p.npatch * kPatchBytes;
-        unsigned char *sbst = sones + (p.bias_mma ? kABytes : 0);
-        const uint32_t bstage = b_bytes;
-        if (p.bias_mma && elect_one()) {   // constant A operand of the bias block, loaded once
-          if (TWO) {
-            if (crank == 0) mbar_arrive_expect_tx(&bars->ident_full, 2u * kABytes);
-            tma2_load_2d(sones, &tmOnes, mapa_rank(smem_u32(&bars->ident_full), 0), 0, 0);
+          unsigned char *sa = smem + stage * stage_bytes;
+          unsigned char *sb = sa + 128 * rb;
+          mbar_arrive_expect_tx(&bars->full[stage], a_bytes + b_bytes);
+          if (p.mode == 1) {
+            tma_load_4d(sa, &tmA, &bars->full[stage], kch, (w0 << p.s2) + dx, (h0 << p.s2) + dy, img);
+          } else if (p.mode == 3) {
+            // stride 2: input pixel 2*o + d = 2*(o + (d < 0 ? -1 : 0)) + parity, on the parity-split 5-D view
+            const int pw = dx < 0 ? 1 : dx, ph = dy < 0 ? 1 : dy;
+            tma_load_5d(sa, &tmA, &bars->full[stage], pw * p.Cin + kch, w0 + (dx < 0 ? -1 : 0), ph, h0 + (dy < 0 ? -1 : 0), img);
+          } else if (p.mode == 0) {
+            tma_load_2d(sa, &tmA, &bars->full[stage], kch, m_tile * 128);
           } else {
-            mbar_arrive_expect_tx(&bars->ident_full, (uint32_t)kABytes);
-            tma_load_2d(sones, &tmOnes, &bars->ident_full, 0, 0);
+            tma_load_5d(sa, &tmA, &bars->full[stage], 0, w0, tap, h0, img);   // stem: filter row `tap`
           }
-        }
-        if (p.b_resident && elect_one()) {   // small layers (64 -> 64): every weight block stays in shared memory
-          const int nb = 9 * p.kblocks_per_tap;
-          mbar_arrive_expect_tx(&bars->res_full, (uint32_t)(nb + (p.bias_mma ? 1 : 0)) * b_bytes);
-          for (int j = 0; j < nb; j++) tma_load_2d(sbst + j * bstage, &tmB, &bars->res_full, j * 64, 0);
-          if (p.bias_mma) tma_load_2d(sbst + nb * bstage, &tmBias, &bars->res_full, 0, 0);
-        }
-        int pb = 0;
-        uint32_t pphase = 0;
-        const int per_img = p.tile_tab ? p.tab_tiles : p.tiles_h * p.tiles_w, half = p.BN >> 1;
-        for (int tile = w_first; tile < w_total; tile += w_step) {
-          int m_tile, n_tile;
-          work_tile(tile, m_tile, n_tile);
-          const int n0 = n_tile * p.BN;
-          const int img = m_tile / per_img, rr = m_tile - img * per_img;
-          int h0 = (rr / p.tiles_w) * p.TH, w0 = (rr % p.tiles_w) * p.TW;
-          if (p.tile_tab) { const int4 e = __ldg(p.tile_tab + rr); h0 = e.x; w0 = e.y; }   // pyramid atlas: tiles listed per level
-          const int c1 = p.tile_t ? h0 - 1 : w0 - 1, c2 = p.tile_t ? w0 - 1 : h0 - 1;
-          for (int kc = 0; kc < p.kblocks_per_tap; kc++) {
-            mbar_wait(&bars->patch_empty[pb], pphase ^ 1u);
-            unsigned char *dst = smem + pb * kPatchBytes;
-            if (elect_one()) {
-              if (TWO) {
-                if (crank == 0) mbar_arrive_expect_tx(&bars->patch_full[pb], 2u * kPatchBytes);
-                tma2_load_4d(dst, &tmA, mapa_rank(smem_u32(&bars->patch_full[pb]), 0), p.grouped ? n0 : kc * 64, c1, c2, img);
-              } else {
-                mbar_arrive_expect_tx(&bars->patch_full[pb], (uint32_t)kPatchBytes);
-                tma_load_4d(dst, &tmA, &bars->patch_full[pb], p.grouped ? n0 : kc * 64, c1, c2, img);   // grouped: the N tile's own 64-channel chunk
-              }
-            }
-            if (++pb == p.npatch) { pb = 0; pphase ^= 1u; }
-            if (p.b_resident) continue;
-            for (int tap = 0; tap < 9; tap++) {
-              mbar_wait(&bars->empty[stage], phase ^ 1u);
-              unsigned char *sb = sbst + stage * bstage;
-              if (elect_one()) {
-                if (TWO) {
-                  if (crank == 0) mbar_arrive_expect_tx(&bars->full[stage], 2u * b_bytes);
-                  tma2_load_2d(sb, &tmB, mapa_rank(smem_u32(&bars->full[stage]), 0), (tap * p.kblocks_per_tap + kc) * 64, n0 + crank * half);
-                } else {
-                  mbar_arrive_expect_tx(&bars->full[stage], b_bytes);
-                  tma_load_2d(sb, &tmB, &bars->full[stage], (tap * p.kblocks_per_tap + kc) * 64, n0);
-                }
-              }
-              if (++stage == kStages) { stage = 0; phase ^= 1u; }
-            }
-          }
-          if (p.bias_mma && !p.b_resident) {
-            mbar_wait(&bars->empty[stage], phase ^ 1u);
-            unsigned char *sb = sbst + stage * bstage;
-            if (elect_one()) {
-              if (TWO) {
-                if (crank == 0) mbar_arrive_expect_tx(&bars->full[stage], 2u * b_bytes);
-                tma2_load_2d(sb, &tmBias, mapa_rank(smem_u32(&bars->full[stage]), 0), 0, n0 + crank * half);
-              } else {
-                mbar_arrive_expect_tx(&bars->full[stage], b_bytes);
-                tma_load_2d(sb, &tmBias, &bars->full[stage], 0, n0);
-              }
-            }
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-        }
-      } else
-      for (int tile = w_first; tile < w_total; tile += w_step) {
-        int m_tile, n_tile;
-        work_tile(tile, m_tile, n_tile);
-        const int n0 = n_tile * p.BN;
-        int img = 0, h0 = 0, w0 = 0;
-        if (p.mode != 0) {
-          const int per_img = p.tiles_h * p.tiles_w;
-          img = m_tile / per_img;
-          const int r = m_tile - img * per_img;
-          h0 = (r / p.tiles_w) * p.TH;
-          w0 = (r % p.tiles_w) * p.TW;
-        }
-        // K order: 64-channel chunk outer, tap inner -- the same order as the halo mode, so that a layer's result does not
-        // depend on which A-operand mode / tile shape the host code picked (fp32 sums are order-sensitive)
-        for (int kb = 0; kb < p.kblocks_per_tap; kb++) {
-          for (int tap = 0; tap < p.taps; tap++) {
-            const int dy = tap / p.kw - p.pad, dx = tap % p.kw - p.pad;
-            mbar_wait(&bars->empty[stage], phase ^ 1u);
-            unsigned char *sa = smem + stage * kStageBytes;
-            unsigned char *sb = sa + kABytes;
-            const int kelems = p.row_bytes >> 1;   // K elements per block: 64 (SW128) or 32 (SW64)
-            const int kch = p.grouped ? n0 : kb * 64;   // input-channel coordinate: grouped convs read their own chunk only
-            if (TWO) {
-              // cta_group::2: both CTAs load their own A rows and their half of the weight rows into their own
-              // shared memory; every byte is counted on the LEADER's barrier, which the leader arms for the pair
-              if (elect_one()) {
-                const uint32_t lbar = mapa_rank(smem_u32(&bars->full[stage]), 0);
-                if (crank == 0) mbar_arrive_expect_tx(&bars->full[stage], 2u * (a_bytes + b_bytes));
-                const int half = p.BN >> 1;
-                if (p.mode == 1)      tma2_load_4d(sa, &tmA, lbar, kch, (w0 << p.s2) + dx, (h0 << p.s2) + dy, img);
-                else if (p.mode == 3) {
-                  const int pw = dx < 0 ? 1 : dx, ph = dy < 0 ? 1 : dy;
-                  tma2_load_5d(sa, &tmA, lbar, pw * p.Cin + kch, w0 + (dx < 0 ? -1 : 0), ph, h0 + (dy < 0 ? -1 : 0), img);
-                } else                tma2_load_2d(sa, &tmA, lbar, kch, m_tile * 128);
-                tma2_load_2d(sb, &tmB, lbar, (tap * p.kblocks_per_tap + kb) * kelems, n0 + crank * half);
-              }
-              if (++stage == kStages) { stage = 0; phase ^= 1u; }
-              continue;
-            }
-            if (elect_one()) {
-              mbar_arrive_expect_tx(&bars->full[stage], a_bytes + b_bytes);
-              if (p.mode == 1)      tma_load_4d(sa, &tmA, &bars->full[stage], kch, (w0 << p.s2) + dx, (h0 << p.s2) + dy, img);
-              else if (p.mode == 3) {
-                // stride 2: input pixel 2*o + d = 2*(o + (d < 0 ? -1 : 0)) + parity, on the parity-split 5-D view
-                const int pw = dx < 0 ? 1 : dx, ph = dy < 0 ? 1 : dy;
-                tma_load_5d(sa, &tmA, &bars->full[stage], pw * p.Cin + kch, w0 + (dx < 0 ? -1 : 0), ph,
-                            h0 + (dy < 0 ? -1 : 0), img);
-              }
-              else if (p.mode == 0) tma_load_2d(sa, &tmA, &bars->full[stage], kch, m_tile * 128);
-              else                  tma_load_5d(sa, &tmA, &bars->full[stage], 0, w0, tap, h0, img);   // stem: filter row `tap`
-              if (CL2) {   // each CTA fetches half of the weight rows and multicasts them to both
-                const int half = p.BN >> 1;
-                tma_load_2d_mc(sb + crank * half * p.row_bytes, &tmB, &bars->full[stage], (tap * p.kblocks_per_tap + kb) * kelems,
-                               n0 + crank * half, (uint16_t)3);
-              } else {
-                tma_load_2d(sb, &tmB, &bars->full[stage], (tap * p.kblocks_per_tap + kb) * kelems, n0);
-              }
-            }
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-        }
-        if (p.bias_mma) {
-          // one more K block: A = rows of (1, 1, 0, ...), B = (bias_hi, bias_lo, 0, ...) per output channel:
-          // the tensor core adds the fp32 bias (split into two fp16 terms, exact to 2^-22) for free
-          mbar_wait(&bars->empty[stage], phase ^ 1u);
-          unsigned char *sa = smem + stage * kStageBytes;
-          if (elect_one()) {
-            if (TWO) {
-              const uint32_t lbar = mapa_rank(smem_u32(&bars->full[stage]), 0);
-              if (crank == 0) mbar_arrive_expect_tx(&bars->full[stage], 2u * ((uint32_t)kABytes + b_bytes));
-              tma2_load_2d(sa, &tmOnes, lbar, 0, 0);
-              tma2_load_2d(sa + kABytes, &tmBias, lbar, 0, n0 + crank * (p.BN >> 1));
-            } else {
-              mbar_arrive_expect_tx(&bars->full[stage], (uint32_t)kABytes + b_bytes);
-              tma_load_2d(sa, &tmOnes, &bars->full[stage], 0, 0);
-              if (CL2) tma_load_2d_mc(sa + kABytes + crank * (p.BN >> 1) * 128, &tmBias, &bars->full[stage], 0, n0 + crank * (p.BN >> 1), (uint16_t)3);
-              else     tma_load_2d(sa + kABytes, &tmBias, &bars->full[stage], 0, n0);
-            }
-          }
+          tma_load_2d(sb, &tmB, &bars->full[stage], (tap * p.kblocks_per_tap + kb) * kelems, n0);
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
-        if (p.res_pipe) {
-          // residual add as BN / 64 extra K blocks through the ordinary pipeline stages: A slot <- residual chunk
-          // [128 pixels x 64 channels] (same box as an activation block), B slot <- the 64 x 64 identity (8 KB, L2-resident
-          // constant): D[:, 64 j .. 64 j + 63] += R_j * I^T on the tensor core (N = 64 MMAs).  Unlike res_mma no shared
-          // memory is reserved, so the layer keeps all its pipeline stages (4 at BN = 256 instead of 2).
-          for (int j = 0; j < (p.BN >> 6); j++) {
-            mbar_wait(&bars->empty[stage], phase ^ 1u);
-            unsigned char *sa = smem + stage * kStageBytes;
-            if (elect_one()) {
-              if (TWO) {   // each CTA: its own 128 residual rows + its half (32 rows) of the identity; bytes counted on the leader
-                const uint32_t lbar = mapa_rank(smem_u32(&bars->full[stage]), 0);
-                if (crank == 0) mbar_arrive_expect_tx(&bars->full[stage], 2u * ((uint32_t)kABytes + 4096u));
-                tma2_load_2d(sa, &tmRes, lbar, n0 + 64 * j, m_tile * 128);
-                tma2_load_2d(sa + kABytes, &tmIdent, lbar, 0, 32 * crank);
-              } else {
-                mbar_arrive_expect_tx(&bars->full[stage], (uint32_t)kABytes + 8192u);
-                tma_load_2d(sa, &tmRes, &bars->full[stage], n0 + 64 * j, m_tile * 128);
-                tma_load_2d(sa + kABytes, &tmIdent, &bars->full[stage], 0, 0);
-              }
-            }
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-        }
-        if (p.res_mma) {
-          // residual tile [128 pixels x 256 channels] as four 128B-swizzled 64-channel slices: it becomes the
-          // MN-major B operand of D += I * R (identity times residual), i.e. the tensor core does the add
-          mbar_wait(&bars->res_empty, rphase ^ 1u);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&bars->res_full, 4u * kABytes);
-#pragma unroll
-            for (int j = 0; j < 4; j++) tma_load_2d(sres + j * kABytes, &tmRes, &bars->res_full, n0 + 64 * j, m_tile * 128);
-          }
-          rphase ^= 1u;
-        }
-        if (p.up_mma) {
-          // FPN top-down path: the 64 source pixels (rows of the coarser level) that the 128 output pixels of this tile
-          // nearest-upsample from, as four 128B-swizzled 64-channel slices of 64 rows: the MN-major B operand of
-          // D += U * P (U[i][k] = (k == i >> 1)).  Output pixels 16g .. 16g+15 sit in one image row (W % 16 == 0), their
-          // sources are 8 consecutive pixels of one source row: one 8-row box (= one swizzle atom) per group and slice.
-          mbar_wait(&bars->res_empty, rphase ^ 1u);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&bars->res_full, 2u * kABytes);
-            const int hw = p.H * p.W;
-#pragma unroll 1
-            for (int g = 0; g < 8; g++) {
-              long long m = (long long)m_tile * 128 + 16 * g;
-              if (m >= p.M) m = p.M - 16;                       // rows beyond M are never stored: any valid source will do
-              const int im = (int)(m / hw), rem = (int)(m - (long long)im * hw), h = rem / p.W, w = rem - h * p.W;
-              const int src = (im * p.up_h + (h >> 1)) * p.up_w + (w >> 1);
-#pragma unroll
-              for (int j = 0; j < 4; j++) tma_load_2d(sres + j * 8192 + g * 1024, &tmRes, &bars->res_full, n0 + 64 * j, src);
-            }
-          }
-          rphase ^= 1u;
-        }
+      }
+      for (int j = 0; j < p.kblocks2; j++) {
+        mbar_wait(&bars->empty[stage], phase ^ 1u);
+        unsigned char *sa = smem + stage * stage_bytes;
+        mbar_arrive_expect_tx(&bars->full[stage], (uint32_t)((128 + BN) * 128));
+        tma_load_2d(sa, &tmA2, &bars->full[stage], j * 64, m_tile * 128);
+        tma_load_2d(sa + 128 * 128, &tmB2, &bars->full[stage], j * 64, n0);
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer ========================================
-    if (!TWO || crank == 0) {   // cta_group::2: the leader CTA issues for the pair; whole warp converged, one elected lane issues
-      // instruction descriptor: D=f32, A=B=f16, both K-major, N = BN, M = 128 (256 across a CTA pair)
-      const uint32_t idesc = (1u << 4) | ((uint32_t)(p.BN >> 3) << 17) | ((uint32_t)((TWO ? 256 : 128) >> 4) << 24);
-      int stage = 0;
-      uint32_t phase = 0, rphase = 0;
-      int it = 0;
-      const uint32_t sres = smem_u32(smem + (p.up_mma ? 3 : 2) * (kABytes + kBBytesMax)), sident = sres + (p.up_mma ? 2 : 4) * kABytes;
-      if (p.res_mma || p.up_mma) mbar_wait(&bars->ident_full, 0);
-      if (p.mode == 5) {
-        const uint32_t sw = smem_u32(smem + kMaxStages * kStemPatchSlot);
-        mbar_wait(&bars->ident_full, 0);
-        for (int tile = w_first; tile < w_total; tile += w_step, it++) {
-          const int buf = it & 1;
-          mbar_wait(&bars->tmem_empty[buf], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + (uint32_t)(buf * kAccStride);
-          mbar_wait(&bars->full[stage], phase);
-          tc_fence_after();
-          const uint32_t patch = smem_u32(smem + stage * kStemPatchSlot);
-          if (elect_one()) {
-#pragma unroll
-            for (int r = 0; r < 7; r++) {
-#pragma unroll
-              for (int k = 0; k < 2; k++) {   // 16 K elements = 4 padded pixels x 4 channels = 32 B of the window
-                const uint64_t da = p.halo_boff ? make_desc_raw(patch + r * kStemPatchRowBytes + k * 32, 2u * kStemPatchRowBytes, 16u)
-                                                : make_desc_raw(patch + r * kStemPatchRowBytes + k * 32, 16u, 2u * kStemPatchRowBytes);
-                const uint64_t db = make_desc_kmajor(sw + (uint32_t)(r * p.BN * 64), 64) + (uint64_t)(2 * k);
-                tc_mma_f16(tmem_d, da, db, idesc, (r | k) ? 1u : 0u);
-              }
-            }
-            tc_commit(&bars->empty[stage]);
-            tc_commit(&bars->tmem_full[buf]);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-      } else if (p.mode == 4) {
-        const uint32_t sones = smem_u32(smem + p.npatch * kPatchBytes);
-        const uint32_t sbst = sones + (p.bias_mma ? (uint32_t)kABytes : 0u);
-        if (p.bias_mma) mbar_wait(&bars->ident_full, 0);
-        if (p.b_resident) mbar_wait(&bars->res_full, 0);
-        int pb = 0;
-        uint32_t pphase = 0;
-        for (int tile = w_first; tile < w_total; tile += w_step, it++) {
-          const int buf = it & 1;
-          mbar_wait(&bars->tmem_empty[buf], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + (uint32_t)(buf * kAccStride);
-          if (p.b_resident) {
-            // weights resident: one patch per 64-channel chunk is all that moves; everything for the tile in one go
-            for (int kc = 0; kc < p.kblocks_per_tap; kc++) {
-              mbar_wait(&bars->patch_full[pb], pphase);
-              tc_fence_after();
-              const uint32_t pbase = smem_u32(smem + pb * kPatchBytes);
-              if (elect_one()) {
-#pragma unroll
-                for (int tap = 0; tap < 9; tap++) {
-                  const int r = tap / 3, s3 = tap - 3 * r;
-                  const uint32_t off = (uint32_t)(p.tile_t ? s3 * 16 + r : r * 16 + s3) * 128u;
-                  const uint64_t da = make_desc_halo(pbase + off, p.halo_boff);
-                  const uint64_t db = make_desc_kmajor(sbst + (uint32_t)(tap * p.kblocks_per_tap + kc) * b_bytes, 128);
-#pragma unroll
-                  for (int k = 0; k < 4; k++) tc_mma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kc | tap | k) ? 1u : 0u);
-                }
-                tc_commit(&bars->patch_empty[pb]);
-              }
-              if (++pb == p.npatch) { pb = 0; pphase ^= 1u; }
-            }
-            if (elect_one()) {
-              if (p.bias_mma)
-                tc_mma_f16(tmem_d, make_desc_kmajor(sones, 128), make_desc_kmajor(sbst + (uint32_t)(9 * p.kblocks_per_tap) * b_bytes, 128), idesc, 1u);
-              tc_commit(&bars->tmem_full[buf]);
-            }
-            continue;
-          }
-          for (int kc = 0; kc < p.kblocks_per_tap; kc++) {
-            mbar_wait(&bars->patch_full[pb], pphase);
-            tc_fence_after();
-            const uint32_t pbase = smem_u32(smem + pb * kPatchBytes);
-            for (int tap = 0; tap < 9; tap++) {
-              mbar_wait(&bars->full[stage], phase);
-              tc_fence_after();
-              const int r = tap / 3, s3 = tap - 3 * r;
-              const uint32_t off = (uint32_t)(p.tile_t ? s3 * 16 + r : r * 16 + s3) * 128u;
-              const uint64_t da = make_desc_halo(pbase + off, p.halo_boff);
-              const uint64_t db = make_desc_kmajor(sbst + (uint32_t)stage * b_bytes, 128);
-              if (elect_one()) {
-#pragma unroll
-                for (int k = 0; k < 4; k++) {
-                  if (TWO) tc_mma2_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kc | tap | k) ? 1u : 0u);
-                  else     tc_mma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kc | tap | k) ? 1u : 0u);
-                }
-                if (TWO) tc_commit2_mc(&bars->empty[stage], (uint16_t)3); else tc_commit(&bars->empty[stage]);
-                if (tap == 8) { if (TWO) tc_commit2_mc(&bars->patch_empty[pb], (uint16_t)3); else tc_commit(&bars->patch_empty[pb]); }
-              }
-              if (++stage == kStages) { stage = 0; phase ^= 1u; }
-            }
-            if (++pb == p.npatch) { pb = 0; pphase ^= 1u; }
-          }
-          if (p.bias_mma) {
-            mbar_wait(&bars->full[stage], phase);
-            tc_fence_after();
-            const uint64_t da = make_desc_kmajor(sones, 128), db = make_desc_kmajor(sbst + (uint32_t)stage * b_bytes, 128);
-            if (elect_one()) {
-              if (TWO) tc_mma2_f16(tmem_d, da, db, idesc, 1u); else tc_mma_f16(tmem_d, da, db, idesc, 1u);
-              if (TWO) tc_commit2_mc(&bars->empty[stage], (uint16_t)3); else tc_commit(&bars->empty[stage]);
-            }
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-          if (elect_one()) { if (TWO) tc_commit2_mc(&bars->tmem_full[buf], (uint16_t)3); else tc_commit(&bars->tmem_full[buf]); }
-        }
-      } else
-      for (int tile = w_first; tile < w_total; tile += w_step, it++) {
-        const int buf = it & 1;
-        mbar_wait(&bars->tmem_empty[buf], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + (uint32_t)(buf * kAccStride);
-        const int kb_total = kblocks + (p.bias_mma ? 1 : 0);
-        for (int kb = 0; kb < kb_total; kb++) {
-          mbar_wait(&bars->full[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-          const uint64_t da = make_desc_kmajor(sa, p.row_bytes), db = make_desc_kmajor(sa + kABytes, p.row_bytes);
-          const int ksteps = (kb == kblocks) ? 1 : (p.row_bytes >> 5);   // UMMA_K(16) steps per block (+32 B each); the bias block has one
-          if (elect_one()) {
-            for (int k = 0; k < ksteps; k++) {
-              if (TWO) tc_mma2_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-              else     tc_mma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) ? 1u : 0u);
-            }
-            if (TWO)      tc_commit2_mc(&bars->empty[stage], (uint16_t)3);
-            else if (CL2) tc_commit_mc(&bars->empty[stage], (uint16_t)3);
-            else          tc_commit(&bars->empty[stage]);
-          }
-          if (++stage == kStages) { stage = 0; phase ^= 1u; }
-        }
-        if (p.res_pipe) {
-          const uint32_t idesc64 = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)((TWO ? 256 : 128) >> 4) << 24);   // N = 64
-          for (int j = 0; j < (p.BN >> 6); j++) {
-            mbar_wait(&bars->full[stage], phase);
-            tc_fence_after();
-            const uint32_t sa = smem_u32(smem + stage * kStageBytes);
-            const uint64_t da = make_desc_kmajor(sa, 128), db = make_desc_kmajor(sa + kABytes, 128);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < 4; k++) {
-                if (TWO) tc_mma2_f16(tmem_d + (uint32_t)(64 * j), da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc64, 1u);
-                else     tc_mma_f16(tmem_d + (uint32_t)(64 * j), da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc64, 1u);
-              }
-              if (TWO) tc_commit2_mc(&bars->empty[stage], (uint16_t)3); else tc_commit(&bars->empty[stage]);
-            }
-            if (++stage == kStages) { stage = 0; phase ^= 1u; }
-          }
-        }
-        if (p.res_mma) {
-          mbar_wait(&bars->res_full, rphase);
-          tc_fence_after();
-          rphase ^= 1u;
-          const uint32_t idesc_r = idesc | (1u << 16);     // B operand MN-major
-          if (elect_one()) {
-#pragma unroll
-            for (int j = 0; j < 8; j++) {   // K = 128 pixels of the tile, 16 per instruction
-              const uint64_t da = make_desc_kmajor(sident + (uint32_t)(j >> 2) * kABytes, 128) + (uint64_t)(2 * (j & 3));
-              const uint64_t db = make_desc_mnmajor(sres + (uint32_t)j * 2048u, (uint32_t)kABytes);
-              tc_mma_f16(tmem_d, da, db, idesc_r, 1u);
-            }
-            tc_commit(&bars->res_empty);
-          }
-        }
-        if (p.up_mma) {
-          mbar_wait(&bars->res_full, rphase);
-          tc_fence_after();
-          rphase ^= 1u;
-          const uint32_t idesc_r = idesc | (1u << 16);     // B operand MN-major
-          if (elect_one()) {
-#pragma unroll
-            for (int j = 0; j < 4; j++) {   // K = 64 source pixels, 16 per instruction
-              const uint64_t da = make_desc_kmajor(sident, 128) + (uint64_t)(2 * j);
-              const uint64_t db = make_desc_mnmajor(sres + (uint32_t)j * 2048u, 8192u);
-              tc_mma_f16(tmem_d, da, db, idesc_r, 1u);
-            }
-            tc_commit(&bars->res_empty);
-          }
-        }
-        if (elect_one()) { if (TWO) tc_commit2_mc(&bars->tmem_full[buf], (uint16_t)3); else tc_commit(&bars->tmem_full[buf]); }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===================================== epilogue ==========================================
-    // 16 warps: warp_id % 4 selects the TMEM lane quarter (hardware rule), (warp_id - 4) / 4 selects
-    // which column segments of the tile the warp owns.  One accumulator row (= output pixel) per
-    // thread.  NHWC fp16 output goes through a padded shared-memory slab per warp so that global
-    // traffic is row-contiguous: residual / upsample rows are READ coalesced into the slab (all
-    // loads of a segment issued back to back, one segment ahead), combined in fp32 with the
-    // accumulator in place, and the slab is WRITTEN back as contiguous row pieces.
-    // Everything that does not depend on the tile is computed once, outside the tile loop.
-    const int q = warp & 3;
-    const int sg = (warp - 4) >> 2;
-    const int row = q * 32 + lane;      // accumulator row == pixel inside the tile
-    unsigned char *slab = smem + kPipeBytes + (warp - 4) * kSlabBytes;   // 1024-aligned: TMA-store source
-    const uint32_t slab_s = smem_u32(slab);                              // shared-space address: LDS / STS, not generic LD / ST
-    const int nchunks = p.BN >> 4;
-    // column split: 4 segments of cpw 16-column chunks (cpw = 1, 2, 4 for BN <= 64, 128, 256);
-    // a slab row holds cpw*32 bytes = lpr lanes x 16 B and one warp access covers 32/lpr rows
-    constexpr int cpw = CPW;
-    constexpr int lsh = cpw == 1 ? 1 : (cpw == 2 ? 2 : 3);
-    constexpr int lpr = 1 << lsh, rpi = 32 >> lsh;
-    const int sub = lane >> lsh, lx = lane & (lpr - 1);
-    const int nsegs = (nchunks + cpw - 1) / cpw;
-    const bool nhwc = p.out_mode == ODTK_OUT_NHWC_F16;
-    const bool has_addend = (p.residual != nullptr && !p.res_mma && !p.res_pipe) || (UPS && p.upsample != nullptr);
-    const int hw = p.H * p.W, per_img = p.tile_tab ? p.tab_tiles : p.tiles_h * p.tiles_w, patch = p.TH * p.TW;
-    // tile-relative (dh, dw) of the rows this lane touches: own row, and the slab rows k*rpi + sub
-    int own_dh = 0, own_dw = 0, dh8[8], dw8[8];
-    if (p.mode != 0) { own_dh = row / p.TW; own_dw = row - own_dh * p.TW; }
-    if (p.tile_t) { own_dh = row & 7; own_dw = row >> 3; }
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-      const int rr = q * 32 + k * rpi + sub;
-      dh8[k] = (p.mode != 0) ? rr / p.TW : 0;
-      dw8[k] = (p.mode != 0) ? rr - dh8[k] * p.TW : rr;
-      if (p.tile_t) { dh8[k] = rr & 7; dw8[k] = rr >> 3; }
-    }
-    int pix8[8];
-    uint4 pre[8];
-    bool prefetched = false;
-    float breg[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
-    int bias_tile = -1;
-    static_assert(kEpiWarps == 8 || kEpiWarps == 16, "bias registers assume <= 2 segments per warp");
-    int it = 0;
-    for (int tile = w_first; tile < w_total; tile += w_step, it++) {
-      const int buf = it & 1;
-      int m_tile, n_tile;
-      const bool real_tile = work_tile(tile, m_tile, n_tile);
-      const int n0 = n_tile * p.BN;
-      const bool active = real_tile && (nhwc ? (sg < nsegs) : (sg < nchunks));
-      mbar_wait(&bars->tmem_full[buf], (uint32_t)(it >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * kAccStride);
-      // warp-uniform tile origin
-      int img0 = 0, h0 = 0, w0 = 0, hlim = p.H, wlim = p.W;   // hlim / wlim: first row / column NOT to be written
-      if (p.mode != 0) {
-        img0 = m_tile / per_img;
-        const int r = m_tile - img0 * per_img;
-        h0 = (r / p.tiles_w) * p.TH;
-        w0 = (r % p.tiles_w) * p.TW;
-        if (p.tile_tab) { const int4 e = __ldg(p.tile_tab + r); h0 = e.x; w0 = e.y; hlim = e.z; wlim = e.w; }
-      }
-      if (active && nhwc) {
-        // pix8: pixel index (-1: outside the tensor) of slab rows sub, rpi+sub, ...
-#pragma unroll
-        for (int k = 0; k < 8; k++) {
-          if (prefetched) break;
-          if (p.mode != 0) {
-            const int rr = q * 32 + k * rpi + sub, h = h0 + dh8[k], w = w0 + dw8[k];
-            pix8[k] = (k < lpr && rr < patch && h < hlim && w < wlim) ? (img0 * p.oH + p.oR + h) * p.oW + w : -1;
-          } else {
-            const int m = m_tile * 128 + dw8[k];
-            pix8[k] = (k < lpr && (long long)m < p.M) ? m : -1;
-          }
-        }
-        auto fetch = [&](int seg, int n0_, uint4 (&dst)[8]) {
-          const int colbase = n0_ + seg * cpw * 16 + lx * 8;
-          const bool lane_on = lx * 8 < min(cpw, nchunks - seg * cpw) * 16 && colbase < p.Cout;
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            dst[k] = make_uint4(0u, 0u, 0u, 0u);
-            if (pix8[k] >= 0 && lane_on) {
-              if (p.residual && !p.res_mma && !p.res_pipe) dst[k] = __ldg(reinterpret_cast<const uint4 *>(p.residual + (long long)pix8[k] * p.ldr + colbase));
-              if (UPS && p.upsample) {
-                const int i2 = pix8[k] / hw, rem = pix8[k] - i2 * hw, h2 = rem / p.W, w2 = rem - h2 * p.W;
-                const long long up = ((long long)i2 * p.up_h + (h2 >> 1)) * p.up_w + (w2 >> 1);
-                uint4 u = __ldg(reinterpret_cast<const uint4 *>(p.upsample + up * p.Cout + colbase));
-                __half2 *a2 = reinterpret_cast<__half2 *>(&dst[k]);
-                const __half2 *u2 = reinterpret_cast<const __half2 *>(&u);
-#pragma unroll
-                for (int j = 0; j < 4; j++) a2[j] = __hadd2(a2[j], u2[j]);
-              }
-            }
-          }
-        };
-        if (p.bias && !p.bias_mma && n_tile != bias_tile) {   // (re)load this warp's bias values: only when the N tile changes
-          bias_tile = n_tile;
-#pragma unroll
-          for (int i = 0; i < 2; i++) {
-            const int cb = n0 + (sg + i * (kEpiWarps / 4)) * cpw * 16;
-            breg[i][0] = (lane < cpw * 16 && cb + lane < p.Cout) ? __ldg(p.bias + cb + lane) : 0.0f;
-            breg[i][1] = (32 + lane < cpw * 16 && cb + 32 + lane < p.Cout) ? __ldg(p.bias + cb + 32 + lane) : 0.0f;
-          }
-        }
-        if (has_addend && !prefetched) fetch(sg, n0, pre);
-        prefetched = false;
-        int si = 0;
-        for (int seg = sg; seg < nsegs; seg += kEpiWarps / 4, si++) {
-          const int segc = min(cpw, nchunks - seg * cpw);      // 16-column chunks in this segment
-          const int colbase = n0 + seg * cpw * 16;
-          const bool lane_on = lx * 8 < segc * 16 && colbase + lx * 8 < p.Cout;
-          if (p.tma_store) {   // the previous bulk store must have finished READING the slab
-            if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-            __syncwarp();
-          }
-          if (has_addend) {
-#pragma unroll
-            for (int k = 0; k < 8; k++)
-              if (k < lpr) sts128(slab_s + (uint32_t)((k * rpi + sub) * kSlabRowBytes + ((lx ^ ((k * rpi + sub) & 7)) << 4)), pre[k]);
-            __syncwarp();
-            if (seg + kEpiWarps / 4 < nsegs) fetch(seg + kEpiWarps / 4, n0, pre);
-            else if (p.tma_store && !CLUSTER && tile + w_step < w_total) {
-              // last segment of this tile: the write-out below goes through the TMA unit and no longer
-              // needs pix8, so fetch the addend of the NEXT tile's first segment now -- its DRAM latency
-              // then overlaps this segment's maths and the wait for the next accumulator
-              const int nt = tile + w_step, m2 = nt / p.num_n_tiles, n2 = nt - m2 * p.num_n_tiles;
-#pragma unroll
-              for (int k = 0; k < 8; k++) {
-                const int m = m2 * 128 + dw8[k];
-                pix8[k] = (k < lpr && (long long)m < p.M) ? m : -1;
-              }
-              fetch(sg, n2 * p.BN, pre);
-              prefetched = true;
-            }
-          }
-          // ---- accumulator (+bias, +staged addend, ReLU) -> fp16 into the own slab row ----
-          uint32_t v[2][16];
-          tc_ld16(taddr + (uint32_t)(seg * cpw * 16), v[0]);
-#pragma unroll
-          for (int cc = 0; cc < 4; cc++) {
-            if (cc < segc) {
-              tc_ld_wait();
-              if (cc + 1 < segc) tc_ld16(taddr + (uint32_t)((seg * cpw + cc + 1) * 16), v[(cc + 1) & 1]);
-              const int col0 = colbase + cc * 16;
-              float f[16];
-#pragma unroll
-              for (int j = 0; j < 16; j++) f[j] = __uint_as_float(v[cc & 1][j]);
-              if (p.bias && !p.bias_mma) {   // lane l of the warp holds the bias of segment columns l and 32 + l
-                const float bsrc = (cc & 2) ? (si ? breg[1][1] : breg[0][1]) : (si ? breg[1][0] : breg[0][0]);
-#pragma unroll
-                for (int j = 0; j < 16; j++) f[j] += __shfl_sync(0xffffffffu, bsrc, (cc & 1) * 16 + j);
-              }
-              const uint32_t srow = slab_s + (uint32_t)(lane * kSlabRowBytes);
-              const int u0 = ((2 * cc) ^ (lane & 7)) << 4, u1 = u0 ^ 16;
-              if (has_addend) {
-                uint4 r0 = lds128(srow + u0), r1 = lds128(srow + u1);
-                const __half2 *x0 = reinterpret_cast<const __half2 *>(&r0), *x1 = reinterpret_cast<const __half2 *>(&r1);
-#pragma unroll
-                for (int j = 0; j < 4; j++) {
-                  float2 a = __half22float2(x0[j]), b = __half22float2(x1[j]);
-                  f[2 * j] += a.x; f[2 * j + 1] += a.y; f[8 + 2 * j] += b.x; f[8 + 2 * j + 1] += b.y;
-                }
-              }
-              uint4 o0, o1;
-              __half2 *q0 = reinterpret_cast<__half2 *>(&o0), *q1 = reinterpret_cast<__half2 *>(&o1);
-#pragma unroll
-              for (int j = 0; j < 4; j++) {
-                q0[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-                q1[j] = __floats2half2_rn(f[8 + 2 * j], f[8 + 2 * j + 1]);
-              }
-              if (p.relu) {   // on the packed halves: max(round(x), 0) == round(max(x, 0)), half the instructions
-                const __half2 z = __float2half2_rn(0.0f);
-#pragma unroll
-                for (int j = 0; j < 4; j++) { q0[j] = __hmax2(q0[j], z); q1[j] = __hmax2(q1[j], z); }
-                if (p.relu == 2) {   // ReLU6 (MobileNetV2, odtk/backbones/mobilenet.py): 6.0 is exact in fp16
-                  const __half2 six = __float2half2_rn(6.0f);
-#pragma unroll
-                  for (int j = 0; j < 4; j++) { q0[j] = __hmin2(q0[j], six); q1[j] = __hmin2(q1[j], six); }
-                }
-              }
-              sts128(srow + u0, o0);
-              sts128(srow + u1, o1);
-            }
-          }
-          if (p.tma_store) {
-            // ---- slab -> global as ONE asynchronous bulk tensor store (32 rows x 128 B, 128B-swizzled
-            // exactly like the slab; rows beyond M are clipped by the TMA unit) ----
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-            __syncwarp();
-            if (lane == 0) {
-              asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                           ::"l"(&tmC), "r"(smem_u32(slab)), "r"(colbase), "r"(m_tile * 128 + q * 32)
-                           : "memory");
-              asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-            continue;
-          }
-          __syncwarp();
-          // ---- slab -> global: rpi rows x (lpr x 16) contiguous bytes per warp store ----
-#pragma unroll
-          for (int k = 0; k < 8; k++) {
-            if (k < lpr && pix8[k] >= 0 && lane_on) {
-              uint4 val = lds128(slab_s + (uint32_t)((k * rpi + sub) * kSlabRowBytes + ((lx ^ ((k * rpi + sub) & 7)) << 4)));
-              *reinterpret_cast<uint4 *>(reinterpret_cast<__half *>(p.out) + (long long)pix8[k] * p.ldy + colbase + lx * 8) = val;
-            }
-          }
-          __syncwarp();
-        }
-      } else if (active) {
-        // fp32 NCHW (+ sigmoid): lanes of a warp are consecutive pixels of a row -> coalesced
-        int img, h, w;
-        bool valid;
-        if (p.mode != 0) {
-          img = img0; h = h0 + own_dh; w = w0 + own_dw;
-          valid = row < patch && h < hlim && w < wlim;
-        } else {
-          const int m = m_tile * 128 + row;
-          valid = (long long)m < p.M;
-          img = m / hw;
-          const int rem = m - img * hw;
-          h = rem / p.W;
-          w = rem - h * p.W;
-        }
-        const long long cs = hw;
-        if (p.out_mode == ODTK_OUT_CANDIDATES) {
-          // class-head final layer: only the scores above the threshold leave the SM, appended to the decode
-          // workspace as (key, flat NCHW index) pairs + the key histogram, exactly what decode.cu's
-          // score_filter_kernel would have produced from the dense map
-          const int pix = h * p.W + w;
-          // logits of chunk c (+ bias, ReLU) -> v, bit j of the result set where the cheap pre-test x > logit(thresh) - margin passes
-          auto load_chunk = [&](int c, uint32_t (&v)[16]) -> unsigned {
-            tc_ld16(taddr + (uint32_t)(c * 16), v);
-            tc_ld_wait();
-            const int col0 = n0 + c * 16;
-            const int ncol = min(16, p.Cout - col0);
-            unsigned pass = 0;
-            if (valid) {
-#pragma unroll
-              for (int j = 0; j < 16; j++) {
-                if (j < ncol) {
-                  float x = __uint_as_float(v[j]) + ((p.bias && !p.bias_mma) ? __ldg(p.bias + col0 + j) : 0.0f);
-                  if (p.relu) x = fmaxf(x, 0.0f);
-                  v[j] = __float_as_uint(x);
-                  if (x > p.cand_pre) pass |= 1u << j;
-                }
-              }
-            }
-            return pass;
-          };
-          auto emit = [&](int c, const uint32_t (&v)[16], unsigned hit, int base) {   // v holds the SCORES of the hit lanes
-            const int col0 = n0 + c * 16;
-            uint2 *dst = p.cand + (long long)img * p.cand_cap;
-            unsigned *hist = p.cand_hist + (long long)img * p.cand_hist_bins;
-#pragma unroll
-            for (int j = 0; j < 16; j++)
-              if ((hit >> j) & 1u) {
-                const uint32_t key = odtk_float_key(__uint_as_float(v[j]));
-                if ((long long)base < p.cand_cap) dst[base] = make_uint2(key, (uint32_t)((col0 + j) * hw + pix));
-                base++;
-                const uint32_t dd = (key - p.cand_key_thresh) >> p.cand_shift;
-                atomicAdd(hist + (dd < (uint32_t)(p.cand_hist_bins - 1) ? dd : (uint32_t)(p.cand_hist_bins - 1)), 1u);
-              }
-          };
-          // (A two-pass variant -- count all chunks, ONE slot reservation per warp and tile, then write -- measured 5x SLOWER
-          // on B200: 6289 vs 1260 us for the 100 x 160 level; the single pass with one reservation per chunk stays.)
-          if (p.mode != 0) {
-            // The whole tile lies in one image: one slot reservation (returning atomic) per warp and chunk, software-
-            // pipelined: the reservation of chunk c is ISSUED, chunk c + 2's logits are loaded and tested, and only then
-            // is chunk c written -- the atomic's L2 round trip (~1000 cycles) overlaps the next chunk's work.
-            uint32_t vp[16];
-            unsigned hit_p = 0;
-            int c_p = -1, b0_p = 0, off_p = 0;       // pending chunk: its scores, hit mask, lane 0's reservation, lane offset
-            for (int c = sg; c < nchunks; c += kEpiWarps / 4) {
-              uint32_t v[16];
-              const unsigned pass = load_chunk(c, v);
-              unsigned hit = 0;
-              if (__any_sync(0xffffffffu, pass != 0)) {
-#pragma unroll
-                for (int j = 0; j < 16; j++)
-                  if ((pass >> j) & 1u) {
-                    const float sc = sigmoidf_accurate(__uint_as_float(v[j]));
-                    v[j] = __float_as_uint(sc);
-                    if (sc > p.cand_thresh) hit |= 1u << j;
-                  }
-              }
-              const int cnt = __popc(hit);
-              int incl = cnt;
-#pragma unroll
-              for (int o = 1; o < 32; o <<= 1) {
-                const int u = __shfl_up_sync(0xffffffffu, incl, o);
-                if (lane >= o) incl += u;
-              }
-              const int total = __shfl_sync(0xffffffffu, incl, 31);
-              int b0 = 0;
-              if (total > 0 && lane == 0) b0 = atomicAdd(p.cand_counts + img, total);   // issued; consumed one chunk later
-              if (c_p >= 0) {
-                const int wbase = __shfl_sync(0xffffffffu, b0_p, 0);
-                if (hit_p) emit(c_p, vp, hit_p, wbase + off_p);
-              }
-              if (total > 0) {
-#pragma unroll
-                for (int j = 0; j < 16; j++) vp[j] = v[j];
-                hit_p = hit; c_p = c; b0_p = b0; off_p = incl - cnt;
-              } else c_p = -1;
-            }
-            if (c_p >= 0) {
-              const int wbase = __shfl_sync(0xffffffffu, b0_p, 0);
-              if (hit_p) emit(c_p, vp, hit_p, wbase + off_p);
-            }
-          } else
-          for (int c = sg; c < nchunks; c += kEpiWarps / 4) {   // GEMM-row tiles may straddle images: per-lane reservations
-            uint32_t v[16];
-            const unsigned pass = load_chunk(c, v);
-            if (!__any_sync(0xffffffffu, pass != 0)) continue;
-            unsigned hit = 0;
-#pragma unroll
-            for (int j = 0; j < 16; j++)
-              if ((pass >> j) & 1u) {
-                const float sc = sigmoidf_accurate(__uint_as_float(v[j]));
-                v[j] = __float_as_uint(sc);
-                if (sc > p.cand_thresh) hit |= 1u << j;
-              }
-            const int cnt = __popc(hit);
-            if (cnt) emit(c, v, hit, atomicAdd(p.cand_counts + img, cnt));
-          }
-        } else
-        for (int c = sg; c < nchunks; c += kEpiWarps / 4) {
-          uint32_t v[16];
-          tc_ld16(taddr + (uint32_t)(c * 16), v);
-          tc_ld_wait();
-          const int col0 = n0 + c * 16;
-          const int ncol = min(16, p.Cout - col0);
-          if (!valid || ncol <= 0) continue;
-          float *o = reinterpret_cast<float *>(p.out) + ((long long)img * p.Cout + col0) * cs + (long long)h * p.W + w;
-#pragma unroll
-          for (int j = 0; j < 16; j++) {
-            if (j < ncol) {
-              float x = __uint_as_float(v[j]) + ((p.bias && !p.bias_mma) ? __ldg(p.bias + col0 + j) : 0.0f);
-              if (p.relu) x = fmaxf(x, 0.0f);
-              if (p.out_mode == ODTK_OUT_NCHW_F32_SIGMOID) x = sigmoidf_accurate(x);
-              o[j * cs] = x;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {   // one arrival per warp (256 remote arrivals per tile serialise on the leader's barrier)
-        if (TWO) mbar_arrive_remote(mapa_rank(smem_u32(&bars->tmem_empty[buf]), 0));   // the leader waits for both CTAs
-        else     mbar_arrive(&bars->tmem_empty[buf]);
-      }
-    }
-    if (p.tma_store && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    return;
   }
 
-  tc_fence_before();
-  if (CLUSTER) cluster_sync_all(); else __syncthreads();   // no CTA may leave while its peer can still write to it
-  if (warp == 2) {
-    tc_fence_after();
-    if (TWO) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-    else     asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
+  // ===================================== MMA + epilogue ======================================
+  const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
+  const int q = lane & 3;
+  const int hw = p.H * p.W, patch = p.TH * p.TW;
+  float acc[BN / 2];
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+    int m_tile, n_tile, img0, h0, w0, hlim, wlim;
+    tile_origin(tile, m_tile, n_tile, img0, h0, w0, hlim, wlim);
+    const int n0 = n_tile * BN;
+    int prev = -1;
+    for (int kb = 0; kb < kb_all; kb++) {
+      mbar_wait(&bars->full[stage], phase);
+      const int brb = kb < kb_main ? rb : 128;
+      const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+      const uint64_t da = wgmma_desc(sa + (uint32_t)(cw * 64 * brb), brb), db = wgmma_desc(sa + (uint32_t)(128 * brb), brb);
+      wgmma_fence();
+      if (brb == 128) {
+#pragma unroll
+        for (int k = 0; k < 4; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+      } else {
+#pragma unroll
+        for (int k = 0; k < 2; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+      }
+      wgmma_commit();
+      // the previous K block's MMAs have finished reading their stage once at most one group is in flight
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&bars->empty[prev]);
+      prev = stage;
+      if (++stage == kStages) { stage = 0; phase ^= 1u; }
+    }
+    wgmma_wait<0>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&bars->empty[prev]);
+
+    // ---- epilogue: thread holds rows r and r + 8, columns 8 j + 2 q (+1) ----
+#pragma unroll
+    for (int i = 0; i < 2; i++) {
+      const int row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;
+      bool valid;
+      int img, h, w;
+      long long m;   // dense pixel index (residual / mode-0 rows)
+      if (p.mode != 0) {
+        const int dh = row / p.TW, dw = row - dh * p.TW;
+        img = img0; h = h0 + dh; w = w0 + dw;
+        valid = row < patch && h < hlim && w < wlim;
+        m = ((long long)img * p.H + h) * p.W + w;
+      } else {
+        m = (long long)m_tile * 128 + row;
+        valid = m < p.M;
+        img = (int)(m / hw);
+        const int rem = (int)(m - (long long)img * hw);
+        h = rem / p.W;
+        w = rem - h * p.W;
+      }
+      if (p.out_mode == ODTK_OUT_NHWC_F16) {
+        if (!valid) continue;
+        const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
+        __half *o = reinterpret_cast<__half *>(p.out) + opix * p.ldy;
+        const __half *res = p.residual ? p.residual + m * p.ldr : nullptr;
+        const __half *up = p.upsample ? p.upsample + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++) {
+          const int col = n0 + 8 * j + 2 * q;
+          if (col >= p.Cout) continue;   // Cout % 16 == 0: both columns of the pair are in range or neither
+          float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+          if (p.bias) { v0 += __ldg(p.bias + col); v1 += __ldg(p.bias + col + 1); }
+          if (res) { const float2 r = __half22float2(*reinterpret_cast<const __half2 *>(res + col)); v0 += r.x; v1 += r.y; }
+          if (up) { const float2 u = __half22float2(*reinterpret_cast<const __half2 *>(up + col)); v0 += u.x; v1 += u.y; }
+          __half2 y = __floats2half2_rn(v0, v1);
+          if (p.relu) {   // on the packed halves: max(round(x), 0) == round(max(x, 0))
+            y = __hmax2(y, __float2half2_rn(0.0f));
+            if (p.relu == 2) y = __hmin2(y, __float2half2_rn(6.0f));   // ReLU6: 6.0 is exact in fp16
+          }
+          *reinterpret_cast<__half2 *>(o + col) = y;
+        }
+      } else if (p.out_mode == ODTK_OUT_CANDIDATES) {
+        // class-head final layer: only the scores above the threshold leave the SM, appended to the decode workspace as
+        // (key, flat NCHW index) pairs + the key histogram, exactly what decode.cu's score_filter_kernel would have
+        // produced from the dense map.  Pass 1 counts this row's hits (one slot reservation per thread and row), pass 2
+        // writes them.
+        if (!valid) continue;
+        const int pix = h * p.W + w;
+        auto score = [&](int j, int k, float &sc) -> bool {
+          const int col = n0 + 8 * j + 2 * q + k;
+          if (col >= p.Cout) return false;
+          float x = acc[4 * j + 2 * i + k] + (p.bias ? __ldg(p.bias + col) : 0.0f);
+          if (p.relu) x = fmaxf(x, 0.0f);
+          if (!(x > p.cand_pre)) return false;
+          sc = sigmoidf_accurate(x);
+          return sc > p.cand_thresh;
+        };
+        int cnt = 0;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+          for (int k = 0; k < 2; k++) { float sc; if (score(j, k, sc)) cnt++; }
+        if (!cnt) continue;
+        int base = atomicAdd(p.cand_counts + img, cnt);
+        uint2 *dst = p.cand + (long long)img * p.cand_cap;
+        unsigned *hist = p.cand_hist + (long long)img * p.cand_hist_bins;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+          for (int k = 0; k < 2; k++) {
+            float sc;
+            if (!score(j, k, sc)) continue;
+            const uint32_t key = odtk_float_key(sc);
+            if ((long long)base < p.cand_cap) dst[base] = make_uint2(key, (uint32_t)((n0 + 8 * j + 2 * q + k) * hw + pix));
+            base++;
+            const uint32_t dd = (key - p.cand_key_thresh) >> p.cand_shift;
+            atomicAdd(hist + (dd < (uint32_t)(p.cand_hist_bins - 1) ? dd : (uint32_t)(p.cand_hist_bins - 1)), 1u);
+          }
+      } else {
+        // fp32 NCHW (+ sigmoid)
+        if (!valid) continue;
+        float *o = reinterpret_cast<float *>(p.out) + (long long)img * p.Cout * hw + (long long)h * p.W + w;
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+          for (int k = 0; k < 2; k++) {
+            const int col = n0 + 8 * j + 2 * q + k;
+            if (col >= p.Cout) continue;
+            float x = acc[4 * j + 2 * i + k] + (p.bias ? __ldg(p.bias + col) : 0.0f);
+            if (p.relu) x = fmaxf(x, 0.0f);
+            if (p.out_mode == ODTK_OUT_NCHW_F32_SIGMOID) x = sigmoidf_accurate(x);
+            o[(long long)col * hw] = x;
+          }
+      }
+    }
   }
 }
 
+// ---------------------------------------------------------------------------------- host
 // ---------------------------------------------------------------------------------- host
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
@@ -1021,8 +313,10 @@ std::mutex g_map_mu;
 std::unordered_map<MapKey, CUtensorMap, MapKeyHash> g_map_cache;
 long long g_map_hits = 0, g_map_misses = 0;
 
+}  // namespace
+
 bool encode_map(CUtensorMap *m, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
-                const uint32_t *box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, const uint32_t *elem_strides = nullptr) {
+                const uint32_t *box, CUtensorMapSwizzle swz, const uint32_t *elem_strides) {
   MapKey key;
   memset(&key, 0, sizeof key);
   key.base = base; key.rank = rank; key.swz = (int)swz;
@@ -1066,119 +360,66 @@ void choose_patch(int H, int W, int &TH, int &TW) {
   }
 }
 
-template <int CPW, bool UPS, int CL2>
-bool configure_one() {
-  return cudaFuncSetAttribute(conv_gemm_kernel<CPW, UPS, CL2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) ==
-         cudaSuccess;
-}
-bool configure_kernels() {
-  return configure_one<1, false, 0>() && configure_one<2, false, 0>() && configure_one<4, false, 0>() &&
-         configure_one<4, true, 0>() && configure_one<4, false, 1>() && configure_one<4, false, 2>();
-}
-template <int CPW, bool UPS, int CL2, class... Args>
-void launch_one(int grid, cudaStream_t stream, Args... args) {
+namespace {
+
+template <int BN>
+void launch_bn(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
+               const CUtensorMap &tmB2, const ConvParams &p) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(kThreads);
   cfg.dynamicSmemBytes = kSmemBytes;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (CL2) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = 2; attr[na].val.clusterDim.y = 1; attr[na].val.clusterDim.z = 1;
-    na++;
-  }
-  if (odtk_pdl_on()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    na++;
-  }
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = na;
-  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<CPW, UPS, CL2>, args...);
-}
-void launch_conv(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmC,
-                 const CUtensorMap &tmO, const CUtensorMap &tmBi, const CUtensorMap &tmR, const CUtensorMap &tmI,
-                 const ConvParams &p) {
-  const int nchunks = p.BN >> 4;
-  // narrow tiles: 32-column segments (CPW 2) give every epilogue warp ONE segment whose second TMEM load overlaps the
-  // conversion of the first, instead of two serialised 16-column segments (CPW 1)
-  static int cpw1_max = -1;
-  if (cpw1_max < 0) { const char *e = getenv("ODTK_CONV_CPW1_MAX"); cpw1_max = e ? atoi(e) : 2; }
-  if (p.cluster2 == 2)   launch_one<4, false, 2>(grid & ~1, stream, tmA, tmB, tmC, tmO, tmBi, tmR, tmI, p);
-  else if (p.cluster2)   launch_one<4, false, 1>(grid & ~1, stream, tmA, tmB, tmC, tmO, tmBi, tmR, tmI, p);
-  else if (p.upsample && !p.up_mma) launch_one<4, true, 0>(grid, stream, tmA, tmB, tmC, tmO, tmBi, tmR, tmI, p);
-  else if (nchunks <= cpw1_max) launch_one<1, false, 0>(grid, stream, tmA, tmB, tmC, tmO, tmBi, tmR, tmI, p);
-  else if (nchunks <= 8) launch_one<2, false, 0>(grid, stream, tmA, tmB, tmC, tmO, tmBi, tmR, tmI, p);
-  else                   launch_one<4, false, 0>(grid, stream, tmA, tmB, tmC, tmO, tmBi, tmR, tmI, p);
+  cfg.numAttrs = odtk_pdl_on() ? 1 : 0;
+  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN>, tmA, tmB, tmA2, tmB2, p);
 }
 
-// constant operands: the 128 x 128 identity (A operand of the residual MMAs) and the ones tile (A operand of the bias
-// block: 128 rows x 64 fp16, columns 0 and 1 are 1.0).  __device__ globals: one instance per device.
-__device__ __half g_ident_op[128 * 128];
-__device__ __half g_upsel_op[128 * 64];   // U[i][k] = (k == i >> 1): nearest-upsample selection (A operand of the FPN add)
-__device__ __half g_ident64_op[64 * 64];   // 64 x 64 identity: B operand of the pipelined residual add
-__device__ __half g_ones_op[128 * 64];
-__global__ void init_const_operands_kernel() {
-  for (int i = threadIdx.x; i < 64 * 64; i += blockDim.x) g_ident64_op[i] = __float2half_rn((i >> 6) == (i & 63) ? 1.0f : 0.0f);
-  for (int i = threadIdx.x; i < 128 * 64; i += blockDim.x) g_upsel_op[i] = __float2half_rn((i & 63) == (i >> 7) ? 1.0f : 0.0f);
-  for (int i = threadIdx.x; i < 128 * 128; i += blockDim.x) g_ident_op[i] = __float2half_rn((i >> 7) == (i & 127) ? 1.0f : 0.0f);
-  for (int i = threadIdx.x; i < 128 * 64; i += blockDim.x) g_ones_op[i] = __float2half_rn((i & 63) < 2 ? 1.0f : 0.0f);
-}
-// bias operand: [cout, 64] fp16 with (hi, lo, 0, ...): hi + lo == bias to 2^-22 relative
-__global__ void pack_bias_kernel(const float *bias, __half *out, int cout) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cout * 64; i += gridDim.x * blockDim.x) {
-    const int c = i >> 6, k = i & 63;
-    float v = 0.0f;
-    if (k < 2) {
-      const float b = bias[c];
-      const float hi = __half2float(__float2half_rn(b));
-      v = (k == 0) ? hi : b - hi;
-    }
-    out[i] = __float2half_rn(v);
-  }
-}
-
-// Per-device state (one process may drive several GPUs): SM count, the > 48 KB dynamic-shared-memory opt-in of every
-// kernel instance (a per-device function attribute) and the addresses of the constant operands, initialised once per
-// device.  The init kernel runs on the caller's stream and is followed by a device-wide synchronisation unless that
-// stream is capturing (then it simply becomes part of the graph), so later callers on OTHER streams are ordered too.
+// Per-device state (one process may drive several GPUs): the > 48 KB dynamic-shared-memory opt-in of every kernel
+// instance is a per-device function attribute.
 constexpr int kMaxDevices = 64;
-struct DeviceState {
-  bool ready;
-  int num_sms;
-  void *ident, *ones, *upsel, *ident64;
-};
-DeviceState g_dev[kMaxDevices];
+bool g_dev_ready[kMaxDevices];
 std::mutex g_dev_mu;
 
-const DeviceState *device_state(cudaStream_t stream) {
+bool device_ready() {
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return nullptr;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return false;
   std::lock_guard<std::mutex> lk(g_dev_mu);
-  DeviceState &d = g_dev[dev];
-  if (d.ready) return &d;
-  if (cudaDeviceGetAttribute(&d.num_sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || d.num_sms <= 0) return nullptr;
-  if (!configure_kernels()) return nullptr;
-  if (cudaGetSymbolAddress(&d.ident, g_ident_op) != cudaSuccess || cudaGetSymbolAddress(&d.ones, g_ones_op) != cudaSuccess ||
-      cudaGetSymbolAddress(&d.upsel, g_upsel_op) != cudaSuccess ||
-      cudaGetSymbolAddress(&d.ident64, g_ident64_op) != cudaSuccess) return nullptr;
-  init_const_operands_kernel<<<1, 256, 0, stream>>>();
-  if (cudaGetLastError() != cudaSuccess) return nullptr;
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(stream, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone) {
-    if (cudaDeviceSynchronize() != cudaSuccess) return nullptr;
-  }
-  d.ready = true;
-  return &d;
+  if (g_dev_ready[dev]) return true;
+  if (cudaFuncSetAttribute(conv_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
+    return false;
+  g_dev_ready[dev] = true;
+  return true;
 }
 
 thread_local odtk_conv_plan_t g_last_plan;
 
-}  // namespace
+void set_stages(ConvParams &p, int BN) {
+  p.nstages = kPipeBytes / ((128 + BN) * p.row_bytes);
+  if (p.nstages > kMaxStages) p.nstages = kMaxStages;
+}
 
-extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
+int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
+           const CUtensorMap &tmB2, cudaStream_t stream) {
+  const int total = p.num_m_tiles * p.num_n_tiles;
+  const int sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
+  const int grid = total < sms ? total : sms;
+  g_last_plan = odtk_conv_plan_t{p.mode, 0, BN, p.num_m_tiles, p.num_n_tiles, p.nstages, 0, 0, 0, 0, 0, 0, p.TH, p.TW, grid, 0};
+  {
+    OdtkProfScope prof(ODTK_PROF_CONV, stream);
+    if (BN == 64) launch_bn<64>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    else          launch_bn<128>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+// odtk_conv2d, plus (mode 0 only) a second operand pair added to the same accumulator: y = x * w^T + x2 * w2^T with
+// x2 [M, c2in], w2 [cout, c2in] (the projected identity of a bottleneck block)
+int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cudaStream_t stream) {
   if (!d || !d->x || !d->w) return ODTK_E_INVALID;
   if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
   if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
@@ -1198,10 +439,9 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
   if (d->out_mode != ODTK_OUT_NHWC_F16 && (d->residual || d->upsample)) return ODTK_E_UNSUPPORTED;
   if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
   if (((uintptr_t)d->x | (uintptr_t)d->w | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15) return ODTK_E_INVALID;
-  cudaStream_t stream = (cudaStream_t)stream_;
-  const DeviceState *dstate = device_state(stream);
-  if (!dstate) return ODTK_E_CUDA;
-  const int g_num_sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
+  if ((d->residual && ((uintptr_t)d->residual & 3)) || (d->upsample && ((uintptr_t)d->upsample & 3))) return ODTK_E_INVALID;
+  if (!device_ready()) return ODTK_E_CUDA;
+  const int sms = odtk_sm_count();
   ConvParams p;
   memset(&p, 0, sizeof p);
   p.N = d->n; p.H = d->h; p.W = d->width; p.Cin = d->cin; p.Cout = d->cout;
@@ -1210,37 +450,6 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
   p.grouped = groups > 1;
   p.row_bytes = 128;
   p.M = (long long)d->n * d->h * d->width;
-  // N tile: whole Cout when it fits 256 columns, else the largest multiple-of-16 divisor-ish tile
-  int BN;
-  if (groups > 1) BN = 64;
-  else if (d->cout <= 256) BN = (d->cout + 15) / 16 * 16;
-  else {
-    int nt = (d->cout + 255) / 256;
-    BN = ((d->cout + nt - 1) / nt + 15) / 16 * 16;
-  }
-  {
-    // few tiles (coarse pyramid levels): narrower N tiles put more SMs to work; each CTA's K loop is as long, its MMAs
-    // proportionally shorter.  Only for NHWC outputs whose Cout splits evenly.
-    static int shrink_on = -1;
-    if (shrink_on < 0) { const char *e = getenv("ODTK_CONV_BN_SHRINK"); shrink_on = e ? atoi(e) : 1; }
-    const int st = d->stride > 1 ? 2 : 1;
-    const long long opix = (long long)d->n * ((d->h - 1) / st + 1) * ((d->width - 1) / st + 1);
-    long long mt = (opix + 127) / 128;
-    if (d->ksize == 3 && st == 1) mt = (long long)d->n * ((d->h + 15) / 16) * ((d->width + 7) / 8);   // halo tiles (upper bound)
-    const int sms = odtk_sm_count();
-    // K-heavy layers on few tiles (FPN pyramid6: 3x3 s2 2048 -> 256 on 13 x 20) are bound by the operand stream from L2,
-    // not by the number of busy SMs: 1 = halve N but run cta_group::2 pairs, 2 = keep N = 256 and pair
-    static int kheavy = -1;
-    if (kheavy < 0) { const char *e = getenv("ODTK_CONV_KHEAVY"); kheavy = e ? atoi(e) : 2; }
-    const bool k_heavy = kheavy && (long long)d->ksize * d->ksize * d->cin >= 8192;
-    while (shrink_on && !(k_heavy && kheavy >= 2) && groups == 1 && d->out_mode == ODTK_OUT_NHWC_F16 && !d->upsample && !d->residual && BN > 64 && (BN % 32) == 0 &&
-           d->cout % (BN / 2) == 0 && mt * ((d->cout + BN - 1) / BN) * 2 <= sms)
-      BN /= 2;
-  }
-  p.BN = BN;
-  p.nstages = kPipeBytes / (kABytes + BN * 128);
-  if (p.nstages > kMaxStages) p.nstages = kMaxStages;
-  p.num_n_tiles = (d->cout + BN - 1) / BN;
   p.bias = d->bias;
   p.residual = (const __half *)d->residual;
   p.upsample = (const __half *)d->upsample;
@@ -1261,17 +470,7 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
     p.cand_pre = (k->thresh > 1e-4f && k->thresh < 0.999f) ? logf(k->thresh / (1.0f - k->thresh)) - 0.05f : -INFINITY;
   }
   if (p.out_mode == ODTK_OUT_NHWC_F16 && (p.ldy % 8)) return ODTK_E_INVALID;
-  if (d->upsample && ((d->h & 1) || (d->width & 1))) return ODTK_E_INVALID;
-  if (d->upsample && BN <= 128) return ODTK_E_UNSUPPORTED;  // the upsample-add epilogue is built for 256-wide tiles
-
-  CUtensorMap tmA, tmB;
-  const uint64_t K = (uint64_t)p.taps * (groups > 1 ? 64 : d->cin);
-  {
-    uint64_t dims[2] = {K, (uint64_t)d->cout};
-    uint64_t str[1] = {K * 2};
-    uint32_t box[2] = {64, (uint32_t)BN};
-    if (!encode_map(&tmB, d->w, 2, dims, str, box)) return ODTK_E_CUDA;
-  }
+  if ((p.residual && (p.ldr & 1)) || (d->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
   const int stride = d->stride > 1 ? d->stride : 1;
   if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
   // strided views: the input / output may be a rectangle of a larger NHWC buffer (a level of the pyramid atlas)
@@ -1281,10 +480,11 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
   if ((x_view || y_view || d->tile_tab) && (d->ksize != 3 || d->residual || d->upsample)) return ODTK_E_UNSUPPORTED;
   if (y_view && d->out_mode != ODTK_OUT_NHWC_F16) return ODTK_E_UNSUPPORTED;
   if (d->tile_tab && (d->tab_tiles <= 0 || stride != 1 || x_view || y_view)) return ODTK_E_INVALID;
-  static int s2_strided_box = -1;
-  if (s2_strided_box < 0) { const char *e = getenv("ODTK_CONV_S2_BOX"); s2_strided_box = e ? atoi(e) : 1; }   // 2: also for even sizes
-  if (stride == 2 && !d->upsample && (((d->h & 1) || (d->width & 1)) ? (s2_strided_box >= 1 || x_view) : (s2_strided_box >= 2 || x_view))) {
-    // stride-2 1x1 / 3x3 (pad ksize/2) on ANY size, im2col-free: one box per tap whose W and H dimensions are
+  if (x2 && (d->ksize != 1 || stride != 1 || c2in <= 0 || c2in % 64 || !w2 || (((uintptr_t)x2 | (uintptr_t)w2) & 15))) return ODTK_E_INVALID;
+
+  CUtensorMap tmA;
+  if (stride == 2 && ((d->h & 1) || (d->width & 1) || x_view)) {
+    // stride-2 1x1 / 3x3 (pad ksize/2) on odd sizes, im2col-free: one box per tap whose W and H dimensions are
     // traversed with element stride 2 (boxDim = 2 * pixels, elementStrides = 2: the TMA unit loads every second
     // pixel); the box origin 2*o + d may be -1 or reach past the edge: zero-filled == padding.
     const int OH = (d->h - 1) / 2 + 1, OW = (d->width - 1) / 2 + 1;
@@ -1294,6 +494,7 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
     p.M = (long long)d->n * OH * OW;
     p.up_h = OH / 2; p.up_w = OW / 2;
     choose_patch(OH, OW, p.TH, p.TW);
+    if (2 * p.TW > 256 || 2 * p.TH > 256) return ODTK_E_UNSUPPORTED;
     p.tiles_h = (OH + p.TH - 1) / p.TH;
     p.tiles_w = (OW + p.TW - 1) / p.TW;
     p.num_m_tiles = d->n * p.tiles_h * p.tiles_w;
@@ -1307,7 +508,7 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
     // stride-2 1x1 / 3x3 (pad ksize/2) on even-sized inputs: 5-D parity-split view of the NHWC tensor
     // {2C (column parity x channel), W/2, 2 (row parity), H/2, N}; out-of-range half-rows/columns
     // (the -1 of the top/left taps) are zero-filled by the TMA unit == padding.
-    if ((d->h & 1) || (d->width & 1) || d->upsample) return ODTK_E_UNSUPPORTED;
+    if (d->upsample) return ODTK_E_UNSUPPORTED;
     const int OH = d->h / 2, OW = d->width / 2;
     p.mode = 3;
     p.H = OH; p.W = OW;
@@ -1331,196 +532,69 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
     if (!encode_map(&tmA, d->x, 2, dims, str, box)) return ODTK_E_CUDA;
   } else {
     p.mode = 1;
-    choose_patch(d->h, d->width, p.TH, p.TW);
-    // halo mode: fixed 16x8 (or transposed 8x16) pixel tiles; used when they waste few more accumulator rows
-    // than the free-form patch (the nine-fold smaller input traffic from L2 pays for up to ~15 %)
-    static int halo_on = -1, halo_boff = 0;
-    if (halo_on < 0) {
-      const char *e = getenv("ODTK_CONV_HALO"); halo_on = e ? atoi(e) : 1;
-      const char *b = getenv("ODTK_CONV_HALO_BOFF"); halo_boff = b ? atoi(b) : 0;   // measured on B200: the swizzle phase follows the absolute address, base offset must stay 0
-    }
-    const double hw = (double)d->h * d->width;
-    const double eff_free = hw / ((double)((d->h + p.TH - 1) / p.TH) * ((d->width + p.TW - 1) / p.TW) * 128.0);
-    const double eff_a = hw / ((double)((d->h + 15) / 16) * ((d->width + 7) / 8) * 128.0);
-    const double eff_b = hw / ((double)((d->h + 7) / 8) * ((d->width + 15) / 16) * 128.0);
-    // row-major tiles keep the fp32 NCHW stores of the head outputs in 32-byte runs: prefer them there
-    // (the candidate-append epilogue writes no dense map either: it takes whichever tiling wastes fewer rows)
-    static int cand_t = -1;
-    if (cand_t < 0) { const char *e = getenv("ODTK_CONV_CAND_T"); cand_t = e ? atoi(e) : 1; }
-    const bool dense_f32 = p.out_mode == ODTK_OUT_NCHW_F32 || p.out_mode == ODTK_OUT_NCHW_F32_SIGMOID || (p.out_mode == ODTK_OUT_CANDIDATES && !cand_t);
-    const bool transposed = !dense_f32 ? eff_b > eff_a + 1e-9 : eff_b > 1.15 * eff_a;
-    const double eff_halo = transposed ? eff_b : eff_a;
-    // narrow N (head outputs with few channels): the per-tap A re-load of mode 1 dominates, take the halo tiles anyway
-    if (d->tile_tab || (halo_on && (eff_halo >= 0.84 * eff_free || (BN <= 64 && eff_halo >= 0.6 * eff_free)) && d->h >= 8 && d->width >= 8)) {
-      p.mode = 4;
-      p.tile_t = (transposed || d->tile_tab) ? 1 : 0;       // atlas tile tables list 8 x 16 (transposed) tiles
-      if (d->tile_tab) { p.tile_tab = (const int4 *)d->tile_tab; p.tab_tiles = d->tab_tiles; }
-      p.halo_boff = halo_boff;
-      p.TH = p.tile_t ? 8 : 16;
-      p.TW = p.tile_t ? 16 : 8;
+    if (d->tile_tab) {   // atlas tile tables list 8 x 16 pixel tiles
+      p.TH = 8; p.TW = 16;
+      p.tile_tab = (const int4 *)d->tile_tab; p.tab_tiles = d->tab_tiles;
+    } else {
+      choose_patch(d->h, d->width, p.TH, p.TW);
     }
     p.tiles_h = (d->h + p.TH - 1) / p.TH;
     p.tiles_w = (d->width + p.TW - 1) / p.TW;
     p.num_m_tiles = d->tile_tab ? d->n * d->tab_tiles : d->n * p.tiles_h * p.tiles_w;
     const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->width, H = (uint64_t)d->h;
-    if (p.mode == 4 && p.tile_t) {   // patch stored [18 columns][16-row pitch][64 ch]: H is the faster box dimension
-      uint64_t dims[4] = {C, H, W, (uint64_t)d->n};
-      uint64_t str[3] = {xW * C * 2, C * 2, xH * xW * C * 2};
-      uint32_t box[4] = {64, 16, 18, 1};
-      if (!encode_map(&tmA, d->x, 4, dims, str, box)) return ODTK_E_CUDA;
-    } else {
-      uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-      uint64_t str[3] = {C * 2, xW * C * 2, xH * xW * C * 2};
-      uint32_t box[4] = {64, (uint32_t)(p.mode == 4 ? 16 : p.TW), (uint32_t)(p.mode == 4 ? 18 : p.TH), 1};
-      if (!encode_map(&tmA, d->x, 4, dims, str, box)) return ODTK_E_CUDA;
-    }
+    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
+    uint64_t str[3] = {C * 2, xW * C * 2, xH * xW * C * 2};
+    uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+    if (!encode_map(&tmA, d->x, 4, dims, str, box)) return ODTK_E_CUDA;
   }
   p.oH = d->y_rows > 0 ? d->y_rows : p.H;
   p.oR = d->y_row_off > 0 ? d->y_row_off : 0;
   p.oW = d->y_width > 0 ? d->y_width : p.W;
   if ((long long)d->n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
-  // wide 1x1 outputs (the memory-bound layers): the epilogue hands its staged slabs to the TMA unit
-  CUtensorMap tmC = tmB;
-  static int tma_store_on = -1;
-  if (tma_store_on < 0) { const char *e = getenv("ODTK_CONV_TMA_STORE"); tma_store_on = e ? atoi(e) : 1; }
-  if (tma_store_on && p.mode == 0 && p.out_mode == ODTK_OUT_NHWC_F16 && BN > 128 && (BN % 64) == 0 && d->cout % 64 == 0) {   // 64-column store boxes must not reach into the next N tile
-    uint64_t dims[2] = {(uint64_t)p.ldy, (uint64_t)p.M};
-    uint64_t str[1] = {(uint64_t)p.ldy * 2};
-    uint32_t box[2] = {64, 32};
-    if (encode_map(&tmC, d->y, 2, dims, str, box)) p.tma_store = 1;
-  }
-  CUtensorMap tmOnes = tmB, tmBias = tmB;
-  static int bias_mma_on = -1;
-  if (bias_mma_on < 0) { const char *e = getenv("ODTK_CONV_BIAS_MMA"); bias_mma_on = e ? atoi(e) : 1; }
-  static int deep_bias_epi = -1;
-  if (deep_bias_epi < 0) { const char *e = getenv("ODTK_CONV_DEEP_BIAS_EPI"); deep_bias_epi = e ? atoi(e) : 1; }   // measured: 512 -> 2048 +res 88.5 -> 81.6 us, others within noise
-  const bool deep_layer = d->ksize == 1 && stride == 1 && BN == 256 && d->cin >= 256 && p.M <= 160000 && p.out_mode == ODTK_OUT_NHWC_F16 && !d->upsample;
-  if (bias_mma_on && d->bias_op && d->bias && !(deep_bias_epi && deep_layer)) {
-    const void *ones = dstate->ones;
-    uint64_t dimsO[2] = {64, 128}, strO[1] = {128};
-    uint32_t boxO[2] = {64, 128};
-    uint64_t dimsB[2] = {64, (uint64_t)d->cout}, strB[1] = {128};
-    uint32_t boxB[2] = {64, (uint32_t)BN};
-    if (ones && encode_map(&tmOnes, ones, 2, dimsO, strO, boxO) && encode_map(&tmBias, d->bias_op, 2, dimsB, strB, boxB))
-      p.bias_mma = 1;
-  }
-  // 2-CTA clusters with weight multicast: the compute-bound 256-wide layers with enough tiles for every cluster
-  static int cluster_on = -1;
-  if (cluster_on < 0) { const char *e = getenv("ODTK_CONV_CLUSTER"); cluster_on = e ? atoi(e) : 2; }   // 0 off, 1 multicast, 2 cta_group::2
-  static int cluster_1x1 = -1;
-  if (cluster_1x1 < 0) { const char *e = getenv("ODTK_CONV_CLUSTER_1X1"); cluster_1x1 = e ? atoi(e) : 0; }   // measured: 1x1 layers are faster unclustered with the TMA-store epilogue (+2.6 % per step)
-  static int cluster_res = -1;
-  if (cluster_res < 0) { const char *e = getenv("ODTK_CONV_CLUSTER_RES"); cluster_res = e ? atoi(e) : 0; }   // 1x1 + residual layers as multicast pairs (weights read once per pair from L2)
-  const bool res_pair = cluster_res && d->residual && d->ksize == 1 && stride == 1 && BN == 256 && d->cout % 256 == 0;
-  static int two_narrow = -1;
-  if (two_narrow < 0) { const char *e = getenv("ODTK_CONV_TWO_NARROW"); two_narrow = e ? atoi(e) : 1; }   // cta_group::2 pairs for narrow fp32-output head layers (halved weight stream per CTA)
-  const bool narrow_pair = two_narrow && cluster_on >= 2 && p.mode == 4 && p.out_mode != ODTK_OUT_NHWC_F16 && BN >= 32 && BN <= 128;
-  // deep 1x1 layers (few pixels, long K): a 128 x 256 tile needs 48 KB of operands per 512 tensor-core cycles -- more than
-  // the L2 -> SM fabric delivers to 148 SMs at once; as cta_group::2 pairs (256 x 256 per pair, each CTA loads half of the
-  // weight block) the same work moves a third fewer bytes.  Big-M layers are HBM-bound and stay unclustered (measured).
-  static int deep_1x1 = -1;
-  if (deep_1x1 < 0) { const char *e = getenv("ODTK_CONV_DEEP_1X1"); deep_1x1 = e ? atoi(e) : 1; }
-  const bool deep_pair = deep_1x1 && cluster_on >= 2 && p.mode == 0 && BN == 256 && d->cin >= 256 && p.M <= 160000 &&
-                         p.out_mode == ODTK_OUT_NHWC_F16 && !d->upsample;
-  // 128-wide 3x3 layers (ResNet layer2's conv2): a 128 x 128 tile streams 16 KB of weights per 256 tensor-core cycles --
-  // as cta_group::2 pairs each CTA fetches half of that
-  static int two_128 = -1;
-  if (two_128 < 0) { const char *e = getenv("ODTK_CONV_TWO_128"); two_128 = e ? atoi(e) : 1; }
-  const bool mid_pair = two_128 && cluster_on >= 2 && d->ksize == 3 && BN == 128 && p.out_mode == ODTK_OUT_NHWC_F16 && groups == 1;
-  static int kheavy2 = -1;
-  if (kheavy2 < 0) { const char *e = getenv("ODTK_CONV_KHEAVY"); kheavy2 = e ? atoi(e) : 2; }
-  const bool k_heavy2 = kheavy2 && (long long)d->ksize * d->ksize * d->cin >= 8192 && cluster_on >= 2 && BN >= 128;
-  if (cluster_on && (BN > 128 || narrow_pair || mid_pair || k_heavy2) && !d->upsample && (!d->residual || res_pair || deep_pair) &&
-      (cluster_1x1 || d->ksize == 3 || res_pair || deep_pair) &&
-      (p.mode == 0 || p.mode == 1 || p.mode == 3 || (p.mode == 4 && cluster_on >= 2)) &&
-      ((p.num_m_tiles + 1) / 2) * p.num_n_tiles >= (k_heavy2 ? g_num_sms / 8 : g_num_sms / 2) && (BN / 2) % 8 == 0) {
-    const uint64_t Kw = (uint64_t)p.taps * d->cin;
-    uint64_t dims[2] = {Kw, (uint64_t)d->cout}, str[1] = {Kw * 2};
-    uint32_t box[2] = {64, (uint32_t)(BN / 2)};
-    bool ok = encode_map(&tmB, d->w, 2, dims, str, box);
-    if (ok && p.bias_mma) {
-      uint64_t dimsB[2] = {64, (uint64_t)d->cout}, strB[1] = {128};
-      uint32_t boxB[2] = {64, (uint32_t)(BN / 2)};
-      ok = encode_map(&tmBias, d->bias_op, 2, dimsB, strB, boxB);
-    }
-    if (ok) {
-      p.cluster2 = (cluster_on >= 2 && !res_pair) ? 2 : 1;   // residual pairs: cta_group::1 MMAs, multicast weights
-      if (!(res_pair && cluster_res >= 2) && !(deep_pair && deep_1x1 >= 1)) p.tma_store = 0;
-      if (p.cluster2 == 2) { p.nstages = kPipeBytes / (kABytes + BN * 64); if (p.nstages > kMaxStages) p.nstages = kMaxStages; }
-    }
-    else return ODTK_E_CUDA;
-  }
-  // residual add on the tensor core (D += I * R): wide 1x1 residual layers (bottleneck conv3)
-  CUtensorMap tmRes = tmB, tmIdent = tmB;
-  static int res_pipe_on = -1;
-  if (res_pipe_on < 0) { const char *e = getenv("ODTK_CONV_RES_PIPE"); res_pipe_on = e ? atoi(e) : 1; }
-  if (res_pipe_on && d->residual && p.mode == 0 && p.out_mode == ODTK_OUT_NHWC_F16 && p.cluster2 != 1 && (BN % 64) == 0 &&
-      d->cout % 64 == 0 && (p.ldr % 8) == 0 && (((uintptr_t)d->residual) & 15) == 0) {
-    uint64_t dimsR[2] = {(uint64_t)p.ldr, (uint64_t)p.M}, strR[1] = {(uint64_t)p.ldr * 2};
-    uint32_t boxR[2] = {64, 128};
-    uint64_t dimsI[2] = {64, 64}, strI[1] = {128};
-    uint32_t boxI[2] = {64, (uint32_t)(p.cluster2 == 2 ? 32 : 64)};   // cta_group::2: each CTA holds half of the identity's rows
-    if (encode_map(&tmRes, d->residual, 2, dimsR, strR, boxR) && encode_map(&tmIdent, dstate->ident64, 2, dimsI, strI, boxI))
-      p.res_pipe = 1;
-  }
-  static int res_mma_on = -1;
-  if (res_mma_on < 0) { const char *e = getenv("ODTK_CONV_RES_MMA"); res_mma_on = e ? atoi(e) : 1; }
-  if (res_mma_on && !p.res_pipe && d->residual && p.mode == 0 && p.out_mode == ODTK_OUT_NHWC_F16 && BN == 256 && d->cout % 256 == 0 &&
-      (p.ldr % 8) == 0 && (((uintptr_t)d->residual) & 15) == 0) {
-    const void *ident = dstate->ident;
-    uint64_t dimsR[2] = {(uint64_t)p.ldr, (uint64_t)p.M}, strR[1] = {(uint64_t)p.ldr * 2};
-    uint32_t boxR[2] = {64, 128};
-    uint64_t dimsI[2] = {128, 128}, strI[1] = {256};
-    uint32_t boxI[2] = {64, 128};
-    if (ident && encode_map(&tmRes, d->residual, 2, dimsR, strR, boxR) && encode_map(&tmIdent, ident, 2, dimsI, strI, boxI)) {
-      p.res_mma = 1;
-      p.nstages = 2;   // the rest of the pipeline region holds the residual tile (64 KB) and the identity (32 KB)
-    }
-  }
-  // FPN upsample-add on the tensor core (D += U * P): 1x1 lateral layers whose rows split into 16-pixel groups
-  static int up_mma_on = -1;
-  if (up_mma_on < 0) { const char *e = getenv("ODTK_CONV_UP_MMA"); up_mma_on = e ? atoi(e) : 1; }
-  if (up_mma_on && d->upsample && !d->residual && p.mode == 0 && p.out_mode == ODTK_OUT_NHWC_F16 && BN == 256 &&
-      d->cout % 256 == 0 && d->width % 16 == 0 && !p.cluster2 && (((uintptr_t)d->upsample) & 15) == 0) {
-    const uint64_t msrc = (uint64_t)d->n * p.up_h * p.up_w;
-    uint64_t dimsR[2] = {(uint64_t)d->cout, msrc}, strR[1] = {(uint64_t)d->cout * 2};
-    uint32_t boxR[2] = {64, 8};
-    uint64_t dimsU[2] = {64, 128}, strU[1] = {128};
-    uint32_t boxU[2] = {64, 128};
-    if (encode_map(&tmRes, d->upsample, 2, dimsR, strR, boxR) && encode_map(&tmIdent, dstate->upsel, 2, dimsU, strU, boxU)) {
-      p.up_mma = 1;
-      p.nstages = 3;   // the fourth stage's 48 KB hold the source-pixel tile (32 KB) and U (16 KB)
-    }
-  }
-  if (p.mode == 4) {   // pipeline region: patches | ones tile (bias block) | weight-block stages
-    const int bstage = (p.cluster2 == 2 ? BN / 2 : BN) * 128;
-    const int fixed = p.bias_mma ? kABytes : 0;
-    static int resident_on = -1;
-    if (resident_on < 0) { const char *e = getenv("ODTK_CONV_RESIDENT_W"); resident_on = e ? atoi(e) : 1; }
-    const int nblocks = 9 * p.kblocks_per_tap + (p.bias_mma ? 1 : 0);
-    if (resident_on && !p.cluster2 && p.num_n_tiles == 1 && 2 * kPatchBytes + fixed + nblocks * bstage <= kPipeBytes) {
-      p.b_resident = 1;
-      p.npatch = (3 * kPatchBytes + fixed + nblocks * bstage <= kPipeBytes) ? 3 : 2;
-      p.nstages = 2;   // unused
-    } else {
-    p.npatch = (kPipeBytes - fixed - 3 * kPatchBytes) / bstage >= 6 ? 3 : 2;
-    p.nstages = (kPipeBytes - fixed - p.npatch * kPatchBytes) / bstage;
-    }
-    if (p.nstages > kMaxStages) p.nstages = kMaxStages;
-    if (p.nstages < 2) return ODTK_E_UNSUPPORTED;
-  }
-  static int max_stages = -1;
-  if (max_stages < 0) { const char *e = getenv("ODTK_CONV_MAX_STAGES"); max_stages = e ? atoi(e) : kMaxStages; if (max_stages < 2 || max_stages > kMaxStages) max_stages = kMaxStages; }
-  if (p.nstages > max_stages) p.nstages = max_stages;
-  const int total = p.num_m_tiles * p.num_n_tiles;
-  const int grid = total < g_num_sms ? total : g_num_sms;
-  g_last_plan = odtk_conv_plan_t{p.mode, p.cluster2, p.BN, p.num_m_tiles, p.num_n_tiles, p.nstages, p.npatch, p.tile_t,
-                                 p.b_resident, p.bias_mma, p.res_mma + 2 * p.res_pipe, p.tma_store, p.TH, p.TW, grid, p.up_mma};
+  // N tile: 64 or 128 output channels.  128 halves the A-operand traffic; 64 when Cout is narrow, for grouped convs (one
+  // 64-channel chunk per tile), or when 128-wide tiles would leave SMs idle.
+  int BN = (groups > 1 || d->cout <= 64) ? 64 : 128;
+  if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
+  p.num_n_tiles = (d->cout + BN - 1) / BN;
+  set_stages(p, BN);
+  CUtensorMap tmB, tmA2, tmB2;
+  const uint64_t K = (uint64_t)p.taps * (groups > 1 ? 64 : d->cin);
   {
-    OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    launch_conv(grid, stream, tmA, tmB, tmC, tmOnes, tmBias, tmRes, tmIdent, p);
+    uint64_t dims[2] = {K, (uint64_t)d->cout};
+    uint64_t str[1] = {K * 2};
+    uint32_t box[2] = {64, (uint32_t)BN};
+    if (!encode_map(&tmB, d->w, 2, dims, str, box)) return ODTK_E_CUDA;
   }
-  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+  tmA2 = tmA; tmB2 = tmB;
+  if (x2) {
+    p.kblocks2 = c2in / 64;
+    uint64_t dims[2] = {(uint64_t)c2in, (uint64_t)p.M}, str[1] = {(uint64_t)c2in * 2};
+    uint32_t box[2] = {64, 128};
+    uint64_t dimsW[2] = {(uint64_t)c2in, (uint64_t)d->cout}, strW[1] = {(uint64_t)c2in * 2};
+    uint32_t boxW[2] = {64, (uint32_t)BN};
+    if (!encode_map(&tmA2, x2, 2, dims, str, box) || !encode_map(&tmB2, w2, 2, dimsW, strW, boxW)) return ODTK_E_CUDA;
+  }
+  return launch(p, BN, tmA, tmB, tmA2, tmB2, stream);
+}
+
+// bias operand: [cout, 64] fp16 with (hi, lo, 0, ...): hi + lo == bias to 2^-22 relative
+__global__ void pack_bias_kernel(const float *bias, __half *out, int cout) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cout * 64; i += gridDim.x * blockDim.x) {
+    const int c = i >> 6, k = i & 63;
+    float v = 0.0f;
+    if (k < 2) {
+      const float b = bias[c];
+      const float hi = __half2float(__float2half_rn(b));
+      v = (k == 0) ? hi : b - hi;
+    }
+    out[i] = __float2half_rn(v);
+  }
+}
+
+}  // namespace
+
+extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
+  return conv_run(d, nullptr, nullptr, 0, (cudaStream_t)stream_);
 }
 
 // ResNet stem: 7x7 stride-2 pad-3 convolution of the RGB image, im2col-free.  `xp` is the image
@@ -1528,16 +602,14 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
 // output pixels (oh, ow..) is the 8-pixel x 4-channel window starting at padded pixel (2*oh + r, 2*ow):
 // 64 contiguous bytes, consecutive output pixels 16 bytes apart -- an OVERLAPPING-window 5-D tensor map
 // {32 elements, OW (16 B), 7 rows (one padded row), OH (two padded rows), N}.  K = 7 blocks of 32
-// (SWIZZLE_64B), weights packed [64, 7*32] with k = r*32 + s*4 + c (zero for s = 7 or c = 3).
+// (SWIZZLE_64B), weights packed [cout, 7*32] with k = r*32 + s*4 + c (zero for s = 7 or c = 3).
 extern "C" int odtk_stem_conv(const void *xp, const void *w, const float *bias, void *y, int n, int h, int width,
                               int cout, int relu, odtk_stream_t stream_) {
   if (!xp || !w || !y || n <= 0 || h <= 0 || width <= 0) return ODTK_E_INVALID;
-  if ((h & 1) || (width & 1) || cout % 16 || cout > 256) return ODTK_E_UNSUPPORTED;
+  if ((h & 1) || (width & 1) || cout % 16 || cout > 128) return ODTK_E_UNSUPPORTED;
   if (((uintptr_t)xp | (uintptr_t)w | (uintptr_t)y) & 15) return ODTK_E_INVALID;
   cudaStream_t stream = (cudaStream_t)stream_;
-  const DeviceState *dstate = device_state(stream);
-  if (!dstate) return ODTK_E_CUDA;
-  const int g_num_sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
+  if (!device_ready()) return ODTK_E_CUDA;
   const int OH = h / 2, OW = width / 2, HP = h + 6, WP = width + 8;
   if ((long long)n * OH * OW >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
   ConvParams p;
@@ -1547,41 +619,17 @@ extern "C" int odtk_stem_conv(const void *xp, const void *w, const float *bias, 
   p.kw = 1; p.taps = 7; p.pad = 0; p.kblocks_per_tap = 1;
   p.row_bytes = 64;
   p.M = (long long)n * OH * OW;
-  p.BN = cout;
+  const int BN = cout <= 64 ? 64 : 128;
   p.num_n_tiles = 1;
-  p.nstages = kPipeBytes / (kABytes + p.BN * 128);
-  if (p.nstages > kMaxStages) p.nstages = kMaxStages;
+  set_stages(p, BN);
   p.bias = bias; p.out = y; p.relu = relu; p.out_mode = ODTK_OUT_NHWC_F16; p.ldy = cout; p.ldr = cout;
-  p.oH = OH; p.oR = 0; p.oW = OW;   // dense output (the epilogue addresses pixels through the output view's geometry)
+  p.oH = OH; p.oR = 0; p.oW = OW;
   choose_patch(OH, OW, p.TH, p.TW);
-  // raw-window mode: 16 x 8 output-pixel tiles whose A operand is an un-swizzled view of the padded image patch
-  static int stem_raw = -1, stem_swap = 0;
-  if (stem_raw < 0) {
-    const char *e = getenv("ODTK_STEM_RAW"); stem_raw = e ? atoi(e) : 1;
-    const char *f = getenv("ODTK_STEM_RAW_SWAP"); stem_swap = f ? atoi(f) : 0;   // diagnostic: swap LBO / SBO
-  }
-  const bool raw = stem_raw && cout <= 128 && kMaxStages * kStemPatchSlot + 7 * cout * 64 <= kPipeBytes;
-  if (raw) { p.mode = 5; p.TH = 16; p.TW = 8; p.nstages = kMaxStages; p.halo_boff = stem_swap; }
   p.tiles_h = (OH + p.TH - 1) / p.TH;
   p.tiles_w = (OW + p.TW - 1) / p.TW;
   p.num_m_tiles = n * p.tiles_h * p.tiles_w;
   CUtensorMap tmA, tmB;
-  static int stem_rows = -1;
-  if (stem_rows < 0) { const char *e = getenv("ODTK_STEM_ROWS"); stem_rows = e ? atoi(e) : 1; }
-  if (raw && stem_rows) {
-    // padded image [n, HP, WP, 4] as rows of WP*4 elements: patch = 37 rows x 96 elements (192 B) -- 37 TMA rows per tile
-    p.stem_rows = 1;
-    uint64_t dims[3] = {(uint64_t)WP * 4, (uint64_t)HP, (uint64_t)n};
-    uint64_t str[2] = {(uint64_t)WP * 8, (uint64_t)HP * WP * 8};
-    uint32_t box[3] = {kStemPatchW * 4, 37, 1};
-    if (!encode_map(&tmA, xp, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE)) return ODTK_E_UNSUPPORTED;
-  } else if (raw) {
-    // padded image [n, HP, WP, 4] viewed as 16-byte pixel pairs: {8 el, WP/2, HP, n}; patch = 12 pairs x 37 rows
-    uint64_t dims[4] = {8, (uint64_t)WP / 2, (uint64_t)HP, (uint64_t)n};
-    uint64_t str[3] = {16, (uint64_t)WP * 8, (uint64_t)HP * WP * 8};
-    uint32_t box[4] = {8, kStemPatchW / 2, 37, 1};
-    if (!encode_map(&tmA, xp, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE)) return ODTK_E_UNSUPPORTED;
-  } else {
+  {
     uint64_t dims[5] = {32, (uint64_t)OW, 7, (uint64_t)OH, (uint64_t)n};
     uint64_t str[4] = {16, (uint64_t)WP * 8, (uint64_t)WP * 16, (uint64_t)HP * WP * 8};
     uint32_t box[5] = {32, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
@@ -1590,20 +638,13 @@ extern "C" int odtk_stem_conv(const void *xp, const void *w, const float *bias, 
   {
     uint64_t dims[2] = {224, (uint64_t)cout};
     uint64_t str[1] = {224 * 2};
-    uint32_t box[2] = {32, (uint32_t)cout};
+    uint32_t box[2] = {32, (uint32_t)BN};
     if (!encode_map(&tmB, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B)) return ODTK_E_CUDA;
   }
-  const int total = p.num_m_tiles;
-  const int grid = total < g_num_sms ? total : g_num_sms;
-  g_last_plan = odtk_conv_plan_t{p.mode, 0, p.BN, p.num_m_tiles, 1, p.nstages, 0, 0, 0, 0, 0, 0, p.TH, p.TW, grid, 0};
-  {
-    OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    launch_conv(grid, stream, tmA, tmB, tmB, tmB, tmB, tmB, tmB, p);
-  }
-  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+  return launch(p, BN, tmA, tmB, tmA, tmB, stream);
 }
 
-// Pack a fp32 bias vector into the [cout, 64] fp16 operand of the bias K block (see odtk_conv_t.bias_op).
+// Pack a fp32 bias vector into the [cout, 64] fp16 (hi, lo) layout (see odtk_conv_t.bias_op).
 extern "C" int odtk_conv_pack_bias(const float *bias, void *out, int cout, odtk_stream_t stream_) {
   if (!bias || !out || cout <= 0) return ODTK_E_INVALID;
   pack_bias_kernel<<<(cout * 64 + 255) / 256, 256, 0, (cudaStream_t)stream_>>>(bias, (__half *)out, cout);

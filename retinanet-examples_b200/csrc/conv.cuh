@@ -1,14 +1,25 @@
 // conv.cuh -- kernel-side parameter block of conv_gemm_kernel (see conv.cu).
 #pragma once
+#include <cuda.h>
 #include <cuda_fp16.h>
+#include <stdint.h>
+
+// Host helpers shared by the TMA kernels (conv.cu, bottleneck.cu, stem.cu).
+// Encode a tiled fp16 tensor map (cached per base pointer and geometry); false if the driver rejects it.
+bool encode_map(CUtensorMap *m, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
+                const uint32_t *box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, const uint32_t *elem_strides = nullptr);
+// The spatial patch (TW x TH <= 128 pixels) that wastes the fewest accumulator rows on an H x W image.
+void choose_patch(int H, int W, int &TH, int &TW);
 
 struct ConvParams {
-  int mode;             // 0: rows of a [M, Cin] matrix (1x1 / lowered conv); 1: spatial patches (3x3, pad 1);
-                        // 2: 7x7 stride-2 stem over a zero-padded NHWC4 image (overlapping-window 5-D map)
+  int mode;             // 0: rows of a [M, Cin] matrix (1x1 / lowered conv); 1: spatial patch, one shifted box per tap
+                        // (3x3 pad 1, or stride 2 with element-strided boxes when s2); 2: 7x7 stride-2 stem over a
+                        // zero-padded NHWC4 image (overlapping-window 5-D map); 3: stride 2 on even sizes (parity-split view)
   int N, H, W, Cin, Cout;
-  int taps, kw, pad;    // 1 / 9 taps
-  int TH, TW, tiles_h, tiles_w;   // mode 1: patch and patches per image
-  int num_m_tiles, num_n_tiles, BN, kblocks_per_tap;
+  int taps, kw, pad;    // 1 / 7 / 9 taps
+  int TH, TW, tiles_h, tiles_w;   // modes 1-3: patch and patches per image
+  int num_m_tiles, num_n_tiles, kblocks_per_tap;
+  int kblocks2;         // mode 0: extra K blocks from a second operand pair (A2 [M, 64 * kblocks2], B2 [Cout, 64 * kblocks2])
   long long M;          // N*H*W
   const float *bias;    // [Cout] fp32 (folded BatchNorm shift / conv bias) or NULL
   const __half *residual;  // NHWC fp16, row stride ldr, or NULL
@@ -16,26 +27,12 @@ struct ConvParams {
   void *out;
   int relu, out_mode, ldy, ldr, up_h, up_w;
   int row_bytes;        // bytes of one K block row in shared memory: 128 (SWIZZLE_128B) or 64 (SWIZZLE_64B, stem)
-  int cluster2;         // launched as 2-CTA clusters: each CTA loads half of the weight tile and multicasts it
-  int res_mma;          // the residual is added by the tensor core: D += I * R (mode 0, BN = 256)
-  int res_pipe;         // the residual is added as BN / 64 extra K blocks (A = residual chunk, B = 64 x 64 identity, N = 64 MMAs)
-  int bias_mma;         // the bias is added by one extra K block on the tensor core (A = ones, B = bias hi/lo)
-  int tma_store;        // epilogue hands 32x64 slabs to cp.async.bulk.tensor stores (mode 0, BN > 128)
-  int nstages;          // pipeline stages that fit: (16 KB + BN*128 B) each
-  // mode 4 ("halo"): 3x3 stride-1 conv whose input patch (18 x 16-pixel pitch x 64 channels, 36 KB) is loaded ONCE per
-  // 64-channel chunk; the nine taps are nine shifted shared-memory views of it (UMMA descriptors, 2048-byte group stride)
-  int npatch;           // patch buffers (2 or 3); the weight-block stages follow them in the pipeline region
-  int tile_t;           // 0: tile = 16 rows x 8 columns of pixels (accumulator row m -> (m / 8, m % 8));
-                        // 1: transposed, 8 rows x 16 columns (m -> (m % 8, m / 8)), patch stored column-major
-  int b_resident;       // halo mode: all weight blocks (+ the bias block) fit next to the patches and are loaded once per CTA
-  int halo_boff;        // put (start address >> 7) & 7 into the descriptor's base-offset field
-  int up_mma;           // FPN upsample-add on the tensor core: D += U * P (U = constant 128 x 64 nearest-upsample selection matrix)
-  const int4 *tile_tab;   // mode 4 over a pyramid atlas: per tile of one image (h0, w0, first row / column not to write)
+  int nstages;          // pipeline stages that fit: (128 + BN) * row_bytes each
+  const int4 *tile_tab;   // mode 1 over a pyramid atlas: per tile of one image (h0, w0, first row / column not to write)
   int tab_tiles;          // tiles per image in tile_tab
   int oH, oR, oW;         // NHWC output placement: pixel (img, h, w) is written at ((img * oH + oR + h) * oW + w) * ldy
   int grouped;          // grouped conv: kblocks_per_tap == 1 and the A channel coordinate is the N tile's own chunk (n0)
   int s2;               // mode 1: input pixel = 2 * output pixel + tap offset (element-strided TMA boxes), else 0
-  int stem_rows;        // mode 5: the patch is loaded as 37 rows of 192 B (3-D map) instead of 444 pieces of 16 B (4-D map)
   // out_mode ODTK_OUT_CANDIDATES: the decode workspace of this pyramid level (decode.cu)
   int *cand_counts;          // [N]
   unsigned *cand_hist;       // [N, cand_hist_bins]

@@ -1,4 +1,4 @@
-// decode.cu -- score filter + exact top-n + anchor box decode for sm_100a.
+// decode.cu -- score filter + exact top-n + anchor box decode for sm_90a.
 //
 // Replaces odtk::cuda::decode / decode_rotate (reference csrc/cuda/decode.cu:44-171,
 // decode_rotate.cu:42-179), which run, PER IMAGE and PER LEVEL with a host sync in between,
@@ -610,11 +610,11 @@ static long long decode_levels_impl(int mode, odtk_cand_sink_t *sinks, int batch
   static int ctas_per_sm = 0;
   if (!ctas_per_sm) {
     const char *e = getenv("ODTK_FILTER_CTAS_PER_SM");
-    ctas_per_sm = e ? atoi(e) : 12;  // measured on B200: 4 -> 3.7, 6 -> 4.67, 12 -> 4.79 TB/s
+    ctas_per_sm = e ? atoi(e) : 12;  // CTAs per SM of the streaming score filter
     if (ctas_per_sm < 1) ctas_per_sm = 12;
   }
   static int filter_vec = 0;
-  if (!filter_vec) { const char *e = getenv("ODTK_FILTER_VEC"); filter_vec = (e && atoi(e) == 8) ? 8 : 4; }   // measured on B200: 4 -> 4.8 TB/s, 8 -> 3.5 TB/s (100 registers: half the resident warps)
+  if (!filter_vec) { const char *e = getenv("ODTK_FILTER_VEC"); filter_vec = (e && atoi(e) == 8) ? 8 : 4; }   // float4 loads (8-wide: 100 registers, half the resident warps)
   static int filter_bulk = -1;
   if (filter_bulk < 0) { const char *e = getenv("ODTK_FILTER_BULK"); filter_bulk = e ? atoi(e) : 0; }
   bool bulk_ok = filter_bulk != 0;

@@ -1,4 +1,4 @@
-// iou.cu -- polygon IoU of rotated target boxes against rotated anchors for sm_100a.
+// iou.cu -- polygon IoU of rotated target boxes against rotated anchors for sm_90a.
 //
 // Replaces odtk::cuda::iou + iou_cuda_kernel (reference csrc/cuda/nms_iou.cu:324-387, declared nms_iou.h:33-35), the
 // kernel behind odtk._C.iou (csrc/extensions.cpp:47-67) that snap_to_anchors_rotated (odtk/box.py:218) uses to match

@@ -1,4 +1,4 @@
-// loss.cu -- fused focal loss forward + backward for sm_100a (HBM-bound, one pass).
+// loss.cu -- fused focal loss forward + backward for sm_90a (HBM-bound, one pass).
 //
 // Replaces FocalLoss.forward (reference odtk/loss.py:13-18) as used by Model._compute_loss
 // (odtk/model.py:195-199): sigmoid, BCE-with-logits, alpha_t, p_t, the modulating factor, the

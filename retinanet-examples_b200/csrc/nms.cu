@@ -1,4 +1,4 @@
-// nms.cu -- batched per-image greedy NMS (axis-aligned and rotated) for sm_100a.
+// nms.cu -- batched per-image greedy NMS (axis-aligned and rotated) for sm_90a.
 //
 // Replaces odtk::cuda::nms + nms_kernel (reference csrc/cuda/nms.cu:44-160) and
 // odtk::cuda::nms_rotate + nms_rotate_kernel (csrc/cuda/nms_iou.cu:114-322).  The
@@ -14,8 +14,7 @@
 //      for all pairs at once into a 128 x 128 bit matrix (class gate first, IEEE division, +1
 //      widths), and one warp resolves the chunk sequentially with bit operations only.  The walk
 //      stops at detections_per_im keepers -- exact, because the output is the first D entries of
-//      (kept..., suppressed...) and later candidates never change earlier decisions (SURVEY.md
-//      section 8 note N1); with the BASELINE workload one chunk is enough;
+//      (kept..., suppressed...) and later candidates never change earlier decisions; with the BASELINE workload one chunk is enough;
 //   3. if fewer than D were kept the tail is the first suppressed candidates in rank order
 //      with score 0 and their boxes/classes, exactly what the reference's second sort
 //      leaves there (nms.cu:146-156).

@@ -1,277 +1,153 @@
-// stem.cu -- ResNet stem in ONE kernel: 7x7 stride-2 convolution (+ folded BatchNorm + ReLU) and the 3x3 stride-2
-// max-pool that follows it (torchvision resnet.py: conv1 / bn1 / relu / maxpool; odtk/backbones/resnet.py:25-28),
-// on the 5th-gen tensor cores.  The [N, H/2, W/2, 64] stem activation -- the largest tensor of the whole network,
-// 1 GB per 32 images at 800 x 1280 -- never exists in HBM: only the pooled [N, H/4, W/4, 64] tensor is written.
+// stem.cu -- ResNet stem fused on the Hopper tensor cores (sm_90a): 7x7 stride-2 pad-3 convolution + bias (folded
+// BatchNorm) + ReLU + 3x3 stride-2 pad-1 max-pool in ONE kernel; the [n, h/2, w/2, 64] stem activation is never written.
 //
-// Tile = 7 x 7 pooled pixels.  They need the 15 x 15 stem pixels (2*ph0 - 1 .. 2*ph0 + 13) around them; the kernel
-// computes 16 x 16 (two M = 128 accumulators of 16 rows x 8 columns each; ~30 % of the stem FLOPs are recomputed
-// halo, the stem is 1 % of the network) from ONE TMA load of the zero-padded NHWC4 image patch (37 rows x 320 B).
-// As in conv.cu's raw-window mode the tensor core reads its A operand straight out of that patch: an un-swizzled
-// K-major view whose 16-byte row pitch is the distance between the windows of neighbouring output pixels (stride 2 x
-// 4 channels x 2 B), LBO = 16 B (the windows overlap in place), SBO = two patch rows.  Weights (28 KB) stay resident.
-//
-//   warp 0  TMA producer: one 3-D box per tile (negative / past-the-edge coordinates are zero-filled).
-//   warp 1  MMA issuer: 2 halves x 7 filter rows x 2 K steps = 28 tcgen05.mma (M128 N64 K16) per tile.
-//   warp 2  TMEM allocator (2 accumulator buffers of 128 columns).
-//   warps 4-11 epilogue: tcgen05.ld -> + bias, ReLU, fp16 -> XOR-swizzled staging tile [16 x 16 pixels][64 ch] in
-//           shared memory (stem pixels outside the image are written as 0 == the pool's padding, exact after ReLU)
-//           -> named barrier -> 3x3/2 max over the staging tile -> coalesced 128-byte stores of the pooled pixels.
+// A CTA tile is 5 x 5 pooled pixels.  Their 3x3 windows cover an 11 x 11 patch of stem pixels (121 accumulator rows,
+// starting one stem row / column before 2 * the pooled origin), computed like odtk_stem_conv computes them: the A
+// operand of filter row r is the overlapping-window 5-D tensor map of the zero-padded NHWC4 image (K = 32 per row,
+// SWIZZLE_64B), 7 K blocks per tile, wgmma m64n64k16 with fp32 accumulation.  The epilogue rounds bias + accumulator
+// to fp16 and applies ReLU exactly as the convolution epilogue does, stages the 11 x 11 x 64 tile in shared memory and
+// pools it; stem pixels outside the image (the patch's first row / column at the top / left edge, its end at the
+// bottom / right) are left out of the maximum, which is max-pool padding.  Bit-identical to odtk_stem_conv followed by
+// odtk_maxpool3x3s2.
+//   warpgroup 0     TMA producer (one thread): image patch + weight block per filter row, through an mbarrier ring.
+//   warpgroups 1-2  64 of the 121 patch rows each: wgmma, epilogue; then all 256 threads pool.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
 
+#include <mutex>
+
 #include "common.cuh"
+#include "conv.cuh"
 #include "prof.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
-constexpr int kStages = 6;
-constexpr int kPatchCols = 40;                       // padded pixels per patch row: 2*16 + 6, rounded up to 16-byte pairs
-constexpr int kRowBytes = kPatchCols * 8;            // 320
-constexpr int kPatchRows = 37;                       // 2*16 + 5
-constexpr int kPatchBytes = kPatchRows * kRowBytes;  // 11840
-constexpr int kPatchSlot = 12288;
+constexpr int kThreads = 384;
+constexpr int kPool = 5;                    // pooled pixels per tile side
+constexpr int kSide = 2 * kPool + 1;        // stem pixels per patch side: 11
+constexpr int kRows = kSide * kSide;        // 121 accumulator rows
 constexpr int kCout = 64;
-constexpr int kWBytes = 7 * kCout * 64;              // 7 filter rows x [64 cout x 32 k] fp16 (SWIZZLE_64B rows)
-constexpr int kStageTile = 256 * 128;                // staging: 16 x 16 stem pixels x 64 ch fp16
-#ifndef ODTK_STEM_EPI_WARPS
-#define ODTK_STEM_EPI_WARPS 16   /* 8: each warp converts 64 columns; 16: 32 columns (the epilogue, not the 28 MMAs, bounds a tile) */
-#endif
-constexpr int kEpiWarps = ODTK_STEM_EPI_WARPS;
-constexpr int kColSplit = kEpiWarps / 8;             // warps sharing one (lane quarter, half) accumulator: each takes 64 / kColSplit columns
-constexpr int kThreads = 128 + 32 * kEpiWarps;
-constexpr int kTmemCols = 256;                       // 2 buffers x (2 halves x 64 columns)
-constexpr int kPool = 7;                             // pooled pixels per tile side
-
-struct StemBars {
-  uint64_t full[kStages], empty[kStages];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint64_t w_full;
-  uint32_t tmem_base;
-};
-constexpr int kSmemBytes = 1024 + kStages * kPatchSlot + kWBytes + 2 * kStageTile + 256 /*bias*/ + 256 /*barriers*/;
+constexpr int kABytes = 128 * 64;           // A: up to 128 rows x 32 fp16 (64 B)
+constexpr int kStageBytes = kABytes + kCout * 64;
+constexpr int kStages = 8;
+constexpr int kTileBytes = kRows * kCout * 2;   // staged fp16 stem tile, [121][64]
+constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kTileBytes + 2 * kStages * 8;
 
 struct StemParams {
-  int N, OH, OW;        // stem output size (H/2, W/2)
-  int PH, PW;           // pooled output size
-  int tiles_h, tiles_w, total_tiles;
-  const float *bias;    // [64] fp32 (folded BatchNorm shift) or NULL
-  __half *out;          // [N, PH, PW, 64]
-  int relu;
+  int N, OH, OW, PH, PW, tiles_h, tiles_w, total_tiles, relu;
+  const float *bias;
+  __half *out;
 };
 
 __global__ void __launch_bounds__(kThreads, 1)
-stem_pool_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const StemParams p) {
+stem_pool_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ StemParams p) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  unsigned char *spatch = smem;
-  unsigned char *sw = spatch + kStages * kPatchSlot;           // 1024-aligned: 6 * 12288
-  unsigned char *sstage = sw + kWBytes;                        // 28672 = 28 * 1024: aligned
-  float *sbias = reinterpret_cast<float *>(sstage + 2 * kStageTile);
-  StemBars *bars = reinterpret_cast<StemBars *>(reinterpret_cast<unsigned char *>(sbias) + 256);
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < kStages; s++) { mbar_init(&bars->full[s], 1); mbar_init(&bars->empty[s], 1); }
-    for (int b = 0; b < 2; b++) { mbar_init(&bars->tmem_full[b], 1); mbar_init(&bars->tmem_empty[b], 32 * kEpiWarps); }
-    mbar_init(&bars->w_full, 1);
+  __half *stile = reinterpret_cast<__half *>(smem + kStages * kStageBytes);
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + kStages * kStageBytes + kTileBytes);
+  uint64_t *empty = full + kStages;
+  const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0), tid = threadIdx.x & 127;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < kStages; s++) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&bars->tmem_base)), "r"(kTmemCols));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  if (warp == 3) {
-    for (int i = lane; i < kCout; i += 32) sbias[i] = p.bias ? p.bias[i] : 0.0f;
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   grid_dep_launch_dependents();
   grid_dep_wait();
-  const uint32_t tmem_base = bars->tmem_base;
   const int per_img = p.tiles_h * p.tiles_w;
+  auto origin = [&](int tile, int &img, int &ph0, int &pw0) {
+    img = tile / per_img;
+    const int r = tile - img * per_img;
+    ph0 = (r / p.tiles_w) * kPool;
+    pw0 = (r % p.tiles_w) * kPool;
+  };
+  int stage = 0;
+  uint32_t phase = 0;
 
-  if (warp == 0) {
-    // ===================================== TMA producer =====================================
-    if (elect_one()) {
-      mbar_arrive_expect_tx(&bars->w_full, (uint32_t)kWBytes);
-      for (int r = 0; r < 7; r++) tma_load_2d(sw + r * (kCout * 64), &tmB, &bars->w_full, r * 32, 0);
-    }
-    int stage = 0;
-    uint32_t phase = 0;
+  if (wg == 0) {
+    if (tid != 0) return;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-      const int img = tile / per_img, rr = tile - img * per_img;
-      const int sr0 = 2 * kPool * (rr / p.tiles_w) - 1, sc0 = 2 * kPool * (rr % p.tiles_w) - 1;   // first stem pixel of the tile
-      mbar_wait(&bars->empty[stage], phase ^ 1u);
-      if (elect_one()) {
-        mbar_arrive_expect_tx(&bars->full[stage], (uint32_t)kPatchBytes);
-        // padded image rows 2*sr0 .., padded pixel columns 2*sc0 .. (4 fp16 per pixel): may start at -2 / -8 elements
-        tma_load_3d(spatch + stage * kPatchSlot, &tmA, &bars->full[stage], 8 * sc0, 2 * sr0, img);
+      int img, ph0, pw0;
+      origin(tile, img, ph0, pw0);
+      for (int r = 0; r < 7; r++) {
+        mbar_wait(&empty[stage], phase ^ 1u);
+        unsigned char *s = smem + stage * kStageBytes;
+        mbar_arrive_expect_tx(&full[stage], (uint32_t)(kRows * 64 + kCout * 64));
+        // stem pixels (2 ph0 - 1 .., 2 pw0 - 1 ..): coordinate -1 is outside the map and zero-filled (never pooled)
+        tma_load_5d(s, &tmA, &full[stage], 0, 2 * pw0 - 1, r, 2 * ph0 - 1, img);
+        tma_load_2d(s + kABytes, &tmB, &full[stage], r * 32, 0);
+        if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
+    }
+    return;
+  }
+
+  const int cw = wg - 1, warp = tid >> 5, lane = tid & 31, q = lane & 3, t = threadIdx.x - 128;
+  float acc[32];
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+    int img, ph0, pw0;
+    origin(tile, img, ph0, pw0);
+    int prev = -1;
+    for (int r = 0; r < 7; r++) {
+      mbar_wait(&full[stage], phase);
+      const uint32_t sa = smem_u32(smem + stage * kStageBytes);
+      const uint64_t da = wgmma_desc(sa + (uint32_t)(cw * 64 * 64), 64), db = wgmma_desc(sa + kABytes, 64);
+      wgmma_fence();
+      Wgmma<64>::mma(acc, da, db, r ? 1 : 0);
+      Wgmma<64>::mma(acc, da + 2, db + 2, 1);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
       if (++stage == kStages) { stage = 0; phase ^= 1u; }
     }
-  } else if (warp == 1) {
-    // ===================================== MMA issuer ========================================
-    const uint32_t idesc = (1u << 4) | ((uint32_t)(kCout >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);   // f32 acc, f16 x f16, K-major, N 64, M 128
-    const uint32_t swa = smem_u32(sw);
-    mbar_wait(&bars->w_full, 0);
-    int stage = 0, it = 0;
-    uint32_t phase = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, it++) {
-      const int buf = it & 1;
-      mbar_wait(&bars->tmem_empty[buf], ((uint32_t)(it >> 1) & 1u) ^ 1u);
-      mbar_wait(&bars->full[stage], phase);
-      tc_fence_after();
-      const uint32_t patch = smem_u32(spatch + stage * kPatchSlot);
-      if (elect_one()) {
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+    asm volatile("bar.sync 1, 256;" ::: "memory");   // the previous tile's pooling has read the staged tile
 #pragma unroll
-        for (int half = 0; half < 2; half++) {
-          const uint32_t tmem_d = tmem_base + (uint32_t)(buf * 128 + half * 64);
+    for (int i = 0; i < 2; i++) {
+      const int row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;
+      if (row >= kRows) continue;
 #pragma unroll
-          for (int r = 0; r < 7; r++) {
-#pragma unroll
-            for (int k = 0; k < 2; k++) {   // 16 K elements = 4 padded pixels x 4 channels = 32 B of the window
-              const uint64_t da = make_desc_raw(patch + half * 128 + r * kRowBytes + k * 32, 16u, 2u * kRowBytes);
-              const uint64_t db = make_desc_kmajor(swa + (uint32_t)(r * kCout * 64), 64) + (uint64_t)(2 * k);
-              tc_mma_f16(tmem_d, da, db, idesc, (r | k) ? 1u : 0u);
-            }
-          }
-        }
-        tc_commit(&bars->empty[stage]);
-        tc_commit(&bars->tmem_full[buf]);
-      }
-      if (++stage == kStages) { stage = 0; phase ^= 1u; }
-    }
-  } else if (warp >= 4) {
-    // ===================================== epilogue ==========================================
-    const int q = warp & 3, half = ((warp - 4) >> 2) & 1, cpart = (warp - 4) >> 3;   // cpart: which 64 / kColSplit columns
-    const int m = q * 32 + lane;                 // accumulator row
-    const int si = m >> 3, sj = half * 8 + (m & 7);   // stem pixel of this thread inside the 16 x 16 tile
-    const int pix = si * 16 + sj;
-    const int et = (warp - 4) * 32 + lane;       // 0 .. 32 * kEpiWarps - 1
-    const uint32_t sbias_s = smem_u32(sbias);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, it++) {
-      const int buf = it & 1;
-      const int img = tile / per_img, rr = tile - img * per_img;
-      const int ph0 = kPool * (rr / p.tiles_w), pw0 = kPool * (rr % p.tiles_w);
-      const int sr = 2 * ph0 - 1 + si, sc = 2 * pw0 - 1 + sj;
-      const bool inside = sr >= 0 && sr < p.OH && sc >= 0 && sc < p.OW;
-      const uint32_t stg = smem_u32(sstage) + (uint32_t)((it & 1) * kStageTile);   // shared-space address (LDS / STS)
-      mbar_wait(&bars->tmem_full[buf], (uint32_t)(it >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * 128 + half * 64);
-      uint32_t v[2][16];
-      constexpr int kChunks = 4 / kColSplit;
-      const int c_first = cpart * kChunks;
-      tc_ld16(taddr + (uint32_t)(c_first * 16), v[0]);
-#pragma unroll
-      for (int ci = 0; ci < kChunks; ci++) {
-        const int c4 = c_first + ci;
-        tc_ld_wait();
-        if (ci < kChunks - 1) tc_ld16(taddr + (uint32_t)((c4 + 1) * 16), v[(ci + 1) & 1]);
-        uint4 o0 = make_uint4(0u, 0u, 0u, 0u), o1 = o0;
-        if (inside) {
-          float f[16];
-#pragma unroll
-          for (int j4 = 0; j4 < 4; j4++) {
-            const float4 b = lds128f(sbias_s + (uint32_t)((c4 * 16 + j4 * 4) * 4));
-            f[4 * j4] = __uint_as_float(v[ci & 1][4 * j4]) + b.x;
-            f[4 * j4 + 1] = __uint_as_float(v[ci & 1][4 * j4 + 1]) + b.y;
-            f[4 * j4 + 2] = __uint_as_float(v[ci & 1][4 * j4 + 2]) + b.z;
-            f[4 * j4 + 3] = __uint_as_float(v[ci & 1][4 * j4 + 3]) + b.w;
-          }
-          __half2 *q0 = reinterpret_cast<__half2 *>(&o0), *q1 = reinterpret_cast<__half2 *>(&o1);
-          const __half2 z = __float2half2_rn(0.0f);
-#pragma unroll
-          for (int j = 0; j < 4; j++) {
-            q0[j] = __floats2half2_rn(f[2 * j], f[2 * j + 1]);
-            q1[j] = __floats2half2_rn(f[8 + 2 * j], f[8 + 2 * j + 1]);
-            if (p.relu) { q0[j] = __hmax2(q0[j], z); q1[j] = __hmax2(q1[j], z); }
-          }
-        }
-        sts128(stg + (uint32_t)(pix * 128 + (((2 * c4) ^ (pix & 7)) << 4)), o0);
-        sts128(stg + (uint32_t)(pix * 128 + (((2 * c4 + 1) ^ (pix & 7)) << 4)), o1);
-      }
-      tc_fence_before();
-      mbar_arrive(&bars->tmem_empty[buf]);       // the accumulator is in registers / shared memory: hand it back
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
-      // ---- 3x3 stride-2 max over the staging tile: item = (pooled pixel, 8-channel chunk) ----
-#pragma unroll
-      for (int rnd = 0; rnd < (kPool * kPool * 8 + 32 * kEpiWarps - 1) / (32 * kEpiWarps); rnd++) {
-        const int item = et + rnd * 32 * kEpiWarps;
-        if (item < kPool * kPool * 8) {
-          const int c = item & 7, pp = item >> 3, pi = pp / kPool, pj = pp - pi * kPool;
-          const int ph = ph0 + pi, pw = pw0 + pj;
-          if (ph < p.PH && pw < p.PW) {
-            // all nine 16-byte loads first (they are volatile asm: issued in program order, so keep them adjacent and
-            // let the nine latencies overlap), then the max tree
-            uint4 u[9];
-#pragma unroll
-            for (int di = 0; di < 3; di++) {
-#pragma unroll
-              for (int dj = 0; dj < 3; dj++) {
-                const int px = (2 * pi + di) * 16 + 2 * pj + dj;
-                u[di * 3 + dj] = lds128(stg + (uint32_t)(px * 128 + ((c ^ (px & 7)) << 4)));
-              }
-            }
-            __half2 best[4];
-#pragma unroll
-            for (int j = 0; j < 4; j++) best[j] = __float2half2_rn(p.relu ? 0.0f : -65504.0f);   // after ReLU inputs are >= 0: 0 == padding
-#pragma unroll
-            for (int di = 0; di < 3; di++) {
-#pragma unroll
-              for (int dj = 0; dj < 3; dj++) {
-                const int srr = 2 * ph - 1 + di, scc = 2 * pw - 1 + dj;
-                if (!p.relu && (srr < 0 || srr >= p.OH || scc < 0 || scc >= p.OW)) continue;   // without ReLU the padding is -inf
-                const __half2 *h = reinterpret_cast<const __half2 *>(&u[di * 3 + dj]);
-#pragma unroll
-                for (int j = 0; j < 4; j++) best[j] = __hmax2(best[j], h[j]);
-              }
-            }
-            *reinterpret_cast<uint4 *>(p.out + (((long long)img * p.PH + ph) * p.PW + pw) * kCout + c * 8) =
-                *reinterpret_cast<uint4 *>(best);
-          }
-        }
+      for (int j = 0; j < 8; j++) {
+        const int col = 8 * j + 2 * q;
+        const float b0 = p.bias ? __ldg(p.bias + col) : 0.0f, b1 = p.bias ? __ldg(p.bias + col + 1) : 0.0f;
+        __half2 v = __floats2half2_rn(acc[4 * j + 2 * i] + b0, acc[4 * j + 2 * i + 1] + b1);
+        if (p.relu) v = __hmax2(v, __float2half2_rn(0.0f));
+        *reinterpret_cast<__half2 *>(stile + row * kCout + col) = v;
       }
     }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    // ---- 3x3 / 2 max-pool over the staged tile: 25 pooled pixels x 8 groups of 8 channels ----
+    const int sh0 = 2 * ph0 - 1, sw0 = 2 * pw0 - 1;
+    for (int it = t; it < kPool * kPool * 8; it += 256) {
+      const int pix = it >> 3, cg = (it & 7) * 8, py = pix / kPool, px = pix - py * kPool;
+      const int oh = ph0 + py, ow = pw0 + px;
+      if (oh >= p.PH || ow >= p.PW) continue;
+      __half2 m[4];
+      bool any = false;
+#pragma unroll
+      for (int dy = 0; dy < 3; dy++) {
+        const int ly = 2 * py + dy, gy = sh0 + ly;
+        if (gy < 0 || gy >= p.OH) continue;
+#pragma unroll
+        for (int dx = 0; dx < 3; dx++) {
+          const int lx = 2 * px + dx, gx = sw0 + lx;
+          if (gx < 0 || gx >= p.OW) continue;
+          const uint4 v = *reinterpret_cast<const uint4 *>(stile + (ly * kSide + lx) * kCout + cg);
+          const __half2 *h = reinterpret_cast<const __half2 *>(&v);
+#pragma unroll
+          for (int k = 0; k < 4; k++) m[k] = any ? __hmax2(m[k], h[k]) : h[k];
+          any = true;
+        }
+      }
+      *reinterpret_cast<uint4 *>(p.out + (((long long)img * p.PH + oh) * p.PW + ow) * kCout + cg) = *reinterpret_cast<uint4 *>(m);
+    }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTmemCols));
-  }
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-bool encode(CUtensorMap *m, const void *base, int rank, const uint64_t *dims, const uint64_t *strides, const uint32_t *box,
-            CUtensorMapSwizzle swz) {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return false;
-    fn = (EncodeTiledFn)ptr;
-  }
-  cuuint64_t gdim[5], gstr[5];
-  cuuint32_t bx[5], es[5];
-  for (int i = 0; i < rank; i++) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-  for (int i = 0; i < rank - 1; i++) gstr[i] = strides[i];
-  return fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr, bx, es,
-            CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 }  // namespace
@@ -284,13 +160,17 @@ extern "C" int odtk_stem_pool(const void *xp, const void *w, const float *bias, 
   if ((h & 1) || (width & 1) || cout != kCout) return ODTK_E_UNSUPPORTED;
   if (((uintptr_t)xp | (uintptr_t)w | (uintptr_t)y) & 15) return ODTK_E_INVALID;
   cudaStream_t stream = (cudaStream_t)stream_;
-  static bool configured[64] = {};
+  static std::mutex mu;
+  static bool configured[64];
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return ODTK_E_CUDA;
-  if (dev < 0 || dev >= 64 || !configured[dev]) {
-    if (cudaFuncSetAttribute(stem_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
-      return ODTK_E_CUDA;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return ODTK_E_CUDA;
+  {
+    std::lock_guard<std::mutex> lk(mu);
+    if (!configured[dev]) {
+      if (cudaFuncSetAttribute(stem_pool_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
+        return ODTK_E_CUDA;
+      configured[dev] = true;
+    }
   }
   StemParams p;
   memset(&p, 0, sizeof p);
@@ -298,22 +178,22 @@ extern "C" int odtk_stem_pool(const void *xp, const void *w, const float *bias, 
   p.PH = (p.OH - 1) / 2 + 1; p.PW = (p.OW - 1) / 2 + 1;
   p.tiles_h = (p.PH + kPool - 1) / kPool; p.tiles_w = (p.PW + kPool - 1) / kPool;
   const long long total = (long long)n * p.tiles_h * p.tiles_w;
-  if (total >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  if (total >= (1ll << 31) || (long long)n * p.OH * p.OW >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
   p.total_tiles = (int)total;
   p.bias = bias; p.out = (__half *)y; p.relu = relu;
   const int HP = h + 6, WP = width + 8;
   CUtensorMap tmA, tmB;
-  {
-    uint64_t dims[3] = {(uint64_t)WP * 4, (uint64_t)HP, (uint64_t)n};
-    uint64_t str[2] = {(uint64_t)WP * 8, (uint64_t)HP * WP * 8};
-    uint32_t box[3] = {kPatchCols * 4, kPatchRows, 1};
-    if (!encode(&tmA, xp, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE)) return ODTK_E_CUDA;
+  {   // the overlapping-window map of odtk_stem_conv: {32 elements, OW (16 B), 7 filter rows, OH (two padded rows), N}
+    uint64_t dims[5] = {32, (uint64_t)p.OW, 7, (uint64_t)p.OH, (uint64_t)n};
+    uint64_t str[4] = {16, (uint64_t)WP * 8, (uint64_t)WP * 16, (uint64_t)HP * WP * 8};
+    uint32_t box[5] = {32, (uint32_t)kSide, 1, (uint32_t)kSide, 1};
+    if (!encode_map(&tmA, xp, 5, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B)) return ODTK_E_UNSUPPORTED;
   }
   {
     uint64_t dims[2] = {224, (uint64_t)cout};
     uint64_t str[1] = {224 * 2};
     uint32_t box[2] = {32, (uint32_t)cout};
-    if (!encode(&tmB, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B)) return ODTK_E_CUDA;
+    if (!encode_map(&tmB, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B)) return ODTK_E_CUDA;
   }
   const int sms = odtk_sm_count();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;

@@ -1,4 +1,4 @@
-// targets.cu -- anchor target assignment for sm_100a (SURVEY.md section 8f, row 2).
+// targets.cu -- anchor target assignment for sm_90a.
 //
 // Replaces snap_to_anchors (reference odtk/box.py:134-186) as called per image and per pyramid level by
 // Model._extract_targets (odtk/model.py:167-184): the reference builds the [A*H*W, #gt] IoU matrix, the arg-max, the
@@ -8,7 +8,7 @@
 // skipped on the device, which is what `target[target[:, -1] > -1]` does on the host).
 //
 // Outputs, in the reference's layouts: cls_target [B, A, C, H, W] (dense one-hot, optional), box_target [B, A, 4, H, W],
-// depth [B, A, 1, H, W] (-1 ignored, 0 background, class + 1 foreground), and -- B200-native -- cls_index [B, A, H, W]
+// depth [B, A, 1, H, W] (-1 ignored, 0 background, class + 1 foreground), and -- H100-native -- cls_index [B, A, H, W]
 // int32 (class, -1 background, -2 ignored): exactly what odtk_focal_loss consumes, so the dense one-hot never has to
 // exist.  Parity: IoU and thresholds in fp32 with the reference's operation order (compiled without FMA contraction,
 // IEEE division): depth / classes / arg-max bit-exact; box deltas differ only by logf vs torch.log (<= 1 ulp).

@@ -1,5 +1,5 @@
-// tc_ptx.cuh -- inline-PTX wrappers shared by the sm_100a tensor-core kernels (conv.cu, stem.cu): mbarrier, TMA
-// (cp.async.bulk.tensor), tcgen05 (mma / commit / ld / fences), cluster helpers and UMMA shared-memory descriptors.
+// tc_ptx.cuh -- inline-PTX wrappers of the sm_90a tensor-core convolution (conv.cu): mbarrier, TMA
+// (cp.async.bulk.tensor) and programmatic dependent launch.  The wgmma wrappers are in wgmma.cuh.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -8,23 +8,6 @@
 namespace {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// Explicit shared-state-space 16-byte accesses.  The kernels carve their dynamic shared memory with integer pointer
-// arithmetic (1024-byte alignment), after which the compiler no longer knows the address space and emits GENERIC
-// LD.E / ST.E (slower, and serialised differently) for plain dereferences: hot epilogue paths use these instead.
-__device__ __forceinline__ void sts128(uint32_t saddr, uint4 v) {
-  asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-__device__ __forceinline__ uint4 lds128(uint32_t saddr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr) : "memory");
-  return v;
-}
-__device__ __forceinline__ float4 lds128f(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr));
-  return v;
-}
 
 __device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -53,12 +36,6 @@ __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_3d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-      : "memory");
-}
 __device__ __forceinline__ void tma_load_4d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1,
                                             int c2, int c3) {
   asm volatile(
@@ -73,146 +50,13 @@ __device__ __forceinline__ void tma_load_5d(void *dst, const CUtensorMap *map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_mc(void *dst, const CUtensorMap *map, uint64_t *bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t saddr, uint32_t rank) {   // same offset in CTA `rank` of the cluster
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-// Arrive on a barrier of another CTA of the cluster.  Default semantics (.release at CTA scope), as CUTLASS's
-// ClusterBarrier::arrive: `.release.cluster` compiles to MEMBAR.ALL.GPU + ERRBAR in front of every arrive (~2000 cycles
-// per call, measured with the in-kernel wait profile of bottleneck.cu).  What the waiter consumes is ordered by the
-// tcgen05 / async-proxy fences the callers execute before arriving.
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// cta_group::2 TMA loads: destination in the executing CTA, completion counted on a barrier that may live in the peer
-__device__ __forceinline__ void tma2_load_2d(void *dst, const CUtensorMap *map, uint32_t bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void *dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_5d(void *dst, const CUtensorMap *map, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
-  asm volatile(
-      "cp.async.bulk.tensor.5d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
-      : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// One lane of a fully converged warp.  The issuing warps stay converged and wrap only the TMA / MMA / commit
-// instructions in `if (elect_one())`: their operands then live in uniform registers, instead of the per-instruction
-// "waterfall" loops (ELECT + R2UR.BROADCAST + branch) the compiler emits around them in lane-0-only code.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
-  return pred != 0;
-}
 // Programmatic dependent launch: a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while
 // its predecessor in the stream is still running.  launch_dependents lets the NEXT kernel's CTAs take the SMs this
-// kernel's CTAs free as they exit (its prologue -- barrier init, TMEM allocation, descriptor prefetch -- then overlaps this
-// kernel's tail); grid_dep_wait blocks until the PREVIOUS kernel has completed and its writes are visible: everything that
-// touches activations comes after it.
+// kernel's CTAs free as they exit (its prologue -- barrier init, descriptor prefetch -- then overlaps this kernel's tail);
+// grid_dep_wait blocks until the PREVIOUS kernel has completed and its writes are visible: everything that touches
+// activations comes after it.
 __device__ __forceinline__ void grid_dep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc(uint64_t *bar, uint16_t mask) {   // arrive on the same barrier in every CTA of `mask`
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ void tc_commit2_mc(uint64_t *bar, uint16_t mask) {   // cta_group::2 commit, arrives in every CTA of `mask`
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask)
-               : "memory");
-}
-__device__ __forceinline__ void tc_mma2_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tc_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// Shared-memory matrix descriptor, K-major, 128-byte swizzle: rows of 64 fp16 = 128 B, 8-row
-// groups 1024 B apart (SBO), LBO unused for swizzled K-major layouts, descriptor version 1.
-// `row_bytes` = 128 (SWIZZLE_128B, layout type 2) or 64 (SWIZZLE_64B, layout type 4): the 8-row
-// swizzle atom is 8 * row_bytes.
-__device__ __forceinline__ uint64_t make_desc_kmajor(uint32_t saddr, int row_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);           // start address  [0,14)
-  d |= (uint64_t)1 << 16;                              // LBO (ignored)  [16,30)
-  d |= (uint64_t)((8 * row_bytes) >> 4) << 32;         // SBO            [32,46)
-  d |= (uint64_t)1 << 46;                              // version = 1    [46,48)
-  d |= (uint64_t)(row_bytes == 128 ? 2 : 4) << 61;     // swizzle mode   [61,64)
-  return d;
-}
-
-// MN-major operand (N contiguous), 128-byte swizzle: 64-element (128 B) chunks along N are `lbo` bytes apart,
-// 8-row groups along K are 1024 B apart.  Used for the residual tile read as the B operand of I * R.
-__device__ __forceinline__ uint64_t make_desc_mnmajor(uint32_t saddr, uint32_t lbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-
-// Un-swizzled K-major operand (layout type 0): 8-row core matrices of 16-byte rows; `lbo` = byte distance between core
-// matrices along K, `sbo` = along M/N.  Used by the stem's raw-window A operand (conv.cu, stem.cu).
-__device__ __forceinline__ uint64_t make_desc_raw(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFFu) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3FFFu) << 32;
-  d |= (uint64_t)1 << 46;
-  return d;                                             // layout type 0: no swizzle
-}
 
 // sigmoid with the SFU approximations (ex2.approx + rcp.approx): relative error < 1e-6, far inside
 // the 1e-3 score tolerance, and ~4x fewer instructions than expf + IEEE division in a hot epilogue

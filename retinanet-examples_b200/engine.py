@@ -15,8 +15,8 @@ STATS = {"launches": 0, "conv_flops": 0, "trace": None}
 
 def _trace(kind, flops, nbytes, **shape):
     """When STATS["trace"] is a list, every kernel launch appends (kind, algorithmic FLOPs, algorithmic HBM bytes =
-    every operand read once + the output written once, shape): bench.py's layer-wise roofline and the per-launch ncu
-    tables in profiles/ are keyed on this order."""
+    every operand read once + the output written once, shape): bench.py's layer-wise roofline is keyed on this
+    order."""
     if STATS["trace"] is not None:
         STATS["trace"].append(dict(kind=kind, flops=int(flops), bytes=int(nbytes), **shape))
 
@@ -78,7 +78,8 @@ def pack_weight_grouped(weight, groups):
 
 
 def pack_bias(bias):
-    """fp32 bias [Cout] (CUDA) -> the [Cout, 64] fp16 operand of the kernel's bias K block."""
+    """fp32 bias [Cout] (CUDA) -> the [Cout, 64] fp16 (hi, lo) layout of odtk_conv_t.bias_op.  The sm_90a kernel adds
+    the fp32 bias in its epilogue and does not read it."""
     out = torch.empty((bias.numel(), 64), dtype=torch.float16, device=bias.device)
     _lib.check(_lib.lib().odtk_conv_pack_bias(ctypes.c_void_p(bias.data_ptr()), ctypes.c_void_p(out.data_ptr()),
                                               bias.numel(), _stream()), "conv_pack_bias")

@@ -1,5 +1,5 @@
 """Host-side mirror of the hot loop of the reference's odtk/infer.py:71-102 on tensors that are
-already in memory (datasets, COCO json/eval, DALI and apex are outside the hot path, SURVEY.md
+already in memory (datasets, COCO json/eval, DALI and apex are outside the hot path
 section 2): per batch `model(data)`, collect, and -- when several ranks shard the images -- gather the
 detections of all ranks.  The reference issues five all_gathers (scores, boxes, classes, ids, ratios)
 after the loop (infer.py:98-102); here the three detection tensors travel as ONE packed

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's odtk/loss.py FocalLoss on the fused sm_100a kernel
+"""Host-side mirror of the reference's odtk/loss.py FocalLoss on the fused sm_90a kernel
 (odtk_focal_loss in include/odtk_b200.h).  `FocalLoss()(pred_logits, target)` returns the
 element-wise loss like the reference module; `focal_loss_sum` is the fused training form
 (masked sum + gradient in one pass, usable with autograd)."""

@@ -1,15 +1,15 @@
 """RetinaNet inference model -- host-side mirror of the reference's odtk/model.py `Model`
 (constructor arguments, `config` keys, state_dict key names, `forward(x) -> (scores, boxes,
-classes)`), executing on the sm_100a kernels behind the C ABI instead of nn.Conv2d/cuDNN +
+classes)`), executing on the sm_90a kernels behind the C ABI instead of nn.Conv2d/cuDNN +
 odtk._C.  `_compute_loss` (training-mode forward) runs target assignment + ONE fused loss kernel; `save` / `load` /
 `initialize(pre_trained)` read and write the reference's checkpoint dict; ONNX/TensorRT export is outside the
-hot path (SURVEY.md section 2); `load_state_dict` ingests exactly the reference's key layout
+hot path; `load_state_dict` ingests exactly the reference's key layout
 (odtk/model.py:217-258): `backbones.<Name>.features.*`, `backbones.<Name>.{lateral,pyramid,smooth}*`,
 `cls_head.{0,2,4,6,8}.*`, `box_head.{0,2,4,6,8}.*`.
 
 Data flow of forward() (reference: odtk/model.py:125-165, odtk/backbones/fpn.py:45-61,
 odtk/backbones/resnet.py:24-39, torchvision BasicBlock/Bottleneck):
-  NHWC fp16 activations; every conv is one launch of the tcgen05 kernel with BatchNorm folded
+  NHWC fp16 activations; every conv is one launch of the wgmma kernel with BatchNorm folded
   into weights/bias, ReLU / residual add / FPN upsample-add fused in its epilogue; the last conv
   of each head writes fp32 NCHW (sigmoid fused for the class head) which feeds the all-levels
   decode (3 launches) and the batched NMS (1 launch)."""
@@ -119,7 +119,7 @@ def conv_specs(backbone, classes=80, num_anchors=9, rotated=False):
 def make_state_dict(backbone="ResNet50FPN", classes=80, num_anchors=9, rotated=False, seed=0, cls_prior=0.01):
     """Deterministic random-init weights in the reference's state_dict layout (no checkpoint or
     pretrained weights exist offline).  BatchNorm statistics are randomised so that folding is
-    exercised (SURVEY.md section 8d, config 3); the last BN of each residual block is damped so
+    exercised; the last BN of each residual block is damped so
     that activations stay well inside fp16 range through 50+ layers."""
     g = torch.Generator().manual_seed(seed)
     sd = {}
@@ -154,7 +154,6 @@ class _Conv:
             self.kpad = kh * kw * 64
             self.w = engine.pack_weight_grouped(weight, groups).to(device)
             self.b = bias.float().contiguous().to(device) if bias is not None else None
-            self.bop = engine.pack_bias(self.b) if self.b is not None else None
             return
         self.cout, self.cin, self.ks, self.stride = cout, cin, kh, stride
         self.direct = stride == 1 and kh in (1, 3) and cin % 64 == 0
@@ -164,7 +163,6 @@ class _Conv:
         self.kpad = kreal if self.direct else (kreal + 63) // 64 * 64
         self.w = engine.pack_weight(weight, self.kpad).to(device)
         self.b = bias.float().contiguous().to(device) if bias is not None else None
-        self.bop = engine.pack_bias(self.b) if self.b is not None else None     # bias as a tensor-core K block
 
     def __call__(self, x, relu=False, residual=None, upsample=None, out_mode=engine.OUT_NHWC_F16, in_relu=False,
                  sink=None, out=None, tile_tab=None, valid_px=None):
@@ -176,7 +174,7 @@ class _Conv:
         if self.direct:
             assert not in_relu
             return engine.conv2d(x, self.w, self.b, self.cout, self.ks, relu, residual, upsample, out_mode,
-                                 bias_op=self.bop, sink=sink, groups=self.groups, out=out, tile_tab=tile_tab)
+                                 sink=sink, groups=self.groups, out=out, tile_tab=tile_tab)
         assert sink is None
         if self.stride == 2 and self.ks in (1, 3) and self.cin % 64 == 0 and upsample is None:
             # stride-2 convolution, any size: strided TMA view (even sizes: parity split, odd sizes: element-strided
@@ -184,9 +182,9 @@ class _Conv:
             if in_relu:
                 x = engine.relu_from_view(x) if isinstance(x, engine.AtlasView) else engine.relu(x)
             return engine.conv2d(x, self.w, self.b, self.cout, self.ks, relu, residual, None, out_mode, stride=2,
-                                 bias_op=self.bop, groups=self.groups, out=out)
+                                 groups=self.groups, out=out)
         low = engine.lower_conv(x, self.ks, self.stride, self.ks // 2, self.kpad if self.cin % 8 else None, in_relu)
-        return engine.conv2d(low, self.w, self.b, self.cout, 1, relu, residual, upsample, out_mode, bias_op=self.bop)
+        return engine.conv2d(low, self.w, self.b, self.cout, 1, relu, residual, upsample, out_mode)
 
 
 class Model:
@@ -197,7 +195,7 @@ class Model:
                  anchor_ious=[0.4, 0.5], config={}):
         if isinstance(backbones, (list, tuple)):
             if len(backbones) != 1:
-                raise ValueError("one backbone per model on the B200 path")
+                raise ValueError("one backbone per model on this path")
             backbones = backbones[0]
         if backbones not in BACKBONES:
             raise ValueError("unsupported backbone %r (hot path: %s)" % (backbones, ", ".join(BACKBONES)))
@@ -217,7 +215,7 @@ class Model:
         self.detections = config.get('detections', 100)
         self.stride = 128
         if self.top_n > 4096 or self.detections > 1024 or 5 * self.top_n > 6144:
-            raise ValueError("config outside the sm_100a kernels' limits (include/odtk_b200.h): top_n <= 4096, "
+            raise ValueError("config outside the sm_90a kernels' limits (include/odtk_b200.h): top_n <= 4096, "
                              "5 * top_n <= 6144 candidates per image into NMS, detections <= 1024; got top_n=%d detections=%d"
                              % (self.top_n, self.detections))
         self.num_anchors = len(ratios) * len(scales) * (len(self.angles) if rotated_bbox else 1)
@@ -311,7 +309,7 @@ class Model:
 
     def train(self, mode=True):
         """Training-mode forward (odtk/model.py:130-138): `model([images, targets])` returns (cls_loss, box_loss).  The
-        convolutions have no backward kernels here (the training loop is outside the hot path, SURVEY.md section 2): the
+        convolutions have no backward kernels here (the training loop is outside the hot path): the
         losses and -- `_compute_loss(..., with_grad=True)` -- their gradients w.r.t. the head outputs are what this
         provides."""
         self.training = bool(mode)
@@ -470,7 +468,8 @@ class Model:
                     dn.groups == 1 and cs[1].stride == 1 and cs[1].groups == 1 and cs[1].ks == 3 and cs[1].cin == 64 and
                     cs[1].cout == 64 and cs[2].cin == 64 and cs[2].cout == dn.cout and dn.cout % 128 == 0 and dn.cout <= 512):
                 # first block of layer1: conv2 + conv3 + the 1x1 PROJECTION of the block input (torchvision `downsample`)
-                # + ReLU in one kernel: neither the 3x3's output nor the projected identity touches HBM
+                # + ReLU in one kernel: the 3x3's output stays in shared memory, the projected identity is one more K block
+                # of the 1x1's fp32 accumulator
                 if "b3d" not in blk:
                     blk["b3d"] = (cs[2].b + dn.b).contiguous()
                 out = cs[0](x, relu=True)
@@ -515,7 +514,7 @@ class Model:
         p3 = P["lateral3"](c3, upsample=p4)
         if self.merged_heads and c5.shape[3] % 64 == 0:
             # pyramid atlas: the five levels stacked in ONE zero-separated NHWC buffer, so that every head-tower layer is
-            # one launch over all levels (SURVEY.md section 7 step 4) instead of five
+            # one launch over all levels instead of five
             n = c5.shape[0]
             h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
             sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
@@ -655,7 +654,7 @@ class Model:
         return x.permute(0, 2, 3, 1).contiguous().to(torch.float16)   # zero-copy for channels_last fp16
 
     def forward_heads_u8(self, images, sigmoid=True):
-        """Input side of `odtk infer` fused in (SURVEY.md section 8f row 3): `images` is a uint8 HWC batch
+        """Input side of `odtk infer` fused in: `images` is a uint8 HWC batch
         [B, H, W, 3]; normalisation, stride padding (odtk/data.py:113-123) and the stem's zero border are one
         kernel that writes the stem's input buffer directly."""
         if self._packed is None:

@@ -1,4 +1,4 @@
-"""Deterministic synthetic workloads of the shapes BASELINE.json names (SURVEY.md section 8d).
+"""Deterministic synthetic workloads of the shapes BASELINE.json names.
 No dataset or checkpoint exists offline: head outputs follow the measured candidate statistics
 (cls logits ~ N(-7, 1.6^2) -> ~0.56 % of scores above 0.05; box deltas ~ N(0, 0.2^2))."""
 import math
@@ -43,7 +43,7 @@ def head_outputs(batch, height=800, width=1280, classes=80, anchors=9, rotated=F
 
 def calibrate_cls_head(sd, logits_fn, mean=-7.0, std=1.6, seed=0):
     """Rescale the last class-head convolution of a random-init state_dict so that its logits follow
-    ~N(mean, std^2) (SURVEY.md section 8d: ~0.56 % of scores above 0.05, so decode and NMS do
+    ~N(mean, std^2) (~0.56 % of scores above 0.05, so decode and NMS do
     representative work; a fresh model yields zero detections).  `logits_fn(state_dict)` must return
     the per-level raw class logits of some probe batch under these weights (the caller decides
     how: the GPU engine via Model.forward_heads(sigmoid=False) in the product arm)."""

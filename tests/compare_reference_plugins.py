@@ -1,7 +1,7 @@
-"""Comparator for BASELINE.json configs[1] / [4] (not collected by pytest; run on the B200 box):
-decode + NMS on the RetinaNet head shapes, OUR sm_100a kernels vs the reference's own csrc/cuda
-kernels compiled unmodified for sm_100a (oracle/_ref/libodtk_ref.so), identical fp32 NCHW inputs,
-CUDA-event timing, results compared.  Writes one JSON line (kept under profiles/).
+"""Comparator for BASELINE.json configs[1] / [4] (not collected by pytest; run on an H100):
+decode + NMS on the RetinaNet head shapes, OUR sm_90a kernels vs the reference's own csrc/cuda
+kernels compiled unmodified for sm_90a (oracle/_ref/libodtk_ref.so), identical fp32 NCHW inputs,
+CUDA-event timing, results compared.  Writes one JSON line.
 
     python tests/compare_reference_plugins.py [--batch 8] [--rotated]
 """
@@ -95,7 +95,7 @@ def main():
                       "ours_us_per_image": round(us_ours, 2), "reference_cuda_plugins_us_per_image": round(us_ref, 2),
                       "speedup": round(us_ref / us_ours, 1), "kept_scores_identical_fraction": same_scores,
                       "max_abs_box_diff_vs_fast_math_reference": max_box,
-                      "reference": "csrc/cuda/{decode,decode_rotate,nms,nms_iou}.cu unmodified, nvcc -gencode arch=compute_100a,code=sm_100a --use_fast_math"}))
+                      "reference": "csrc/cuda/{decode,decode_rotate,nms,nms_iou}.cu unmodified, nvcc -gencode arch=compute_90a,code=sm_90a --use_fast_math"}))
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 """GPU tests of the in-kernel detection gather (odtk_nms_gather / odtk_gather_wait, retinanet-examples_b200/peer.py):
-F1 of SURVEY.md section 8 -- `infer.infer` over image-wise shards with the detections of all ranks delivered to every
+`infer.infer` over image-wise shards with the detections of all ranks delivered to every
 rank -- on the real Model, on NCCL ranks, compared with a single-GPU run of the same images.
-The 2-rank tests need 2 GPUs (gpurun --gpus 2); the single-GPU ones exercise the same kernel path with world size 1."""
+The 2-rank tests need 2 GPUs; the single-GPU ones exercise the same kernel path with world size 1."""
 import ctypes
 import os
 import socket
@@ -115,7 +115,7 @@ def _worker(rank, world, port, q):
         q.put((rank, "error", traceback.format_exc(), None, None))
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 @pytest.mark.timeout(600)
 def test_two_rank_gather_matches_single_gpu_run():
     import torch.multiprocessing as mp

@@ -27,12 +27,12 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(L, n), n
         assert n in _lib.SIGNATURES, "ctypes signature missing for %s" % n
-    assert b"sm_100a" in L.odtk_b200_version()
+    assert b"sm_90a" in L.odtk_b200_version()
 
 
 def test_workspace_size_queries_need_no_gpu():
     L = _lib.lib()
-    # decode: P3 of RetinaNet at 800x1280, batch 8 (SURVEY.md section 8)
+    # decode: P3 of RetinaNet at 800x1280, batch 8
     sz = L.odtk_decode_ex(8, None, None, 100, 160, 8, 9, 80, None, 36, 0.05, 1000, 4, 1000, 0, None, 0, None)
     assert sz > 8 * (1 << 20) * 8          # candidate lists dominate
     assert sz % 256 == 0
@@ -72,26 +72,6 @@ def test_cpu_tensors_are_rejected_no_fallback():
 
 def test_level_sizes_match_survey():
     assert synth.level_sizes(800, 1280) == [(100, 160), (50, 80), (25, 40), (13, 20), (7, 10)]
-
-
-def test_layer_table_tool_reproduces_committed_profile(tmp_path):
-    """tools/layer_table.py joins the committed ncu launch list with the engine trace of the same step; the
-    committed summary (which bench.py reads for roofline.traffic) must be what the tool computes from them."""
-    import json
-    import subprocess
-    import sys
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    prof = os.path.join(root, "profiles")
-    out = str(tmp_path / "table")
-    subprocess.run([sys.executable, os.path.join(root, "tools", "layer_table.py"), os.path.join(prof, "r01_step_launches.csv"),
-                    os.path.join(prof, "r01_step_trace.json"), "--out", out], check=True, capture_output=True)
-    new = json.load(open(out + ".json"))["summary"]
-    old = json.load(open(os.path.join(prof, "r01_layer_table.json")))["summary"]
-    for k in ("launches", "sum_us", "sum_ideal_us", "conv_dram_bytes"):
-        assert new[k] == old[k], k
-    assert 0.5 < new["frac"] <= 1.0
-    trace = json.load(open(os.path.join(prof, "r01_step_trace.json")))
-    assert sum(l["flops"] for l in trace) == 15266307768320      # 477.07 GFLOP/image x 32 (DESIGN.md section 4)
 
 
 def test_plugin_shaped_wrappers_compile_and_query_sizes(tmp_path):

@@ -1,9 +1,9 @@
 """Time every DISTINCT layer launch of one step of bench.py's default workload in isolation (CUDA events on the
-launching stream, 2 warm-up + N timed launches each) and print / save a table keyed like tools/layer_table.py:
-    python tools/layer_bench.py [--batch 32] [--backbone ResNet50FPN] [--reps 5] [--tag name] [--rotated]
+launching stream, 2 warm-up + N timed launches each) and print / save a table:
+    python tools/layer_bench.py [--batch 32] [--backbone ResNet50FPN] [--reps 5] [--tag name] [--rotated] [--out DIR]
 The calls are recorded by wrapping the engine's entry points while one eager forward runs, then replayed with the very
 same tensors (so shapes, strides, fused epilogues and the kernel variant chosen by the host code are the model's own).
-Environment toggles (ODTK_CONV_*, ODTK_STEM_*) are read by the library at first use: run once per setting and compare
+Environment toggles (ODTK_PDL, ODTK_FUSED_*) are read at first use: run once per setting and compare
 the JSON files.  Inputs of the small pyramid levels fit the L2, exactly as they do inside the real step."""
 import argparse
 import collections
@@ -23,6 +23,7 @@ def main():
     ap.add_argument("--tag", default="base")
     ap.add_argument("--rotated", action="store_true")
     ap.add_argument("--only", default=None, help="substring filter on the layer key")
+    ap.add_argument("--out", default=".", help="directory of layer_bench_<tag>.json")
     ap.add_argument("--calibrated", action="store_true", help="class-head bias calibrated like bench.py (~0.56 %% of the scores above the threshold)")
     args = ap.parse_args()
     import torch
@@ -30,8 +31,7 @@ def main():
     from retinanet_examples_b200.model import Model, make_state_dict
     dev = torch.device("cuda:0")
     torch.cuda.set_device(dev)
-    peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    tf, bw = peaks.get("bf16_tflops_sustained") or peaks["bf16_tflops"], peaks["hbm_gbs"]
+    tf, bw = 989.0, 3350.0   # H100 SXM data sheet: dense FP16 TFLOP/s, HBM3 GB/s
 
     calls = []
     names = ["conv2d", "stem_conv", "stem_conv_padded", "maxpool3x3s2", "lower_conv", "relu", "pad_input", "stem_pool_padded", "bottleneck_tail"]
@@ -120,10 +120,10 @@ def main():
                 p["mode"], p["cluster"], p["bn"], p["nstages"], p["npatch"], p["tile_t"], p["b_resident"], p["res_mma"],
                 p["tma_store"], p["up_mma"], p["grid"])) if p else ""))
     print("sum over the step (isolated launches): %.1f us, layer-wise ideal %.1f us, frac %.3f" % (tot, ideal, ideal / tot))
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
+    os.makedirs(args.out, exist_ok=True)
     json.dump({"tag": args.tag, "batch": args.batch, "backbone": args.backbone, "sum_us": round(tot, 1),
                "ideal_us": round(ideal, 1), "rows": rows},
-              open(os.path.join(ROOT, "gpurun_out", "layer_bench_%s.json" % args.tag), "w"), indent=1)
+              open(os.path.join(args.out, "layer_bench_%s.json" % args.tag), "w"), indent=1)
 
 
 if __name__ == "__main__":

@@ -2,10 +2,12 @@
     compute-sanitizer --tool memcheck  python tools/sanitize_cases.py
     compute-sanitizer --tool racecheck python tools/sanitize_cases.py
     compute-sanitizer --tool synccheck python tools/sanitize_cases.py
-Shapes are tiny (the tools slow kernels down 10-100x) but chosen to reach each variant: conv modes 0 / 1 / 3 / 4 / 5,
-2-CTA multicast pairs and cta_group::2 pairs (remote mbarrier arrives), resident weights, bias / residual / upsample on
-the tensor core, TMA-store epilogue, candidate epilogue, fused stem + pool, fused bottleneck tail (bottleneck.cu, all three modes), decode (filter / gather / select), NMS
-(shared-memory aliasing of the sort scratch), rotated NMS, iou, target assignment, the cooperative loss kernel."""
+Shapes are tiny (the tools slow kernels down 10-100x) but chosen to reach each variant of the wgmma kernels and their
+mbarrier rings: conv modes 0 / 1 / 2 / 3 with N tiles 64 and 128, ragged M and N tiles, residual / upsample / ReLU6 /
+fp32 / sigmoid / candidate epilogues, the fused stem + pool (stem.cu: halo rows at the image edges), the fused bottleneck
+tail (bottleneck.cu: C1 64 / 128, projected identity, GEMM3 with 64 / 128 outputs -- shared-memory A operands written
+by the epilogues), decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
+iou, target assignment, the cooperative loss kernel."""
 import os
 import sys
 
@@ -29,7 +31,7 @@ def conv(n, h, w, cin, cout, ks, **kw):
     x, wt, b = rnd(n, h, w, cin), engine.pack_weight(torch.randn((cout, cin, ks, ks), generator=g) * 0.05).to(DEV), torch.randn(cout, generator=g).to(DEV)
     res = rnd(n, h, w, cout) if kw.pop("residual", False) else None
     up = rnd(n, h // 2, w // 2, cout) if kw.pop("upsample", False) else None
-    y = engine.conv2d(x, wt, b, cout, ks, residual=res, upsample=up, bias_op=engine.pack_bias(b), **kw)
+    y = engine.conv2d(x, wt, b, cout, ks, residual=res, upsample=up, **kw)
     torch.cuda.synchronize()
     print("conv %s -> plan %s" % ((n, h, w, cin, cout, ks), {k: v for k, v in engine.last_plan().items() if v}), flush=True)
     return y
@@ -39,13 +41,13 @@ def main():
     only = sys.argv[1] if len(sys.argv) > 1 else ""
     if only in ("", "conv"):
         conv(2, 16, 16, 64, 64, 1, relu=True)                              # mode 0
-        conv(2, 16, 16, 256, 256, 1, relu=True, residual=True)             # residual chunks through the pipeline, TMA store
-        conv(1, 16, 32, 256, 256, 1, upsample=True)                        # upsample-add on the tensor core
-        conv(1, 18, 20, 256, 256, 1, upsample=True)                        # epilogue upsample-add fallback
-        conv(1, 16, 24, 64, 64, 3, relu=True)                              # halo, resident weights
-        conv(1, 7, 10, 256, 256, 3, relu=True)                             # mode 1, shrunk N tile
-        conv(10, 48, 64, 256, 256, 3, relu=True)                           # halo, cta_group::2 pairs (>= 74 pairs)
-        conv(2, 100, 160, 256, 36, 3, out_mode=engine.OUT_NCHW_F32)        # narrow head output, cta_group::2 pairs
+        conv(2, 16, 16, 256, 256, 1, relu=True, residual=True)             # residual epilogue
+        conv(1, 16, 32, 256, 256, 1, upsample=True)                        # upsample-add epilogue
+        conv(1, 18, 20, 256, 256, 1, upsample=True)                        # ragged last M tile
+        conv(1, 16, 24, 64, 64, 3, relu=True)                              # mode 1, N tile 64
+        conv(1, 7, 10, 256, 256, 3, relu=True)                             # mode 1, patch of 70 pixels
+        conv(10, 48, 64, 256, 256, 3, relu=True)                           # mode 1, N tile 128, several tiles per CTA
+        conv(2, 100, 160, 256, 36, 3, out_mode=engine.OUT_NCHW_F32)        # narrow head output, ragged N tile
         conv(1, 24, 32, 256, 720, 3, out_mode=engine.OUT_NCHW_F32_SIGMOID)
         conv(2, 26, 40, 128, 128, 3, relu=True, stride=2)                  # parity-split stride 2
         conv(2, 25, 39, 256, 256, 3, relu=True, stride=2)                  # element-strided boxes
@@ -70,7 +72,7 @@ def main():
             torch.cuda.synchronize()
             print("bottleneck_tail + next conv1 (%d) ok" % c3, flush=True)
         engine.depthwise3x3(rnd(2, 9, 11, 192), rnd(9, 192), torch.randn(192, generator=g).to(DEV), stride=2, act=2)
-        conv(1, 4, 4, 192, 960, 1, relu=2)                                 # ReLU6, 240-wide N tiles (row-store epilogue)
+        conv(1, 48, 48, 192, 960, 1, relu=2)                               # ReLU6, ragged last 128-wide N tile
         torch.cuda.synchronize()
         x = rnd(2, 64, 96, 3)
         wt, b = engine.pack_stem_weight(torch.randn((64, 3, 7, 7), generator=g) * 0.1).to(DEV), torch.randn(64, generator=g).to(DEV)
