@@ -218,6 +218,34 @@ typedef struct {
   int tab_tiles;
 } odtk_conv_t;
 int odtk_conv2d(const odtk_conv_t *desc, odtk_stream_t stream);
+
+/* INT8 convolution (H100-native; the reference's INT8 mode is a TensorRT engine built with its entropy calibrator):
+ * s8 activations x s8 weights on the integer tensor cores, exact s32 accumulation, then per output channel c
+ *     y = fmaf((float)acc, alpha[c], bias[c])      alpha[c] = s_in * s_w[c], computed by the caller in fp32
+ * then ReLU if requested, then one output mode:
+ *     ODTK_OUT_NHWC_S8          y: NHWC s8 [n, h, width, cout], clamp(rint(y * inv_out_scale), -127, 127)
+ *     ODTK_OUT_NCHW_F32[_SIGMOID], ODTK_OUT_CANDIDATES   as for odtk_conv2d
+ * Weights: s8 [cout, ksize*ksize*cin] (tap-major, channel-minor, symmetric per output channel); activations symmetric,
+ * zero-point 0, so zero padding (and the atlas gap rows / columns) stays exact.  Stride 1, ksize 1 or 3, cin % 128 == 0;
+ * anything else returns ODTK_E_UNSUPPORTED.  x_rows / x_width (3x3 only) and tile_tab / tab_tiles are the atlas views of
+ * odtk_conv_t (with a tile table y is a whole atlas like x).                                                          */
+#define ODTK_OUT_NHWC_S8 4
+typedef struct {
+  const void *x;        /* NHWC s8 [n, h, width, cin]                                   */
+  const void *w;        /* s8 [cout, ksize*ksize*cin]                                   */
+  const float *alpha;   /* fp32 [cout]: s_in * s_w[c]                                   */
+  const float *bias;    /* fp32 [cout] or NULL                                          */
+  void *y;
+  int n, h, width, cin, cout, ksize, relu, out_mode;
+  float inv_out_scale;  /* ODTK_OUT_NHWC_S8: 1 / s_out                                  */
+  const odtk_cand_sink_t *sink;
+  int x_rows, x_width;
+  const void *tile_tab;
+  int tab_tiles;
+} odtk_conv_s8_t;
+int odtk_conv2d_s8(const odtk_conv_s8_t *desc, odtk_stream_t stream);
+/* y[i] = clamp(rint((float)x[i] * inv_scale), -127, 127): fp16 -> s8, n % 8 == 0, 16-byte aligned x, 8-byte aligned y. */
+int odtk_quantize_f16_s8(const void *x, void *y, long long n, float inv_scale, odtk_stream_t stream);
 /* Introspection (tests): the kernel variant the last odtk_conv2d / odtk_stem_conv call of the calling host thread
  * launched.  mode: 0 GEMM rows (1x1), 1 shifted box per tap (3x3, odd-size stride 2), 2 stem, 3 even-size stride 2;
  * bn: N tile (64 or 128); grid: persistent CTAs.  cluster, npatch, tile_t, b_resident, bias_mma, res_mma, tma_store and

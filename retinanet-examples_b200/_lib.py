@@ -51,6 +51,8 @@ SIGNATURES = {
     "odtk_gather_wait": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),
     "odtk_iou": (ctypes.c_int, [_c_vpp, _c_vpp, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "odtk_conv2d": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_conv2d_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_quantize_f16_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p]),
     "odtk_conv_last_plan": (ctypes.c_int, [ctypes.c_void_p]),
     "odtk_conv_map_cache_stats": (ctypes.c_int, [ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),
     "odtk_conv_pack_bias": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p]),

@@ -25,6 +25,8 @@
 //   3  stride-2 1x1 / 3x3 on even sizes: parity-split 5-D view {2C, W/2, 2, H/2, N}.
 //   2  7x7 stride-2 stem: overlapping-window 5-D map of the zero-padded NHWC4 image, 64-byte swizzle.
 // Only Cin % 64 != 0 callers (RGB stems other than the 7x7) are first lowered to GEMM rows by layers.cu and run as mode 0.
+// INT8 (odtk_conv2d_s8): the same kernel instantiated on s8 operands -- 128-channel K blocks, wgmma m64nNk32 with s32
+// accumulators, a dequantising epilogue -- in modes 0 and 1 (stride 1).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -32,6 +34,7 @@
 #include <string.h>
 
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 
 #include "common.cuh"
@@ -54,7 +57,9 @@ struct Barriers {
 static_assert(sizeof(Barriers) <= 256, "barrier block too small");
 
 // ---------------------------------------------------------------------------------- kernel
-template <int BN>
+// S8: int8 operands (odtk_conv2d_s8).  A K block is then one 128-byte swizzle row of 128 channels instead of 64, the MMAs
+// are the integer m64nNk32 form with exact s32 accumulators, and the epilogue dequantises with fmaf(acc, alpha, bias).
+template <int BN, bool S8>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
@@ -97,16 +102,16 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // ===================================== TMA producer =====================================
     if (tid != 0) return;
     const uint32_t a_bytes = (uint32_t)((p.mode == 0 ? 128 : p.TH * p.TW) * rb), b_bytes = (uint32_t)(BN * rb);
-    const int kelems = rb >> 1;   // K elements per block: 64 (SW128) or 32 (SW64)
+    const int kelems = S8 ? rb : rb >> 1;   // K elements per block: 64 (SW128) or 32 (SW64); s8: 128
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int m_tile, n_tile, img, h0, w0, hlim, wlim;
       tile_origin(tile, m_tile, n_tile, img, h0, w0, hlim, wlim);
       const int n0 = n_tile * BN;
-      // K order: 64-channel chunk outer, tap inner
+      // K order: 64-channel (s8: 128-channel) chunk outer, tap inner
       for (int kb = 0; kb < p.kblocks_per_tap; kb++) {
-        const int kch = p.grouped ? n0 : kb * 64;   // input-channel coordinate: grouped convs read their own chunk only
+        const int kch = p.grouped ? n0 : kb * (S8 ? 128 : 64);   // input-channel coordinate: grouped convs read their own chunk only
         for (int tap = 0; tap < p.taps; tap++) {
           const int dy = tap / p.kw - p.pad, dx = tap % p.kw - p.pad;
           mbar_wait(&bars->empty[stage], phase ^ 1u);
@@ -144,7 +149,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
   const int q = lane & 3;
   const int hw = p.H * p.W, patch = p.TH * p.TW;
-  float acc[BN / 2];
+  typename std::conditional<S8, int, float>::type acc[BN / 2];
   int stage = 0;
   uint32_t phase = 0;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
@@ -158,7 +163,10 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const uint32_t sa = smem_u32(smem + stage * stage_bytes);
       const uint64_t da = wgmma_desc(sa + (uint32_t)(cw * 64 * brb), brb), db = wgmma_desc(sa + (uint32_t)(128 * brb), brb);
       wgmma_fence();
-      if (brb == 128) {
+      if constexpr (S8) {
+#pragma unroll
+        for (int k = 0; k < 4; k++) WgmmaS8<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+      } else if (brb == 128) {
 #pragma unroll
         for (int k = 0; k < 4; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
       } else {
@@ -176,6 +184,12 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (prev >= 0 && lane == 0) mbar_arrive(&bars->empty[prev]);
 
     // ---- epilogue: thread holds rows r and r + 8, columns 8 j + 2 q (+1) ----
+    // fp32 value of accumulator a in column col before the activation: + bias; s8: fmaf(acc, alpha, bias) (dequantise)
+    auto head_val = [&](int a, int col) -> float {
+      const float b = p.bias ? __ldg(p.bias + col) : 0.0f;
+      if constexpr (S8) return fmaf((float)acc[a], __ldg(p.alpha + col), b);
+      else return acc[a] + b;
+    };
 #pragma unroll
     for (int i = 0; i < 2; i++) {
       const int row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;
@@ -195,7 +209,29 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         h = rem / p.W;
         w = rem - h * p.W;
       }
-      if (p.out_mode == ODTK_OUT_NHWC_F16) {
+      if constexpr (S8) {
+        if (p.out_mode == ODTK_OUT_NHWC_S8) {
+          // requantise for the next s8 layer: one fp32 multiply, round to nearest even, saturate to the symmetric range
+          if (!valid) continue;
+          const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
+          int8_t *o = reinterpret_cast<int8_t *>(p.out) + opix * p.ldy;
+#pragma unroll
+          for (int j = 0; j < BN / 8; j++) {
+            const int col = n0 + 8 * j + 2 * q;
+            if (col >= p.Cout) continue;   // Cout % 16 == 0: both columns of the pair are in range or neither
+            int qv[2];
+#pragma unroll
+            for (int k = 0; k < 2; k++) {
+              float y = head_val(4 * j + 2 * i + k, col + k);
+              if (p.relu) y = fmaxf(y, 0.0f);
+              qv[k] = min(max(__float2int_rn(__fmul_rn(y, p.inv_out_scale)), -127), 127);
+            }
+            *reinterpret_cast<char2 *>(o + col) = make_char2((signed char)qv[0], (signed char)qv[1]);
+          }
+          continue;
+        }
+      }
+      if (!S8 && p.out_mode == ODTK_OUT_NHWC_F16) {
         if (!valid) continue;
         const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
         __half *o = reinterpret_cast<__half *>(p.out) + opix * p.ldy;
@@ -226,7 +262,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         auto score = [&](int j, int k, float &sc) -> bool {
           const int col = n0 + 8 * j + 2 * q + k;
           if (col >= p.Cout) return false;
-          float x = acc[4 * j + 2 * i + k] + (p.bias ? __ldg(p.bias + col) : 0.0f);
+          float x = head_val(4 * j + 2 * i + k, col);
           if (p.relu) x = fmaxf(x, 0.0f);
           if (!(x > p.cand_pre)) return false;
           sc = sigmoidf_accurate(x);
@@ -263,7 +299,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           for (int k = 0; k < 2; k++) {
             const int col = n0 + 8 * j + 2 * q + k;
             if (col >= p.Cout) continue;
-            float x = acc[4 * j + 2 * i + k] + (p.bias ? __ldg(p.bias + col) : 0.0f);
+            float x = head_val(4 * j + 2 * i + k, col);
             if (p.relu) x = fmaxf(x, 0.0f);
             if (p.out_mode == ODTK_OUT_NCHW_F32_SIGMOID) x = sigmoidf_accurate(x);
             o[(long long)col * hw] = x;
@@ -296,7 +332,7 @@ EncodeTiledFn get_encode() {
 // 3-7 driver encodes per convolution (a CUDA-graph replay never did).  Keyed by value; bounded; thread-safe.
 struct MapKey {
   const void *base;
-  int rank, swz;
+  int rank, swz, dtype;
   uint64_t dims[5], strides[4];
   uint32_t box[5], es[5];
   bool operator==(const MapKey &o) const { return memcmp(this, &o, sizeof(MapKey)) == 0; }
@@ -316,10 +352,10 @@ long long g_map_hits = 0, g_map_misses = 0;
 }  // namespace
 
 bool encode_map(CUtensorMap *m, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
-                const uint32_t *box, CUtensorMapSwizzle swz, const uint32_t *elem_strides) {
+                const uint32_t *box, CUtensorMapSwizzle swz, const uint32_t *elem_strides, CUtensorMapDataType dtype) {
   MapKey key;
   memset(&key, 0, sizeof key);
-  key.base = base; key.rank = rank; key.swz = (int)swz;
+  key.base = base; key.rank = rank; key.swz = (int)swz; key.dtype = (int)dtype;
   for (int i = 0; i < rank; i++) { key.dims[i] = dims[i]; key.box[i] = box[i]; key.es[i] = elem_strides ? elem_strides[i] : 1; }
   for (int i = 0; i < rank - 1; i++) key.strides[i] = strides_bytes[i];
   {
@@ -333,7 +369,7 @@ bool encode_map(CUtensorMap *m, const void *base, int rank, const uint64_t *dims
   cuuint32_t bx[5], es[5];
   for (int i = 0; i < rank; i++) { gdim[i] = dims[i]; bx[i] = box[i]; es[i] = key.es[i]; }
   for (int i = 0; i < rank - 1; i++) gstr[i] = strides_bytes[i];
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr, bx, es,
+  CUresult r = fn(m, dtype, (cuuint32_t)rank, const_cast<void *>(base), gdim, gstr, bx, es,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return false;
@@ -362,7 +398,7 @@ void choose_patch(int H, int W, int &TH, int &TW) {
 
 namespace {
 
-template <int BN>
+template <int BN, bool S8>
 void launch_bn(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
                const CUtensorMap &tmB2, const ConvParams &p) {
   cudaLaunchConfig_t cfg = {};
@@ -375,7 +411,7 @@ void launch_bn(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUte
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = odtk_pdl_on() ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN>, tmA, tmB, tmA2, tmB2, p);
+  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, S8>, tmA, tmB, tmA2, tmB2, p);
 }
 
 // Per-device state (one process may drive several GPUs): the > 48 KB dynamic-shared-memory opt-in of every kernel
@@ -389,8 +425,10 @@ bool device_ready() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return false;
   std::lock_guard<std::mutex> lk(g_dev_mu);
   if (g_dev_ready[dev]) return true;
-  if (cudaFuncSetAttribute(conv_gemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
+  if (cudaFuncSetAttribute(conv_gemm_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
     return false;
   g_dev_ready[dev] = true;
   return true;
@@ -404,17 +442,34 @@ void set_stages(ConvParams &p, int BN) {
 }
 
 int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
-           const CUtensorMap &tmB2, cudaStream_t stream) {
+           const CUtensorMap &tmB2, cudaStream_t stream, bool s8 = false) {
   const int total = p.num_m_tiles * p.num_n_tiles;
   const int sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
   const int grid = total < sms ? total : sms;
   g_last_plan = odtk_conv_plan_t{p.mode, 0, BN, p.num_m_tiles, p.num_n_tiles, p.nstages, 0, 0, 0, 0, 0, 0, p.TH, p.TW, grid, 0};
   {
     OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    if (BN == 64) launch_bn<64>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-    else          launch_bn<128>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    if (s8) {
+      if (BN == 64) launch_bn<64, true>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      else          launch_bn<128, true>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    } else {
+      if (BN == 64) launch_bn<64, false>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      else          launch_bn<128, false>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    }
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+// out_mode ODTK_OUT_CANDIDATES: the decode workspace of the level the launch covers
+int set_sink(ConvParams &p, const odtk_cand_sink_t *k, int cout, int h, int width) {
+  if (!k->counts || !k->hist || !k->cand || k->hist_bins <= 0) return ODTK_E_INVALID;
+  if ((long long)cout * h * width >= (1ll << 32)) return ODTK_E_UNSUPPORTED;
+  p.cand_counts = k->counts; p.cand_hist = k->hist; p.cand = (uint2 *)k->cand; p.cand_cap = k->cap;
+  p.cand_key_thresh = k->key_thresh; p.cand_shift = k->shift; p.cand_hist_bins = k->hist_bins;
+  p.cand_thresh = k->thresh;
+  // sigmoid(x) > thresh implies x > logit(thresh) - margin (the SFU sigmoid is accurate to 1e-6 relative)
+  p.cand_pre = (k->thresh > 1e-4f && k->thresh < 0.999f) ? logf(k->thresh / (1.0f - k->thresh)) - 0.05f : -INFINITY;
+  return ODTK_OK;
 }
 
 // odtk_conv2d, plus (mode 0 only) a second operand pair added to the same accumulator: y = x * w^T + x2 * w2^T with
@@ -460,14 +515,8 @@ int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cud
   p.ldr = d->ldr > 0 ? d->ldr : d->cout;
   p.up_h = d->h / 2; p.up_w = d->width / 2;
   if (p.out_mode == ODTK_OUT_CANDIDATES) {
-    const odtk_cand_sink_t *k = d->sink;
-    if (!k->counts || !k->hist || !k->cand || k->hist_bins <= 0) return ODTK_E_INVALID;
-    if ((long long)d->cout * d->h * d->width >= (1ll << 32)) return ODTK_E_UNSUPPORTED;
-    p.cand_counts = k->counts; p.cand_hist = k->hist; p.cand = (uint2 *)k->cand; p.cand_cap = k->cap;
-    p.cand_key_thresh = k->key_thresh; p.cand_shift = k->shift; p.cand_hist_bins = k->hist_bins;
-    p.cand_thresh = k->thresh;
-    // sigmoid(x) > thresh implies x > logit(thresh) - margin (the SFU sigmoid is accurate to 1e-6 relative)
-    p.cand_pre = (k->thresh > 1e-4f && k->thresh < 0.999f) ? logf(k->thresh / (1.0f - k->thresh)) - 0.05f : -INFINITY;
+    const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
+    if (rc != ODTK_OK) return rc;
   }
   if (p.out_mode == ODTK_OUT_NHWC_F16 && (p.ldy % 8)) return ODTK_E_INVALID;
   if ((p.residual && (p.ldr & 1)) || (d->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
@@ -577,6 +626,86 @@ int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cud
   return launch(p, BN, tmA, tmB, tmA2, tmB2, stream);
 }
 
+// odtk_conv2d_s8: the same kernel on s8 operands.  Stride 1 only: 1x1 as GEMM rows (mode 0), 3x3 as shifted boxes
+// (mode 1) over a dense tensor, a level view of the atlas or the whole atlas with its tile table.
+int conv_run_s8(const odtk_conv_s8_t *d, cudaStream_t stream) {
+  if (!d || !d->x || !d->w || !d->alpha) return ODTK_E_INVALID;
+  if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
+  if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
+  if (d->out_mode != ODTK_OUT_NHWC_S8 && d->out_mode != ODTK_OUT_NCHW_F32 && d->out_mode != ODTK_OUT_NCHW_F32_SIGMOID &&
+      d->out_mode != ODTK_OUT_CANDIDATES)
+    return ODTK_E_INVALID;
+  if ((d->ksize != 1 && d->ksize != 3) || d->cin % 128) return ODTK_E_UNSUPPORTED;   // 128-channel K blocks
+  if (d->relu != 0 && d->relu != 1) return ODTK_E_UNSUPPORTED;
+  if (d->out_mode == ODTK_OUT_NHWC_S8 && (d->cout % 16)) return ODTK_E_UNSUPPORTED;
+  if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  if (((uintptr_t)d->x | (uintptr_t)d->w | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15) return ODTK_E_INVALID;
+  const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
+  const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
+  if ((x_view || d->tile_tab) && d->ksize != 3) return ODTK_E_UNSUPPORTED;
+  if (d->tile_tab && (d->tab_tiles <= 0 || x_view)) return ODTK_E_INVALID;
+  if (!device_ready()) return ODTK_E_CUDA;
+  const int sms = odtk_sm_count();
+  ConvParams p;
+  memset(&p, 0, sizeof p);
+  p.N = d->n; p.H = d->h; p.W = d->width; p.Cin = d->cin; p.Cout = d->cout;
+  p.kw = d->ksize; p.taps = d->ksize * d->ksize; p.pad = d->ksize / 2;
+  p.kblocks_per_tap = d->cin / 128;
+  p.row_bytes = 128;
+  p.M = (long long)d->n * d->h * d->width;
+  p.alpha = d->alpha;
+  p.bias = d->bias;
+  p.out = d->y;
+  p.relu = d->relu;
+  p.out_mode = d->out_mode;
+  p.ldy = d->cout;
+  p.ldr = d->cout;
+  p.inv_out_scale = d->inv_out_scale;
+  if (p.out_mode == ODTK_OUT_CANDIDATES) {
+    const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
+    if (rc != ODTK_OK) return rc;
+  }
+  CUtensorMap tmA, tmB;
+  if (d->ksize == 1) {
+    p.mode = 0;
+    p.num_m_tiles = (int)((p.M + 127) / 128);
+    uint64_t dims[2] = {(uint64_t)d->cin, (uint64_t)p.M};
+    uint64_t str[1] = {(uint64_t)d->cin};
+    uint32_t box[2] = {128, 128};
+    if (!encode_map(&tmA, d->x, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
+  } else {
+    p.mode = 1;
+    if (d->tile_tab) {   // atlas tile tables list 8 x 16 pixel tiles
+      p.TH = 8; p.TW = 16;
+      p.tile_tab = (const int4 *)d->tile_tab; p.tab_tiles = d->tab_tiles;
+    } else {
+      choose_patch(d->h, d->width, p.TH, p.TW);
+    }
+    p.tiles_h = (d->h + p.TH - 1) / p.TH;
+    p.tiles_w = (d->width + p.TW - 1) / p.TW;
+    p.num_m_tiles = d->tile_tab ? d->n * d->tab_tiles : d->n * p.tiles_h * p.tiles_w;
+    const uint64_t C = (uint64_t)d->cin;
+    uint64_t dims[4] = {C, (uint64_t)d->width, (uint64_t)d->h, (uint64_t)d->n};
+    uint64_t str[3] = {C, xW * C, xH * xW * C};
+    uint32_t box[4] = {128, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+    if (!encode_map(&tmA, d->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
+  }
+  p.oH = p.H; p.oR = 0; p.oW = p.W;
+  // N tile as for odtk_conv2d
+  int BN = d->cout <= 64 ? 64 : 128;
+  if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
+  p.num_n_tiles = (d->cout + BN - 1) / BN;
+  set_stages(p, BN);
+  {
+    const uint64_t K = (uint64_t)p.taps * d->cin;
+    uint64_t dims[2] = {K, (uint64_t)d->cout};
+    uint64_t str[1] = {K};
+    uint32_t box[2] = {128, (uint32_t)BN};
+    if (!encode_map(&tmB, d->w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
+  }
+  return launch(p, BN, tmA, tmB, tmA, tmB, stream, true);
+}
+
 // bias operand: [cout, 64] fp16 with (hi, lo, 0, ...): hi + lo == bias to 2^-22 relative
 __global__ void pack_bias_kernel(const float *bias, __half *out, int cout) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cout * 64; i += gridDim.x * blockDim.x) {
@@ -595,6 +724,10 @@ __global__ void pack_bias_kernel(const float *bias, __half *out, int cout) {
 
 extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
   return conv_run(d, nullptr, nullptr, 0, (cudaStream_t)stream_);
+}
+
+extern "C" int odtk_conv2d_s8(const odtk_conv_s8_t *d, odtk_stream_t stream_) {
+  return conv_run_s8(d, (cudaStream_t)stream_);
 }
 
 // ResNet stem: 7x7 stride-2 pad-3 convolution of the RGB image, im2col-free.  `xp` is the image

@@ -5,9 +5,11 @@
 #include <stdint.h>
 
 // Host helpers shared by the TMA kernels (conv.cu, bottleneck.cu, stem.cu).
-// Encode a tiled fp16 tensor map (cached per base pointer and geometry); false if the driver rejects it.
+// Encode a tiled tensor map (cached per base pointer, data type and geometry); false if the driver rejects it.  dims and
+// box are in elements of `dtype` (fp16, or UINT8 for int8 bytes).
 bool encode_map(CUtensorMap *m, const void *base, int rank, const uint64_t *dims, const uint64_t *strides_bytes,
-                const uint32_t *box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, const uint32_t *elem_strides = nullptr);
+                const uint32_t *box, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B, const uint32_t *elem_strides = nullptr,
+                CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
 // The spatial patch (TW x TH <= 128 pixels) that wastes the fewest accumulator rows on an H x W image.
 void choose_patch(int H, int W, int &TH, int &TW);
 
@@ -41,4 +43,8 @@ struct ConvParams {
   unsigned cand_key_thresh;
   int cand_shift, cand_hist_bins;
   float cand_thresh, cand_pre;   // candidate iff sigmoid(x) > thresh; x <= cand_pre can never pass
+  // s8 launches (odtk_conv2d_s8): y = fmaf((float)acc, alpha[c], bias[c]); ODTK_OUT_NHWC_S8 stores
+  // clamp(rint(y * inv_out_scale), -127, 127)
+  const float *alpha;
+  float inv_out_scale;
 };

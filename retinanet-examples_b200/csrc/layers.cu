@@ -209,6 +209,24 @@ __global__ void copy_rows_f16_kernel(const __half *__restrict__ x, __half *__res
   }
 }
 
+// fp16 -> s8 with one per-tensor scale (the INT8 heads' input atlas): q = clamp(rint(x * inv_scale), -127, 127), 8
+// elements per thread (16-byte load, 8-byte store).  Zeros stay zeros, so the atlas gap rows remain exact padding.
+__global__ void quantize_f16_s8_kernel(const uint4 *__restrict__ x, uint2 *__restrict__ y, long long n8, float inv_scale) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n8; i += (long long)gridDim.x * blockDim.x) {
+    const uint4 v = __ldg(x + i);
+    const __half2 *h = reinterpret_cast<const __half2 *>(&v);
+    uint32_t out[2] = {0u, 0u};
+#pragma unroll
+    for (int j = 0; j < 4; j++) {
+      const float2 f = __half22float2(h[j]);
+      const int q0 = min(max(__float2int_rn(__fmul_rn(f.x, inv_scale)), -127), 127);
+      const int q1 = min(max(__float2int_rn(__fmul_rn(f.y, inv_scale)), -127), 127);
+      out[j >> 1] |= (((uint32_t)q0 & 0xffu) | (((uint32_t)q1 & 0xffu) << 8)) << (16 * (j & 1));
+    }
+    y[i] = make_uint2(out[0], out[1]);
+  }
+}
+
 inline int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
   long long cap = (long long)odtk_sm_count() * 16;
@@ -334,6 +352,13 @@ extern "C" int odtk_relu_f16(const void *x, void *y, long long n, odtk_stream_t 
   if (!x || !y || n <= 0 || (n % 8) || (((uintptr_t)x | (uintptr_t)y) & 15)) return ODTK_E_INVALID;
   OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
   relu_f16_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream_>>>((const uint4 *)x, (uint4 *)y, n / 8);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_quantize_f16_s8(const void *x, void *y, long long n, float inv_scale, odtk_stream_t stream_) {
+  if (!x || !y || n <= 0 || (n % 8) || ((uintptr_t)x & 15) || ((uintptr_t)y & 7)) return ODTK_E_INVALID;
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  quantize_f16_s8_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream_>>>((const uint4 *)x, (uint2 *)y, n / 8, inv_scale);
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 

@@ -6,7 +6,7 @@ import torch
 
 from . import _lib
 
-OUT_NHWC_F16, OUT_NCHW_F32, OUT_NCHW_F32_SIGMOID, OUT_CANDIDATES = 0, 1, 2, 3
+OUT_NHWC_F16, OUT_NCHW_F32, OUT_NCHW_F32_SIGMOID, OUT_CANDIDATES, OUT_NHWC_S8 = 0, 1, 2, 3, 4
 
 # host-side accounting of what was launched (bench.py reads it): kernels launched by this
 # module and algorithmic convolution FLOPs (2 * pixels * Cout * taps * Cin, unpadded)
@@ -32,6 +32,15 @@ class ConvDesc(ctypes.Structure):
                 ("sink", ctypes.c_void_p), ("groups", ctypes.c_int), ("x_rows", ctypes.c_int), ("x_width", ctypes.c_int),
                 ("y_rows", ctypes.c_int), ("y_row_off", ctypes.c_int), ("y_width", ctypes.c_int), ("tile_tab", ctypes.c_void_p),
                 ("tab_tiles", ctypes.c_int)]
+
+
+class ConvS8Desc(ctypes.Structure):
+    """odtk_conv_s8_t (include/odtk_b200.h)."""
+    _fields_ = [("x", ctypes.c_void_p), ("w", ctypes.c_void_p), ("alpha", ctypes.c_void_p), ("bias", ctypes.c_void_p),
+                ("y", ctypes.c_void_p), ("n", ctypes.c_int), ("h", ctypes.c_int), ("width", ctypes.c_int),
+                ("cin", ctypes.c_int), ("cout", ctypes.c_int), ("ksize", ctypes.c_int), ("relu", ctypes.c_int),
+                ("out_mode", ctypes.c_int), ("inv_out_scale", ctypes.c_float), ("sink", ctypes.c_void_p),
+                ("x_rows", ctypes.c_int), ("x_width", ctypes.c_int), ("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int)]
 
 
 def _stream():
@@ -86,11 +95,24 @@ def pack_bias(bias):
     return out
 
 
+def pack_weight_s8(weight):
+    """[Cout, Cin, kh, kw] fp32 -> (q, s_w): symmetric per-output-channel INT8 weights in the K order of pack_weight,
+    q = clamp(rint(W / s_w[c]), -127, 127) int8 [Cout, kh*kw*Cin], s_w[c] = max|W[c]| / 127 (1 for an all-zero channel)
+    fp32 [Cout]."""
+    w = weight.float()
+    amax = w.abs().amax(dim=(1, 2, 3))
+    s_w = torch.where(amax > 0, amax / 127.0, torch.ones_like(amax))
+    q = torch.round(w / s_w.view(-1, 1, 1, 1)).clamp_(-127, 127)
+    return pack_weight(q).to(torch.int8).contiguous(), s_w.contiguous()
+
+
 class AtlasView:
-    """A level of the pyramid atlas: the top-left h x w rectangle at row `row_off` of an atlas tensor [N, rows, width, C]."""
+    """A level of the pyramid atlas: the top-left h x w rectangle at row `row_off` of an atlas tensor [N, rows, width, C]
+    (fp16, or int8 for the INT8 heads: `elem` bytes per element)."""
 
     def __init__(self, atlas, row_off, h, w):
         self.atlas, self.row_off, self.h, self.w = atlas, int(row_off), int(h), int(w)
+        self.elem = atlas.element_size()
 
     @property
     def shape(self):
@@ -105,7 +127,7 @@ class AtlasView:
         return self.atlas[:, self.row_off:self.row_off + self.h, :self.w, :].contiguous()
 
     def data_ptr(self):
-        return self.atlas.data_ptr() + self.row_off * self.atlas.shape[2] * self.atlas.shape[3] * 2
+        return self.atlas.data_ptr() + self.row_off * self.atlas.shape[2] * self.atlas.shape[3] * self.elem
 
 
 def conv2d(x, w, bias, cout, ksize, relu=False, residual=None, upsample=None, out_mode=OUT_NHWC_F16, out=None,
@@ -152,6 +174,57 @@ def conv2d(x, w, bias, cout, ksize, relu=False, residual=None, upsample=None, ou
                + (px * cout // 2 if upsample is not None else 0),
                n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
                upsample=upsample is not None, out_mode=out_mode)
+    return out
+
+
+def conv2d_s8(x, w, alpha, bias, cout, ksize, relu=False, out_mode=OUT_NHWC_S8, out=None, inv_out_scale=1.0, sink=None,
+              tile_tab=None):
+    """INT8 convolution (odtk_conv2d_s8), stride 1, pad ksize//2.  x: NHWC int8 [N,H,W,Cin] (or an int8 AtlasView);
+    w: int8 [Cout, ksize*ksize*Cin] from pack_weight_s8; alpha fp32 [Cout] = s_in * s_w; bias fp32 [Cout] or None.
+    Returns NHWC int8 [N,H,W,Cout] (out_mode OUT_NHWC_S8, requantised with inv_out_scale) or NCHW fp32 [N,Cout,H,W].
+    tile_tab: x and out are whole int8 atlases, one launch covers every level the table lists."""
+    xv = x if isinstance(x, AtlasView) else None
+    assert xv is not None or (x.is_cuda and x.dtype == torch.int8 and x.is_contiguous())
+    assert (xv.atlas if xv is not None else x).dtype == torch.int8 and w.dtype == torch.int8
+    n, h, wd, cin = x.shape
+    if out_mode == OUT_CANDIDATES:
+        assert sink is not None
+    elif out is None:
+        if out_mode == OUT_NHWC_S8:
+            out = torch.empty((n, h, wd, cout), dtype=torch.int8, device=x.device)
+        else:
+            out = torch.empty((n, cout, h, wd), dtype=torch.float32, device=x.device)
+    d = ConvS8Desc()
+    d.x, d.w, d.alpha, d.y = x.data_ptr(), w.data_ptr(), alpha.data_ptr(), (out.data_ptr() if out is not None else None)
+    d.bias = bias.data_ptr() if bias is not None else None
+    if xv is not None:
+        d.x_rows, d.x_width = xv.atlas.shape[1], xv.atlas.shape[2]
+    if tile_tab is not None:
+        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    d.sink = ctypes.addressof(sink) if sink is not None else None
+    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cin, cout, ksize
+    d.relu, d.out_mode, d.inv_out_scale = int(relu), out_mode, float(inv_out_scale)
+    _lib.check(_lib.lib().odtk_conv2d_s8(ctypes.byref(d), _stream()), "conv2d_s8")
+    STATS["launches"] += 1
+    if STATS["trace"] is not None:
+        # 1-byte operands: activations read once (atlas launches: the pixels of the levels), int8 weights, the output
+        px = n * h * wd if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
+        obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * (1 if out_mode == OUT_NHWC_S8 else 4)
+        _trace("conv%dx%d_s8" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin, px * cin + w.numel() + obytes,
+               n=n, h=h, w=wd, cin=cin, cout=cout, stride=1, residual=False, upsample=False, out_mode=out_mode)
+    return out
+
+
+def quantize_f16_s8(x, inv_scale, out=None):
+    """fp16 tensor -> int8 of the same shape, q = clamp(rint(x * inv_scale), -127, 127) (odtk_quantize_f16_s8)."""
+    assert x.is_cuda and x.dtype == torch.float16 and x.is_contiguous()
+    if out is None:
+        out = torch.empty(x.shape, dtype=torch.int8, device=x.device)
+    assert out.dtype == torch.int8 and out.numel() == x.numel() and out.is_contiguous()
+    _lib.check(_lib.lib().odtk_quantize_f16_s8(ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(out.data_ptr()), x.numel(),
+                                               float(inv_scale), _stream()), "quantize_f16_s8")
+    STATS["launches"] += 1
+    _trace("quantize_s8", 0, x.numel() * 3, n=x.shape[0], h=x.shape[1], w=x.shape[2], cin=x.shape[3])
     return out
 
 

@@ -19,7 +19,7 @@ import os
 import numpy as np
 import torch
 
-from . import _C, box, engine
+from . import _C, box, calib, engine
 
 RESNET_LAYERS = {"ResNet18FPN": ("basic", [2, 2, 2, 2]), "ResNet34FPN": ("basic", [3, 4, 6, 3]),
                  "ResNet50FPN": ("bottleneck", [3, 4, 6, 3]), "ResNet101FPN": ("bottleneck", [3, 4, 23, 3]),
@@ -233,6 +233,10 @@ class Model:
         self._head_streams = None
         self.gather = None            # peer.PeerGather: image-wise sharding, detections pushed to all ranks by the NMS kernel
         self._packed_out = {}
+        self.precision = "fp16"
+        self._int8_table = None       # calibration table of the INT8 heads (set_precision)
+        self._int8 = None             # their packed s8 weights, alpha, bias, requantisation scales
+        self._calib_hook = None
 
     def __repr__(self):
         return '\n'.join(['     model: {}'.format(self.name), '  backbone: {}'.format(self.backbone),
@@ -333,6 +337,7 @@ class Model:
         if self.backbone in MOBILENET:
             self._pack_mobilenet(P)
             self._packed = P
+            self._pack_int8()
             return
         block, layers = RESNET_LAYERS[self.backbone]
         f = "backbones.%s.features." % self.backbone
@@ -360,6 +365,87 @@ class Model:
         for head in ("cls_head", "box_head"):
             P[head] = [conv_b("%s.%d" % (head, i)) for i in (0, 2, 4, 6, 8)]
         self._packed = P
+        self._pack_int8()
+
+    def _pack_int8(self):
+        """s8 weights of the 10 head layers (symmetric, per output channel) and their epilogue constants from the
+        calibration table: alpha[c] = s_in * s_w[c] (fp32), the fp32 bias, inv_out = 1 / s_out for the tower layers."""
+        self._int8 = None
+        if self._int8_table is None or self.device is None:
+            return
+        scales, sd, dev = self._int8_table["scales"], self._sd, self.device
+        P = {"inv_in": float(np.float32(1.0) / np.float32(scales["heads.input"]))}
+        for head in calib.HEADS:
+            layers = []
+            for (s_in, inv), i in zip(calib.layer_scales(scales, head), (0, 2, 4, 6, 8)):
+                w = sd["%s.%d.weight" % (head, i)]
+                b = sd.get("%s.%d.bias" % (head, i))
+                q, s_w = engine.pack_weight_s8(w)
+                alpha = s_w * torch.tensor(s_in, dtype=torch.float32)
+                layers.append({"w": q.to(dev), "alpha": alpha.contiguous().to(dev), "cout": w.shape[0],
+                               "b": b.float().contiguous().to(dev) if b is not None else None,
+                               "inv_out": float(inv) if inv is not None else None})
+            P[head] = layers
+        self._int8 = P
+
+    def set_precision(self, precision, table=None):
+        """"fp16" (default) or "int8": the head towers and the two final head layers run on the s8 tensor cores with the
+        activation scales of `table` (a path or a dict, from `calibrate`); the backbone and the FPN stay fp16, and so does
+        the training-mode forward.  INT8 needs the pyramid atlas (ODTK_MERGED_HEADS=1).  Captured CUDA graphs are dropped."""
+        if precision == "fp16":
+            self._int8_table = None
+            self._int8 = None
+        elif precision == "int8":
+            if table is None:
+                raise ValueError("set_precision('int8') needs a calibration table (Model.calibrate)")
+            if not self.merged_heads:
+                raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
+            self._int8_table = calib.check_table(calib.load_table(table), self.backbone, self.classes, self.num_anchors)
+            if self._packed is not None:
+                self._pack_int8()
+        else:
+            raise ValueError("precision must be 'fp16' or 'int8', got %r" % (precision,))
+        self.precision = precision
+        if getattr(self, "_graphs", None):
+            self._graphs = {}
+        return self
+
+    def calibrate(self, batches, table=None, method="entropy"):
+        """INT8 calibration: eager fp16 forwards over `batches` (each one what `forward` takes) record, for the 9 tensors the
+        INT8 heads quantise (calib.TENSORS), max|x| and then a 2048-bin |x| histogram over the valid atlas pixels (the gap
+        rows / columns are left out).  method "max": threshold max|x|; "entropy": TensorRT's KL-divergence search.  Returns
+        the calibration table and, if `table` is a path, writes it there."""
+        if self._packed is None:
+            raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
+        if method not in ("max", "entropy"):
+            raise ValueError("unknown calibration method %r (max, entropy)" % (method,))
+        if not self.merged_heads:
+            raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
+        batches = list(batches)
+        col = calib.Collector()
+        saved = (self._int8, self.parallel_heads, self.training)
+        self._int8, self.parallel_heads, self.training = None, False, False
+        self._calib_hook = col.observe
+        images = 0
+        try:
+            with torch.no_grad():
+                for phase in ((0, 1) if method == "entropy" else (0,)):
+                    col.phase = phase
+                    for x in batches:
+                        x = x.to(self.device)
+                        if x.dtype == torch.uint8:
+                            self.forward_heads_u8(x)
+                        else:
+                            self.forward_heads(x)
+                        images += x.shape[0] if phase == 0 else 0
+            torch.cuda.synchronize()
+        finally:
+            self._int8, self.parallel_heads, self.training = saved
+            self._calib_hook = None
+        t = calib.make_table(self.backbone, self.classes, self.num_anchors, method, images, col.scales(method))
+        if table is not None:
+            calib.save_table(t, table)
+        return t
 
     def _pack_mobilenet(self, P):
         """MobileNetV2FPN (odtk/backbones/mobilenet.py, fpn.py:92-93).  The tensor-core kernels work on 64-channel K
@@ -564,6 +650,9 @@ class Model:
         cls_mode = engine.OUT_NCHW_F32_SIGMOID if sigmoid else engine.OUT_NCHW_F32
         if isinstance(features[0], engine.AtlasView):
             return self._heads_atlas(features, cls_mode, sinks)
+        if self._int8 is not None and not self.training:
+            raise ValueError("INT8 heads run over the pyramid atlas, which this model does not use (ODTK_MERGED_HEADS=0 "
+                             "or a backbone whose C5 width is not a multiple of 64)")
 
         def chain(head, t, final_mode, sink=None):
             for conv in P[head][:-1]:
@@ -612,12 +701,22 @@ class Model:
         at = self._atlas_for(atlas0.shape[0], sizes, atlas0.device)
         nl = len(views)
         cls_heads, box_heads = [None] * nl, [None] * nl
+        hook = self._calib_hook
+        if hook is not None:              # calibration: the valid atlas pixels of the heads' input and of every tower output
+            if "valid" not in at:
+                valid = torch.zeros(atlas0.shape[1:3], dtype=torch.bool, device=atlas0.device)
+                for r, (h, w) in zip(at["rows"], sizes):
+                    valid[r:r + h, :w] = True
+                at["valid"] = valid
+            hook("heads.input", atlas0[:, at["valid"]])
 
         def tower(head, bufs, final_mode, use_sinks):
             t = atlas0
             for i, conv in enumerate(P[head][:-1]):
                 nxt = bufs[i & 1]
                 conv(t, relu=True, out=nxt, tile_tab=at["tab"], valid_px=at["px"])
+                if hook is not None:
+                    hook("%s.%d" % (head, 2 * i), nxt[:, at["valid"]])
                 t = nxt
             outs = []
             for l, v in enumerate(views):
@@ -628,9 +727,36 @@ class Model:
                     outs.append(P[head][-1](lv, out_mode=final_mode))
             return outs
 
+        i8 = self._int8 if not self.training else None
+        if i8 is not None:
+            # INT8: the fp16 atlas is quantised once (main stream, before the fork); towers and final layers run on s8
+            if "buf8" not in at:
+                at["buf8"] = [torch.zeros(atlas0.shape, dtype=torch.int8, device=atlas0.device) for _ in range(5)]
+            q_in = engine.quantize_f16_s8(atlas0, i8["inv_in"], out=at["buf8"][0])
+
+            def tower8(head, bufs, final_mode, use_sinks):
+                t = q_in
+                for i, layer in enumerate(i8[head][:-1]):
+                    nxt = bufs[i & 1]
+                    engine.STATS["conv_flops"] += 2 * at["px"] * 256 * 9 * 256
+                    engine.conv2d_s8(t, layer["w"], layer["alpha"], layer["b"], layer["cout"], 3, relu=True,
+                                     out_mode=engine.OUT_NHWC_S8, out=nxt, inv_out_scale=layer["inv_out"], tile_tab=at["tab"])
+                    t = nxt
+                last, outs = i8[head][-1], []
+                for l, v in enumerate(views):
+                    lv = engine.AtlasView(t, at["rows"][l], v.h, v.w)
+                    engine.STATS["conv_flops"] += 2 * lv.shape[0] * v.h * v.w * last["cout"] * 9 * 256
+                    mode, sink = (engine.OUT_CANDIDATES, use_sinks[l]) if use_sinks is not None else (final_mode, None)
+                    outs.append(engine.conv2d_s8(lv, last["w"], last["alpha"], last["b"], last["cout"], 3, out_mode=mode, sink=sink))
+                return outs
+
+            tower, bufs = tower8, at["buf8"]
+        else:
+            bufs = at["buf"]
+
         if not self.parallel_heads:
-            cls_heads = tower("cls_head", at["buf"][1:3], cls_mode, sinks)
-            box_heads = tower("box_head", at["buf"][3:5], engine.OUT_NCHW_F32, None)
+            cls_heads = tower("cls_head", bufs[1:3], cls_mode, sinks)
+            box_heads = tower("box_head", bufs[3:5], engine.OUT_NCHW_F32, None)
             return cls_heads, box_heads
         main = torch.cuda.current_stream()
         if self._head_streams is None or len(self._head_streams) < 1:
@@ -640,10 +766,10 @@ class Model:
         fork.record(main)
         side.wait_event(fork)
         with torch.cuda.stream(side):
-            box_heads = tower("box_head", at["buf"][3:5], engine.OUT_NCHW_F32, None)
+            box_heads = tower("box_head", bufs[3:5], engine.OUT_NCHW_F32, None)
             join = torch.cuda.Event()
             join.record(side)
-        cls_heads = tower("cls_head", at["buf"][1:3], cls_mode, sinks)
+        cls_heads = tower("cls_head", bufs[1:3], cls_mode, sinks)
         main.wait_event(join)
         return cls_heads, box_heads
 

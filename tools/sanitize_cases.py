@@ -6,7 +6,7 @@ Shapes are tiny (the tools slow kernels down 10-100x) but chosen to reach each v
 mbarrier rings: conv modes 0 / 1 / 2 / 3 with N tiles 64 and 128, ragged M and N tiles, residual / upsample / ReLU6 /
 fp32 / sigmoid / candidate epilogues, the fused stem + pool (stem.cu: halo rows at the image edges), the fused bottleneck
 tail (bottleneck.cu: C1 64 / 128, projected identity, GEMM3 with 64 / 128 outputs -- shared-memory A operands written
-by the epilogues), decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
+by the epilogues), the s8 instantiation of the conv kernel and the INT8 heads of the model, decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
 iou, target assignment, the cooperative loss kernel."""
 import os
 import sys
@@ -81,15 +81,29 @@ def main():
         engine.relu(rnd(2, 13, 20, 256))
         torch.cuda.synchronize()
         print("stem ok", flush=True)
+        # s8 kernel: N tiles 64 / 128, s8 NHWC requantising epilogue, fp32 sigmoid epilogue with a ragged N tile, 1x1 rows
+        for n, h, w, cin, cout, ks, mode in ((1, 16, 24, 256, 256, 3, engine.OUT_NHWC_S8), (10, 48, 64, 256, 256, 3, engine.OUT_NHWC_S8),
+                                             (1, 13, 20, 256, 720, 3, engine.OUT_NCHW_F32_SIGMOID), (2, 16, 24, 128, 64, 1, engine.OUT_NHWC_S8)):
+            xq = engine.quantize_f16_s8(rnd(n, h, w, cin), 20.0)
+            wq, s_w = engine.pack_weight_s8(torch.randn((cout, cin, ks, ks), generator=g) * 0.05)
+            engine.conv2d_s8(xq, wq.to(DEV), (s_w * 0.05).to(DEV), torch.randn(cout, generator=g).to(DEV), cout, ks,
+                             relu=mode == engine.OUT_NHWC_S8, out_mode=mode, inv_out_scale=0.1)
+            torch.cuda.synchronize()
+            print("conv_s8 %s -> plan %s" % ((n, h, w, cin, cout, ks), {k: v for k, v in engine.last_plan().items() if v}), flush=True)
     if only in ("", "model"):
         for rotated in (False, True):
             classes, na = 4, 27 if rotated else 9
             sd = make_state_dict("ResNet18FPN", classes, na, rotated, seed=1)
             sd["cls_head.8.bias"] = torch.full_like(sd["cls_head.8.bias"], -2.5)
             m = Model("ResNet18FPN", classes=classes, rotated_bbox=rotated).load_state_dict(sd).cuda(0)
-            out = m(torch.randn((2, 3, 128, 256), generator=g).to(DEV))     # fused candidate epilogue -> decode -> nms
+            x = torch.randn((2, 3, 128, 256), generator=g).to(DEV)
+            out = m(x)                                                      # fused candidate epilogue -> decode -> nms
             torch.cuda.synchronize()
             print("model rotated=%s detections=%d" % (rotated, int((out[0] > 0).sum())), flush=True)
+            m.set_precision("int8", m.calibrate([x], method="max"))       # INT8 heads: quantise, s8 towers over the atlas, s8 candidates
+            out = m(x)
+            torch.cuda.synchronize()
+            print("model int8 rotated=%s detections=%d" % (rotated, int((out[0] > 0).sum())), flush=True)
     if only in ("", "postproc"):
         cls, deltas = synth.head_outputs(1, seed=0)
         anchors = [box.generate_anchors(s, box.DEFAULT_RATIOS, box.DEFAULT_SCALES).reshape(-1).tolist() for s in synth.LEVEL_STRIDES]
