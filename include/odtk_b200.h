@@ -244,6 +244,29 @@ typedef struct {
   int tab_tiles;
 } odtk_conv_s8_t;
 int odtk_conv2d_s8(const odtk_conv_s8_t *desc, odtk_stream_t stream);
+/* INT8 convolution with the backbone / FPN features (H100-native; odtk_conv2d_s8 is this call with the extension zeroed):
+ *   stride     0/1, or 2 (pad ksize/2; y is [n, (h-1)/2+1, (width-1)/2+1, cout]): the parity-split view on even sizes,
+ *              element-strided boxes on odd sizes or an x view, as for odtk_conv2d.
+ *   residual   NHWC s8 [n, oh, ow, cout] (the output geometry) or NULL;  t = fmaf((float)r, res_scale, t)
+ *   upsample   NHWC s8 [n, h/2, width/2, cout] (stride 1, h and width even) or NULL;
+ *              t = fmaf((float)u, up_scale, t) with u the addend at (row >> 1, column >> 1): FPN nearest-2x upsample-add
+ *   y_rows, y_row_off, y_width   ODTK_OUT_NHWC_S8 output into a level view of an atlas, as in odtk_conv_t (3x3 only)
+ * The addends follow fmaf(acc, alpha, bias) in this order, then ReLU and requantisation.  Addends and output views need
+ * out_mode ODTK_OUT_NHWC_S8; views and tile tables take no addends; anything else returns ODTK_E_UNSUPPORTED.           */
+typedef struct {
+  odtk_conv_s8_t base;
+  int stride;
+  const void *residual;
+  float res_scale;
+  const void *upsample;
+  float up_scale;
+  int y_rows, y_row_off, y_width;
+} odtk_conv_s8_ex_t;
+int odtk_conv2d_s8_ex(const odtk_conv_s8_ex_t *desc, odtk_stream_t stream);
+/* s8 twin of odtk_copy_rows_f16 with ReLU: y = max(x, 0) over n x rows runs of row_elems int8 (pitches in elements,
+ * everything a multiple of 16, 16-byte aligned): the input of FPN pyramid7, ReLU(P6), from a level of the s8 atlas. */
+int odtk_relu_copy_rows_s8(const void *x, void *y, int n, int rows, int row_elems, long long x_img_pitch,
+                           long long x_row_pitch, long long y_img_pitch, long long y_row_pitch, odtk_stream_t stream);
 /* y[i] = clamp(rint((float)x[i] * inv_scale), -127, 127): fp16 -> s8, n % 8 == 0, 16-byte aligned x, 8-byte aligned y. */
 int odtk_quantize_f16_s8(const void *x, void *y, long long n, float inv_scale, odtk_stream_t stream);
 /* Introspection (tests): the kernel variant the last odtk_conv2d / odtk_stem_conv call of the calling host thread

@@ -52,6 +52,9 @@ SIGNATURES = {
     "odtk_iou": (ctypes.c_int, [_c_vpp, _c_vpp, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "odtk_conv2d": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     "odtk_conv2d_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_conv2d_s8_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_relu_copy_rows_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int] +
+                               [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     "odtk_quantize_f16_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p]),
     "odtk_conv_last_plan": (ctypes.c_int, [ctypes.c_void_p]),
     "odtk_conv_map_cache_stats": (ctypes.c_int, [ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),

@@ -5,18 +5,43 @@ two final head layers run on the s8 wgmma kernel (engine.conv2d_s8); this module
 (one for the atlas the FPN writes, one per tower layer output) from fp16 forward passes.  One scale covers all five pyramid
 levels, because the atlas is one tensor read by one launch (TensorRT scales P3 ... P7 separately).
 
+Network scope (Model.set_precision("int8", table, scope="network")) also runs ResNet layer3, layer4 and the FPN in INT8; its
+tables (format 2) add one scale per tensor that scope quantises (network_tensors), named by state_dict prefix.  The FPN's
+smooth / pyramid outputs are the atlas, so they use "heads.input".
+
 Offline code: it uses torch / numpy ops and never runs on the inference path."""
 import json
 
 import numpy as np
 import torch
 
-FORMAT = 1
+FORMAT = 1             # heads scope
+FORMAT_NETWORK = 2     # network scope: a superset of the heads scales
+SCOPES = ("heads", "network")
 NBINS = 2048
 LEVELS = 128          # quantisation levels of the symmetric s8 range on one side of zero (TensorRT: 128)
 HEADS = ("cls_head", "box_head")
 TOWER = (0, 2, 4, 6)
 TENSORS = ("heads.input",) + tuple("%s.%d" % (h, i) for h in HEADS for i in TOWER)
+
+
+def network_tensors(backbone):
+    """The tensors the network scope quantises besides the 9 head tensors, in forward order: C3 (layer2's output), then per
+    block of layer3 / layer4 its convolutions' ReLU outputs except the last, its downsample output (first block) and the
+    block output, then P5, P4 and P3 (lateral5, and lateral4 / lateral3 after the top-down add).  ValueError for a backbone
+    the scope does not cover (ResNeXt's grouped 3x3, MobileNetV2)."""
+    from .model import RESNET_LAYERS, RESNEXT
+    if backbone not in RESNET_LAYERS or backbone in RESNEXT:
+        raise ValueError("INT8 network scope covers the ResNet18/34/50/101/152 FPN backbones, not %r" % (backbone,))
+    block, layers = RESNET_LAYERS[backbone]
+    f = "backbones.%s.features." % backbone
+    names = [f + "layer2"]
+    convs = ("conv1", "conv2") if block == "bottleneck" else ("conv1",)
+    for li in (3, 4):
+        for b in range(layers[li - 1]):
+            p = f + "layer%d.%d" % (li, b)
+            names += [p + "." + c for c in convs] + ([p + ".downsample"] if b == 0 else []) + [p]
+    return names + ["backbones.%s.lateral%d" % (backbone, k) for k in (5, 4, 3)]
 
 
 def max_threshold(absmax):
@@ -102,17 +127,24 @@ class Collector:
             return {n: entropy_threshold(self.hist.get(n, np.zeros(NBINS)), self.absmax[n]) for n in self.absmax}
         raise ValueError("unknown calibration method %r (max, entropy)" % (method,))
 
-    def scales(self, method):
+    def scales(self, method, names=TENSORS):
         th = self.thresholds(method)
-        missing = [n for n in TENSORS if n not in th]
+        missing = [n for n in names if n not in th]
         if missing:
             raise RuntimeError("calibration saw no values for %s" % missing)
-        return {n: scale_from_threshold(th[n]) for n in TENSORS}
+        return {n: scale_from_threshold(th[n]) for n in names}
 
 
-def make_table(backbone, classes, num_anchors, method, images, scales):
-    return {"format": FORMAT, "backbone": backbone, "classes": int(classes), "num_anchors": int(num_anchors),
-            "method": method, "images": int(images), "scales": {n: float(scales[n]) for n in TENSORS}}
+def table_tensors(backbone, scope="heads"):
+    return TENSORS + (tuple(network_tensors(backbone)) if scope == "network" else ())
+
+
+def make_table(backbone, classes, num_anchors, method, images, scales, scope="heads"):
+    t = {"format": FORMAT, "backbone": backbone, "classes": int(classes), "num_anchors": int(num_anchors),
+         "method": method, "images": int(images), "scales": {n: float(scales[n]) for n in table_tensors(backbone, scope)}}
+    if scope == "network":
+        t.update(format=FORMAT_NETWORK, scope="network")
+    return t
 
 
 def save_table(table, path):
@@ -128,15 +160,24 @@ def load_table(table):
         return json.load(f)
 
 
-def check_table(table, backbone, classes, num_anchors):
-    """Raises ValueError unless `table` is a calibration table of this model's heads."""
-    if not isinstance(table, dict) or table.get("format") != FORMAT:
-        raise ValueError("not an INT8 calibration table (format %d)" % FORMAT)
+def check_table(table, backbone, classes, num_anchors, scope="heads"):
+    """Raises ValueError unless `table` is a calibration table of this model for `scope`: "heads" takes a format-1 table or
+    a format-2 network table (whose head scales it uses), "network" only a format-2 one."""
+    if scope not in SCOPES:
+        raise ValueError("INT8 scope must be 'heads' or 'network', got %r" % (scope,))
+    if not isinstance(table, dict) or table.get("format") not in (FORMAT, FORMAT_NETWORK):
+        raise ValueError("not an INT8 calibration table (format %d or %d)" % (FORMAT, FORMAT_NETWORK))
+    if table["format"] == FORMAT_NETWORK and table.get("scope") != "network":
+        raise ValueError("a format-%d calibration table must have scope 'network'" % FORMAT_NETWORK)
+    if scope == "network" and table["format"] != FORMAT_NETWORK:
+        raise ValueError("INT8 network scope needs a network calibration table (format %d): calibrate(..., scope='network')"
+                         % FORMAT_NETWORK)
     for key, want in (("backbone", backbone), ("classes", classes), ("num_anchors", num_anchors)):
         if table.get(key) != want:
             raise ValueError("calibration table is for %s=%r, the model has %r" % (key, table.get(key), want))
     scales = table.get("scales", {})
-    bad = [n for n in TENSORS if not (isinstance(scales.get(n), (int, float)) and scales[n] > 0 and np.isfinite(scales[n]))]
+    names = table_tensors(backbone, "network" if table["format"] == FORMAT_NETWORK else "heads")
+    bad = [n for n in names if not (isinstance(scales.get(n), (int, float)) and scales[n] > 0 and np.isfinite(scales[n]))]
     if bad:
         raise ValueError("calibration table lacks a positive scale for %s" % bad)
     return table

@@ -25,8 +25,8 @@
 //   3  stride-2 1x1 / 3x3 on even sizes: parity-split 5-D view {2C, W/2, 2, H/2, N}.
 //   2  7x7 stride-2 stem: overlapping-window 5-D map of the zero-padded NHWC4 image, 64-byte swizzle.
 // Only Cin % 64 != 0 callers (RGB stems other than the 7x7) are first lowered to GEMM rows by layers.cu and run as mode 0.
-// INT8 (odtk_conv2d_s8): the same kernel instantiated on s8 operands -- 128-channel K blocks, wgmma m64nNk32 with s32
-// accumulators, a dequantising epilogue -- in modes 0 and 1 (stride 1).
+// INT8 (odtk_conv2d_s8 / _ex): the same kernel instantiated on s8 operands -- 128-channel K blocks, wgmma m64nNk32 with s32
+// accumulators, a dequantising epilogue (+ s8 residual / upsample addends) -- in modes 0, 1 (incl. s2) and 3.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -215,14 +215,21 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (!valid) continue;
           const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
           int8_t *o = reinterpret_cast<int8_t *>(p.out) + opix * p.ldy;
+          const int8_t *res = p.res8 ? p.res8 + m * p.Cout : nullptr;
+          const int8_t *up = p.up8 ? p.up8 + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
 #pragma unroll
           for (int j = 0; j < BN / 8; j++) {
             const int col = n0 + 8 * j + 2 * q;
             if (col >= p.Cout) continue;   // Cout % 16 == 0: both columns of the pair are in range or neither
+            const char2 r = res ? *reinterpret_cast<const char2 *>(res + col) : make_char2(0, 0);
+            const char2 u = up ? *reinterpret_cast<const char2 *>(up + col) : make_char2(0, 0);
             int qv[2];
 #pragma unroll
             for (int k = 0; k < 2; k++) {
               float y = head_val(4 * j + 2 * i + k, col + k);
+              // one correctly rounded fma per addend, in this order (DESIGN §2)
+              if (res) y = fmaf((float)(k ? r.y : r.x), p.res_scale, y);
+              if (up) y = fmaf((float)(k ? u.y : u.x), p.up_scale, y);
               if (p.relu) y = fmaxf(y, 0.0f);
               qv[k] = min(max(__float2int_rn(__fmul_rn(y, p.inv_out_scale)), -127), 127);
             }
@@ -472,6 +479,78 @@ int set_sink(ConvParams &p, const odtk_cand_sink_t *k, int cout, int h, int widt
   return ODTK_OK;
 }
 
+// A operand of a 1x1 / 3x3, stride 1 / 2 launch: the mode, the output patch and tile grid, and the tensor map of x (the
+// top-left h x width rectangle of images xH x xW pixels apart).  es: bytes per element, 2 (fp16) or 1 (s8); a K block is
+// one 128-byte swizzle row of channels either way.  Shared by odtk_conv2d and odtk_conv2d_s8_ex.
+int a_operand(ConvParams &p, CUtensorMap &tmA, const void *x, int n, int h, int width, int cin, int ksize, int stride,
+              uint64_t xH, uint64_t xW, bool x_view, const void *tile_tab, int tab_tiles, bool upsample, int es) {
+  const CUtensorMapDataType dt = es == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const uint32_t kc = 128 / es;   // channels per K block
+  const uint64_t C = (uint64_t)cin, W = (uint64_t)width, H = (uint64_t)h;
+  if (stride == 2 && ((h & 1) || (width & 1) || x_view)) {
+    // stride-2 1x1 / 3x3 (pad ksize/2) on odd sizes, im2col-free: one box per tap whose W and H dimensions are
+    // traversed with element stride 2 (boxDim = 2 * pixels, elementStrides = 2: the TMA unit loads every second
+    // pixel); the box origin 2*o + d may be -1 or reach past the edge: zero-filled == padding.
+    const int OH = (h - 1) / 2 + 1, OW = (width - 1) / 2 + 1;
+    p.mode = 1;
+    p.s2 = 1;
+    p.H = OH; p.W = OW;
+    p.M = (long long)n * OH * OW;
+    p.up_h = OH / 2; p.up_w = OW / 2;
+    choose_patch(OH, OW, p.TH, p.TW);
+    if (2 * p.TW > 256 || 2 * p.TH > 256) return ODTK_E_UNSUPPORTED;
+    p.tiles_h = (OH + p.TH - 1) / p.TH;
+    p.tiles_w = (OW + p.TW - 1) / p.TW;
+    p.num_m_tiles = n * p.tiles_h * p.tiles_w;
+    uint64_t dims[4] = {C, W, H, (uint64_t)n};
+    uint64_t str[3] = {C * es, xW * C * es, xH * xW * C * es};
+    uint32_t box[4] = {kc, (uint32_t)(2 * p.TW), (uint32_t)(2 * p.TH), 1};
+    uint32_t estr[4] = {1, 2, 2, 1};
+    if (!encode_map(&tmA, x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, estr, dt)) return ODTK_E_CUDA;
+  } else if (stride == 2) {
+    // stride-2 1x1 / 3x3 (pad ksize/2) on even-sized inputs: 5-D parity-split view of the NHWC tensor
+    // {2C (column parity x channel), W/2, 2 (row parity), H/2, N}; out-of-range half-rows/columns
+    // (the -1 of the top/left taps) are zero-filled by the TMA unit == padding.
+    if (upsample) return ODTK_E_UNSUPPORTED;
+    const int OH = h / 2, OW = width / 2;
+    p.mode = 3;
+    p.H = OH; p.W = OW;
+    p.M = (long long)n * OH * OW;
+    p.up_h = OH / 2; p.up_w = OW / 2;
+    choose_patch(OH, OW, p.TH, p.TW);
+    p.tiles_h = (OH + p.TH - 1) / p.TH;
+    p.tiles_w = (OW + p.TW - 1) / p.TW;
+    p.num_m_tiles = n * p.tiles_h * p.tiles_w;
+    uint64_t dims[5] = {2 * C, W / 2, 2, H / 2, (uint64_t)n};
+    uint64_t str[4] = {2 * C * es, W * C * es, 2 * W * C * es, H * W * C * es};
+    uint32_t box[5] = {kc, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
+    if (!encode_map(&tmA, x, 5, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, dt)) return ODTK_E_CUDA;
+  } else if (ksize == 1) {
+    p.mode = 0;
+    p.num_m_tiles = (int)((p.M + 127) / 128);
+    uint64_t dims[2] = {C, (uint64_t)p.M};
+    uint64_t str[1] = {C * es};
+    uint32_t box[2] = {kc, 128};
+    if (!encode_map(&tmA, x, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, dt)) return ODTK_E_CUDA;
+  } else {
+    p.mode = 1;
+    if (tile_tab) {   // atlas tile tables list 8 x 16 pixel tiles
+      p.TH = 8; p.TW = 16;
+      p.tile_tab = (const int4 *)tile_tab; p.tab_tiles = tab_tiles;
+    } else {
+      choose_patch(h, width, p.TH, p.TW);
+    }
+    p.tiles_h = (h + p.TH - 1) / p.TH;
+    p.tiles_w = (width + p.TW - 1) / p.TW;
+    p.num_m_tiles = tile_tab ? n * tab_tiles : n * p.tiles_h * p.tiles_w;
+    uint64_t dims[4] = {C, W, H, (uint64_t)n};
+    uint64_t str[3] = {C * es, xW * C * es, xH * xW * C * es};
+    uint32_t box[4] = {kc, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+    if (!encode_map(&tmA, x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, dt)) return ODTK_E_CUDA;
+  }
+  return ODTK_OK;
+}
+
 // odtk_conv2d, plus (mode 0 only) a second operand pair added to the same accumulator: y = x * w^T + x2 * w2^T with
 // x2 [M, c2in], w2 [cout, c2in] (the projected identity of a bottleneck block)
 int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cudaStream_t stream) {
@@ -532,70 +611,9 @@ int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cud
   if (x2 && (d->ksize != 1 || stride != 1 || c2in <= 0 || c2in % 64 || !w2 || (((uintptr_t)x2 | (uintptr_t)w2) & 15))) return ODTK_E_INVALID;
 
   CUtensorMap tmA;
-  if (stride == 2 && ((d->h & 1) || (d->width & 1) || x_view)) {
-    // stride-2 1x1 / 3x3 (pad ksize/2) on odd sizes, im2col-free: one box per tap whose W and H dimensions are
-    // traversed with element stride 2 (boxDim = 2 * pixels, elementStrides = 2: the TMA unit loads every second
-    // pixel); the box origin 2*o + d may be -1 or reach past the edge: zero-filled == padding.
-    const int OH = (d->h - 1) / 2 + 1, OW = (d->width - 1) / 2 + 1;
-    p.mode = 1;
-    p.s2 = 1;
-    p.H = OH; p.W = OW;
-    p.M = (long long)d->n * OH * OW;
-    p.up_h = OH / 2; p.up_w = OW / 2;
-    choose_patch(OH, OW, p.TH, p.TW);
-    if (2 * p.TW > 256 || 2 * p.TH > 256) return ODTK_E_UNSUPPORTED;
-    p.tiles_h = (OH + p.TH - 1) / p.TH;
-    p.tiles_w = (OW + p.TW - 1) / p.TW;
-    p.num_m_tiles = d->n * p.tiles_h * p.tiles_w;
-    const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->width, H = (uint64_t)d->h;
-    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-    uint64_t str[3] = {C * 2, xW * C * 2, xH * xW * C * 2};
-    uint32_t box[4] = {64, (uint32_t)(2 * p.TW), (uint32_t)(2 * p.TH), 1};
-    uint32_t es[4] = {1, 2, 2, 1};
-    if (!encode_map(&tmA, d->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, es)) return ODTK_E_CUDA;
-  } else if (stride == 2) {
-    // stride-2 1x1 / 3x3 (pad ksize/2) on even-sized inputs: 5-D parity-split view of the NHWC tensor
-    // {2C (column parity x channel), W/2, 2 (row parity), H/2, N}; out-of-range half-rows/columns
-    // (the -1 of the top/left taps) are zero-filled by the TMA unit == padding.
-    if (d->upsample) return ODTK_E_UNSUPPORTED;
-    const int OH = d->h / 2, OW = d->width / 2;
-    p.mode = 3;
-    p.H = OH; p.W = OW;
-    p.M = (long long)d->n * OH * OW;
-    p.up_h = OH / 2; p.up_w = OW / 2;
-    choose_patch(OH, OW, p.TH, p.TW);
-    p.tiles_h = (OH + p.TH - 1) / p.TH;
-    p.tiles_w = (OW + p.TW - 1) / p.TW;
-    p.num_m_tiles = d->n * p.tiles_h * p.tiles_w;
-    const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->width, H = (uint64_t)d->h;
-    uint64_t dims[5] = {2 * C, W / 2, 2, H / 2, (uint64_t)d->n};
-    uint64_t str[4] = {2 * C * 2, W * C * 2, 2 * W * C * 2, H * W * C * 2};
-    uint32_t box[5] = {64, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
-    if (!encode_map(&tmA, d->x, 5, dims, str, box)) return ODTK_E_CUDA;
-  } else if (d->ksize == 1) {
-    p.mode = 0;
-    p.num_m_tiles = (int)((p.M + 127) / 128);
-    uint64_t dims[2] = {(uint64_t)d->cin, (uint64_t)p.M};
-    uint64_t str[1] = {(uint64_t)d->cin * 2};
-    uint32_t box[2] = {64, 128};
-    if (!encode_map(&tmA, d->x, 2, dims, str, box)) return ODTK_E_CUDA;
-  } else {
-    p.mode = 1;
-    if (d->tile_tab) {   // atlas tile tables list 8 x 16 pixel tiles
-      p.TH = 8; p.TW = 16;
-      p.tile_tab = (const int4 *)d->tile_tab; p.tab_tiles = d->tab_tiles;
-    } else {
-      choose_patch(d->h, d->width, p.TH, p.TW);
-    }
-    p.tiles_h = (d->h + p.TH - 1) / p.TH;
-    p.tiles_w = (d->width + p.TW - 1) / p.TW;
-    p.num_m_tiles = d->tile_tab ? d->n * d->tab_tiles : d->n * p.tiles_h * p.tiles_w;
-    const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->width, H = (uint64_t)d->h;
-    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-    uint64_t str[3] = {C * 2, xW * C * 2, xH * xW * C * 2};
-    uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
-    if (!encode_map(&tmA, d->x, 4, dims, str, box)) return ODTK_E_CUDA;
-  }
+  const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
+                           d->tab_tiles, d->upsample != nullptr, 2);
+  if (rc != ODTK_OK) return rc;
   p.oH = d->y_rows > 0 ? d->y_rows : p.H;
   p.oR = d->y_row_off > 0 ? d->y_row_off : 0;
   p.oW = d->y_width > 0 ? d->y_width : p.W;
@@ -626,10 +644,14 @@ int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cud
   return launch(p, BN, tmA, tmB, tmA2, tmB2, stream);
 }
 
-// odtk_conv2d_s8: the same kernel on s8 operands.  Stride 1 only: 1x1 as GEMM rows (mode 0), 3x3 as shifted boxes
-// (mode 1) over a dense tensor, a level view of the atlas or the whole atlas with its tile table.
-int conv_run_s8(const odtk_conv_s8_t *d, cudaStream_t stream) {
-  if (!d || !d->x || !d->w || !d->alpha) return ODTK_E_INVALID;
+// odtk_conv2d_s8_ex: the same kernel on s8 operands, with the geometry of odtk_conv2d: 1x1 as GEMM rows (mode 0), 3x3 as
+// shifted boxes (mode 1) over a dense tensor, a level view of the atlas or the whole atlas with its tile table, stride 2 on
+// the parity-split view (mode 3, even sizes) or element-strided boxes (odd sizes, level views).  NHWC s8 outputs may add a
+// residual and / or a nearest-upsampled addend, and may land in a level view of an atlas.
+int conv_run_s8(const odtk_conv_s8_ex_t *e, cudaStream_t stream) {
+  if (!e) return ODTK_E_INVALID;
+  const odtk_conv_s8_t *d = &e->base;
+  if (!d->x || !d->w || !d->alpha) return ODTK_E_INVALID;
   if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
   if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
   if (d->out_mode != ODTK_OUT_NHWC_S8 && d->out_mode != ODTK_OUT_NCHW_F32 && d->out_mode != ODTK_OUT_NCHW_F32_SIGMOID &&
@@ -640,10 +662,18 @@ int conv_run_s8(const odtk_conv_s8_t *d, cudaStream_t stream) {
   if (d->out_mode == ODTK_OUT_NHWC_S8 && (d->cout % 16)) return ODTK_E_UNSUPPORTED;
   if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
   if (((uintptr_t)d->x | (uintptr_t)d->w | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15) return ODTK_E_INVALID;
+  const int stride = e->stride > 1 ? e->stride : 1;
+  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
   const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
   const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
-  if ((x_view || d->tile_tab) && d->ksize != 3) return ODTK_E_UNSUPPORTED;
-  if (d->tile_tab && (d->tab_tiles <= 0 || x_view)) return ODTK_E_INVALID;
+  const bool y_view = e->y_rows > 0 || e->y_width > 0 || e->y_row_off > 0;
+  const bool addend = e->residual || e->upsample;
+  // addends and output views: NHWC s8 only; views and tile tables: 3x3 without addends (as odtk_conv2d)
+  if ((addend || y_view) && d->out_mode != ODTK_OUT_NHWC_S8) return ODTK_E_UNSUPPORTED;
+  if ((x_view || y_view || d->tile_tab) && (d->ksize != 3 || addend)) return ODTK_E_UNSUPPORTED;
+  if (e->upsample && stride != 1) return ODTK_E_UNSUPPORTED;
+  if (d->tile_tab && (d->tab_tiles <= 0 || x_view || y_view || stride != 1)) return ODTK_E_INVALID;
+  if ((((uintptr_t)e->residual | (uintptr_t)e->upsample) & 1) || (e->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
   if (!device_ready()) return ODTK_E_CUDA;
   const int sms = odtk_sm_count();
   ConvParams p;
@@ -661,36 +691,21 @@ int conv_run_s8(const odtk_conv_s8_t *d, cudaStream_t stream) {
   p.ldy = d->cout;
   p.ldr = d->cout;
   p.inv_out_scale = d->inv_out_scale;
+  p.res8 = (const int8_t *)e->residual; p.res_scale = e->res_scale;
+  p.up8 = (const int8_t *)e->upsample; p.up_scale = e->up_scale;
+  p.up_h = d->h / 2; p.up_w = d->width / 2;
   if (p.out_mode == ODTK_OUT_CANDIDATES) {
     const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
     if (rc != ODTK_OK) return rc;
   }
   CUtensorMap tmA, tmB;
-  if (d->ksize == 1) {
-    p.mode = 0;
-    p.num_m_tiles = (int)((p.M + 127) / 128);
-    uint64_t dims[2] = {(uint64_t)d->cin, (uint64_t)p.M};
-    uint64_t str[1] = {(uint64_t)d->cin};
-    uint32_t box[2] = {128, 128};
-    if (!encode_map(&tmA, d->x, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
-  } else {
-    p.mode = 1;
-    if (d->tile_tab) {   // atlas tile tables list 8 x 16 pixel tiles
-      p.TH = 8; p.TW = 16;
-      p.tile_tab = (const int4 *)d->tile_tab; p.tab_tiles = d->tab_tiles;
-    } else {
-      choose_patch(d->h, d->width, p.TH, p.TW);
-    }
-    p.tiles_h = (d->h + p.TH - 1) / p.TH;
-    p.tiles_w = (d->width + p.TW - 1) / p.TW;
-    p.num_m_tiles = d->tile_tab ? d->n * d->tab_tiles : d->n * p.tiles_h * p.tiles_w;
-    const uint64_t C = (uint64_t)d->cin;
-    uint64_t dims[4] = {C, (uint64_t)d->width, (uint64_t)d->h, (uint64_t)d->n};
-    uint64_t str[3] = {C, xW * C, xH * xW * C};
-    uint32_t box[4] = {128, (uint32_t)p.TW, (uint32_t)p.TH, 1};
-    if (!encode_map(&tmA, d->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
-  }
-  p.oH = p.H; p.oR = 0; p.oW = p.W;
+  const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
+                           d->tab_tiles, e->upsample != nullptr, 1);
+  if (rc != ODTK_OK) return rc;
+  p.oH = e->y_rows > 0 ? e->y_rows : p.H;
+  p.oR = e->y_row_off > 0 ? e->y_row_off : 0;
+  p.oW = e->y_width > 0 ? e->y_width : p.W;
+  if ((long long)d->n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
   // N tile as for odtk_conv2d
   int BN = d->cout <= 64 ? 64 : 128;
   if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
@@ -727,7 +742,15 @@ extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
 }
 
 extern "C" int odtk_conv2d_s8(const odtk_conv_s8_t *d, odtk_stream_t stream_) {
-  return conv_run_s8(d, (cudaStream_t)stream_);
+  if (!d) return ODTK_E_INVALID;
+  odtk_conv_s8_ex_t e;
+  memset(&e, 0, sizeof e);
+  e.base = *d;
+  return conv_run_s8(&e, (cudaStream_t)stream_);
+}
+
+extern "C" int odtk_conv2d_s8_ex(const odtk_conv_s8_ex_t *e, odtk_stream_t stream_) {
+  return conv_run_s8(e, (cudaStream_t)stream_);
 }
 
 // ResNet stem: 7x7 stride-2 pad-3 convolution of the RGB image, im2col-free.  `xp` is the image

@@ -47,4 +47,8 @@ struct ConvParams {
   // clamp(rint(y * inv_out_scale), -127, 127)
   const float *alpha;
   float inv_out_scale;
+  // s8 addends of ODTK_OUT_NHWC_S8 (odtk_conv2d_s8_ex), each one more fmaf before ReLU: residual [M, Cout] at the output
+  // pixel, upsample [N, up_h, up_w, Cout] at (h >> 1, w >> 1); NULL when absent
+  const int8_t *res8, *up8;
+  float res_scale, up_scale;
 };

@@ -227,6 +227,21 @@ __global__ void quantize_f16_s8_kernel(const uint4 *__restrict__ x, uint2 *__res
   }
 }
 
+// 3-D strided copy of s8 rows with ReLU, 16 bytes per thread (pyramid7's input ReLU(P6) from the s8 atlas): max with 0
+// on symmetric s8 values is exact
+__global__ void relu_copy_rows_s8_kernel(const int8_t *__restrict__ x, int8_t *__restrict__ y, int n, int rows, int row16,
+                                         long long x_img, long long x_row, long long y_img, long long y_row) {
+  const long long total = (long long)n * rows * row16;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % row16);
+    const long long t = i / row16;
+    const int r = (int)(t % rows), im = (int)(t / rows);
+    uint4 v = __ldg(reinterpret_cast<const uint4 *>(x + im * x_img + r * x_row) + c);
+    v.x = __vmaxs4(v.x, 0u); v.y = __vmaxs4(v.y, 0u); v.z = __vmaxs4(v.z, 0u); v.w = __vmaxs4(v.w, 0u);
+    reinterpret_cast<uint4 *>(y + im * y_img + r * y_row)[c] = v;
+  }
+}
+
 inline int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
   long long cap = (long long)odtk_sm_count() * 16;
@@ -359,6 +374,17 @@ extern "C" int odtk_quantize_f16_s8(const void *x, void *y, long long n, float i
   if (!x || !y || n <= 0 || (n % 8) || ((uintptr_t)x & 15) || ((uintptr_t)y & 7)) return ODTK_E_INVALID;
   OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
   quantize_f16_s8_kernel<<<grid_for(n / 8, 256), 256, 0, (cudaStream_t)stream_>>>((const uint4 *)x, (uint2 *)y, n / 8, inv_scale);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_relu_copy_rows_s8(const void *x, void *y, int n, int rows, int row_elems, long long x_img_pitch,
+                                      long long x_row_pitch, long long y_img_pitch, long long y_row_pitch, odtk_stream_t stream_) {
+  if (!x || !y || n <= 0 || rows <= 0 || row_elems <= 0 || (row_elems % 16)) return ODTK_E_INVALID;
+  if ((x_img_pitch | x_row_pitch | y_img_pitch | y_row_pitch) % 16 || (((uintptr_t)x | (uintptr_t)y) & 15)) return ODTK_E_INVALID;
+  const long long total = (long long)n * rows * (row_elems / 16);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  relu_copy_rows_s8_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream_>>>((const int8_t *)x, (int8_t *)y, n, rows, row_elems / 16,
+                                                                                    x_img_pitch, x_row_pitch, y_img_pitch, y_row_pitch);
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 

@@ -43,6 +43,13 @@ class ConvS8Desc(ctypes.Structure):
                 ("x_rows", ctypes.c_int), ("x_width", ctypes.c_int), ("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int)]
 
 
+class ConvS8ExDesc(ctypes.Structure):
+    """odtk_conv_s8_ex_t (include/odtk_b200.h)."""
+    _fields_ = [("base", ConvS8Desc), ("stride", ctypes.c_int), ("residual", ctypes.c_void_p), ("res_scale", ctypes.c_float),
+                ("upsample", ctypes.c_void_p), ("up_scale", ctypes.c_float), ("y_rows", ctypes.c_int),
+                ("y_row_off", ctypes.c_int), ("y_width", ctypes.c_int)]
+
+
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
@@ -178,23 +185,30 @@ def conv2d(x, w, bias, cout, ksize, relu=False, residual=None, upsample=None, ou
 
 
 def conv2d_s8(x, w, alpha, bias, cout, ksize, relu=False, out_mode=OUT_NHWC_S8, out=None, inv_out_scale=1.0, sink=None,
-              tile_tab=None):
-    """INT8 convolution (odtk_conv2d_s8), stride 1, pad ksize//2.  x: NHWC int8 [N,H,W,Cin] (or an int8 AtlasView);
-    w: int8 [Cout, ksize*ksize*Cin] from pack_weight_s8; alpha fp32 [Cout] = s_in * s_w; bias fp32 [Cout] or None.
-    Returns NHWC int8 [N,H,W,Cout] (out_mode OUT_NHWC_S8, requantised with inv_out_scale) or NCHW fp32 [N,Cout,H,W].
-    tile_tab: x and out are whole int8 atlases, one launch covers every level the table lists."""
+              tile_tab=None, stride=1, residual=None, res_scale=0.0, upsample=None, up_scale=0.0):
+    """INT8 convolution (odtk_conv2d_s8 / odtk_conv2d_s8_ex), stride 1 / 2, pad ksize//2.  x: NHWC int8 [N,H,W,Cin] (or an
+    int8 AtlasView); w: int8 [Cout, ksize*ksize*Cin] from pack_weight_s8; alpha fp32 [Cout] = s_in * s_w; bias fp32 [Cout]
+    or None.  Returns NHWC int8 [N,OH,OW,Cout] (out_mode OUT_NHWC_S8, requantised with inv_out_scale) or NCHW fp32
+    [N,Cout,OH,OW]; `out` may be an int8 AtlasView (3x3 only: the result lands in that level of the atlas).
+    tile_tab: x and out are whole int8 atlases, one launch covers every level the table lists.  NHWC int8 outputs may add
+    residual (NHWC int8 [N,OH,OW,Cout], dequantised with res_scale) and / or upsample (NHWC int8 [N,H/2,W/2,Cout], nearest
+    2x, dequantised with up_scale), one fmaf each before ReLU."""
     xv = x if isinstance(x, AtlasView) else None
     assert xv is not None or (x.is_cuda and x.dtype == torch.int8 and x.is_contiguous())
     assert (xv.atlas if xv is not None else x).dtype == torch.int8 and w.dtype == torch.int8
     n, h, wd, cin = x.shape
+    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
     if out_mode == OUT_CANDIDATES:
         assert sink is not None
     elif out is None:
         if out_mode == OUT_NHWC_S8:
-            out = torch.empty((n, h, wd, cout), dtype=torch.int8, device=x.device)
+            out = torch.empty((n, oh, ow, cout), dtype=torch.int8, device=x.device)
         else:
-            out = torch.empty((n, cout, h, wd), dtype=torch.float32, device=x.device)
-    d = ConvS8Desc()
+            out = torch.empty((n, cout, oh, ow), dtype=torch.float32, device=x.device)
+    for t in (residual, upsample):
+        assert t is None or (t.is_cuda and t.dtype == torch.int8 and t.is_contiguous())
+    e = ConvS8ExDesc()
+    d = e.base
     d.x, d.w, d.alpha, d.y = x.data_ptr(), w.data_ptr(), alpha.data_ptr(), (out.data_ptr() if out is not None else None)
     d.bias = bias.data_ptr() if bias is not None else None
     if xv is not None:
@@ -204,14 +218,26 @@ def conv2d_s8(x, w, alpha, bias, cout, ksize, relu=False, out_mode=OUT_NHWC_S8, 
     d.sink = ctypes.addressof(sink) if sink is not None else None
     d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cin, cout, ksize
     d.relu, d.out_mode, d.inv_out_scale = int(relu), out_mode, float(inv_out_scale)
-    _lib.check(_lib.lib().odtk_conv2d_s8(ctypes.byref(d), _stream()), "conv2d_s8")
+    e.stride = int(stride)
+    e.residual, e.res_scale = (residual.data_ptr() if residual is not None else None), float(res_scale)
+    e.upsample, e.up_scale = (upsample.data_ptr() if upsample is not None else None), float(up_scale)
+    if isinstance(out, AtlasView):
+        e.y_rows, e.y_row_off, e.y_width = out.atlas.shape[1], 0, out.atlas.shape[2]     # data_ptr() already points at the level
+    if stride == 1 and residual is None and upsample is None and not isinstance(out, AtlasView):
+        _lib.check(_lib.lib().odtk_conv2d_s8(ctypes.byref(d), _stream()), "conv2d_s8")
+    else:
+        _lib.check(_lib.lib().odtk_conv2d_s8_ex(ctypes.byref(e), _stream()), "conv2d_s8_ex")
     STATS["launches"] += 1
     if STATS["trace"] is not None:
-        # 1-byte operands: activations read once (atlas launches: the pixels of the levels), int8 weights, the output
-        px = n * h * wd if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
+        # 1-byte operands: activations read once (atlas launches: the pixels of the levels; 1x1 stride 2: the pixels it
+        # samples), int8 weights, the output, the addends
+        px = n * oh * ow if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
         obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * (1 if out_mode == OUT_NHWC_S8 else 4)
-        _trace("conv%dx%d_s8" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin, px * cin + w.numel() + obytes,
-               n=n, h=h, w=wd, cin=cin, cout=cout, stride=1, residual=False, upsample=False, out_mode=out_mode)
+        xbytes = px * cin if (tile_tab is not None or (ksize == 1 and stride == 2)) else n * h * wd * cin
+        _trace("conv%dx%d_s8" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin,
+               xbytes + w.numel() + obytes + (px * cout if residual is not None else 0) + (px * cout // 4 if upsample is not None else 0),
+               n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
+               upsample=upsample is not None, out_mode=out_mode)
     return out
 
 
@@ -260,6 +286,21 @@ def relu_from_view(view):
                                              a.shape[1] * a.shape[2] * c, a.shape[2] * c, h * w * c, w * c, 1, _stream()), "copy_rows_f16")
     STATS["launches"] += 1
     _trace("relu", 0, out.numel() * 4, n=n, h=h, w=w, cin=c)
+    return out
+
+
+def relu_from_view_s8(view):
+    """ReLU of a level of the int8 atlas into a new dense int8 tensor [N, h, w, C] (odtk_relu_copy_rows_s8): pyramid7's
+    input ReLU(P6) in the INT8 network."""
+    n, h, w, c = view.shape
+    a = view.atlas
+    assert a.dtype == torch.int8
+    out = torch.empty((n, h, w, c), dtype=torch.int8, device=a.device)
+    _lib.check(_lib.lib().odtk_relu_copy_rows_s8(ctypes.c_void_p(view.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w * c,
+                                                 a.shape[1] * a.shape[2] * c, a.shape[2] * c, h * w * c, w * c, _stream()),
+               "relu_copy_rows_s8")
+    STATS["launches"] += 1
+    _trace("relu_s8", 0, out.numel() * 2, n=n, h=h, w=w, cin=c)
     return out
 
 

@@ -236,7 +236,9 @@ class Model:
         self.precision = "fp16"
         self._int8_table = None       # calibration table of the INT8 heads (set_precision)
         self._int8 = None             # their packed s8 weights, alpha, bias, requantisation scales
+        self.int8_scope = "heads"     # "heads" or "network" (layer3, layer4 and the FPN in INT8 as well)
         self._calib_hook = None
+        self._calib_net = False       # calibration also records the network scope's tensors
 
     def __repr__(self):
         return '\n'.join(['     model: {}'.format(self.name), '  backbone: {}'.format(self.backbone),
@@ -347,7 +349,7 @@ class Model:
             for b in range(nblocks):
                 stride = 2 if (b == 0 and li > 0) else 1
                 p = f + "layer%d.%d." % (li + 1, b)
-                blk = {"level": li + 2, "last": b == nblocks - 1}
+                blk = {"level": li + 2, "last": b == nblocks - 1, "name": p[:-1]}
                 if block == "bottleneck":
                     blk["convs"] = [conv_bn(p + "conv1", p + "bn1"),
                                     conv_bn(p + "conv2", p + "bn2", stride, RESNEXT.get(self.backbone, (1, 64))[0]),
@@ -386,21 +388,84 @@ class Model:
                                "b": b.float().contiguous().to(dev) if b is not None else None,
                                "inv_out": float(inv) if inv is not None else None})
             P[head] = layers
+        if self.int8_scope == "network":
+            P["net"] = self._pack_int8_net()
         self._int8 = P
 
-    def set_precision(self, precision, table=None):
+    def _pack_int8_net(self):
+        """Network scope: s8 weights (BatchNorm folded first) and epilogue constants of layer3, layer4 and the FPN.  Every
+        convolution reads a tensor quantised with the scale of its table entry (calib.network_tensors) and requantises its
+        output with the scale of its own; residual / upsample addends are dequantised with the scale of the tensor they
+        are; the smooth and pyramid convolutions write the s8 atlas with the "heads.input" scale."""
+        S, sd, dev = self._int8_table["scales"], self._sd, self.device
+        block, layers = RESNET_LAYERS[self.backbone]
+        f, n = "backbones.%s.features." % self.backbone, "backbones.%s." % self.backbone
+
+        def s32(name):
+            return np.float32(S[name])
+
+        def layer(w, b, s_in, out, stride=1):
+            q, s_w = engine.pack_weight_s8(w)
+            return {"w": q.to(dev), "alpha": (s_w * torch.tensor(s_in, dtype=torch.float32)).contiguous().to(dev),
+                    "b": b.float().contiguous().to(dev) if b is not None else None, "cout": w.shape[0], "ks": w.shape[2],
+                    "stride": stride, "inv_out": float(np.float32(1.0) / s32(out))}
+
+        def folded(pc, pb, s_in, out, stride=1):
+            w, b = engine.fold_bn(sd[pc + ".weight"], sd[pb + ".weight"], sd[pb + ".bias"], sd[pb + ".running_mean"],
+                                  sd[pb + ".running_var"])
+            return layer(w, b, s_in, out, stride)
+
+        def plain(name, s_in, out, stride=1):
+            return layer(sd[n + name + ".weight"], sd.get(n + name + ".bias"), s_in, out, stride)
+
+        x_name = f + "layer2"
+        c3 = x_name
+        blocks, c = [], {}
+        for li in (3, 4):
+            for b in range(layers[li - 1]):
+                p = f + "layer%d.%d" % (li, b)
+                stride = 2 if b == 0 else 1
+                mids = [p + ".conv1", p + ".conv2"] if block == "bottleneck" else [p + ".conv1"]
+                ins, outs = [x_name] + mids, mids + [p]
+                strided = 1 if block == "bottleneck" else 0          # torchvision v1.5: the 3x3 carries the stride
+                convs = [folded(p + ".conv%d" % (k + 1), p + ".bn%d" % (k + 1), s32(ins[k]), outs[k], stride if k == strided else 1)
+                         for k in range(len(ins))]
+                down = None
+                if (p + ".downsample.0.weight") in sd:
+                    down = folded(p + ".downsample.0", p + ".downsample.1", s32(x_name), p + ".downsample", stride)
+                blocks.append({"convs": convs, "down": down, "res_scale": float(s32(p + ".downsample" if down else x_name))})
+                x_name = p
+            c[li + 1] = x_name
+        N = {"inv_c3": float(np.float32(1.0) / s32(c3)), "blocks": blocks}
+        N["lateral5"] = plain("lateral5", s32(c[5]), n + "lateral5")
+        N["lateral4"] = dict(plain("lateral4", s32(c[4]), n + "lateral4"), up_scale=float(s32(n + "lateral5")))
+        N["lateral3"] = dict(plain("lateral3", s32(c3), n + "lateral3"), up_scale=float(s32(n + "lateral4")))
+        for k in (3, 4, 5):
+            N["smooth%d" % k] = plain("smooth%d" % k, s32(n + "lateral%d" % k), "heads.input")
+        N["pyramid6"] = plain("pyramid6", s32(c[5]), "heads.input", 2)
+        N["pyramid7"] = plain("pyramid7", s32("heads.input"), "heads.input", 2)
+        return N
+
+    def set_precision(self, precision, table=None, scope="heads"):
         """"fp16" (default) or "int8": the head towers and the two final head layers run on the s8 tensor cores with the
-        activation scales of `table` (a path or a dict, from `calibrate`); the backbone and the FPN stay fp16, and so does
-        the training-mode forward.  INT8 needs the pyramid atlas (ODTK_MERGED_HEADS=1).  Captured CUDA graphs are dropped."""
+        activation scales of `table` (a path or a dict, from `calibrate`).  scope "heads" (default): the backbone and the
+        FPN stay fp16; "network" (a table from calibrate(..., scope="network")): ResNet layer3, layer4 and the FPN run in
+        INT8 too, from layer2's output quantised once, and the FPN writes the s8 atlas the heads read -- the stem, layer1 and
+        layer2 stay fp16 (ResNet18/34/50/101/152 backbones; ResNeXt and MobileNetV2 take "heads" only).  The training-mode
+        forward stays fp16.  INT8 needs the pyramid atlas (ODTK_MERGED_HEADS=1).  Captured CUDA graphs are dropped."""
         if precision == "fp16":
             self._int8_table = None
             self._int8 = None
+            self.int8_scope = "heads"
         elif precision == "int8":
             if table is None:
                 raise ValueError("set_precision('int8') needs a calibration table (Model.calibrate)")
             if not self.merged_heads:
                 raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
-            self._int8_table = calib.check_table(calib.load_table(table), self.backbone, self.classes, self.num_anchors)
+            if scope == "network":
+                calib.network_tensors(self.backbone)            # ValueError for the backbones the scope does not cover
+            self._int8_table = calib.check_table(calib.load_table(table), self.backbone, self.classes, self.num_anchors, scope)
+            self.int8_scope = scope
             if self._packed is not None:
                 self._pack_int8()
         else:
@@ -410,15 +475,21 @@ class Model:
             self._graphs = {}
         return self
 
-    def calibrate(self, batches, table=None, method="entropy"):
+    def calibrate(self, batches, table=None, method="entropy", scope="heads"):
         """INT8 calibration: eager fp16 forwards over `batches` (each one what `forward` takes) record, for the 9 tensors the
         INT8 heads quantise (calib.TENSORS), max|x| and then a 2048-bin |x| histogram over the valid atlas pixels (the gap
-        rows / columns are left out).  method "max": threshold max|x|; "entropy": TensorRT's KL-divergence search.  Returns
-        the calibration table and, if `table` is a path, writes it there."""
+        rows / columns are left out).  method "max": threshold max|x|; "entropy": TensorRT's KL-divergence search.
+        scope "network" also records every tensor of layer3, layer4 and the FPN that scope quantises
+        (calib.network_tensors) and returns a format-2 table; its 9 head scales are those scope "heads" finds.  Runs on
+        the fp16 network, as TensorRT's calibrator does.  Returns the calibration table and, if `table` is a path, writes it
+        there."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
         if method not in ("max", "entropy"):
             raise ValueError("unknown calibration method %r (max, entropy)" % (method,))
+        if scope not in calib.SCOPES:
+            raise ValueError("INT8 scope must be 'heads' or 'network', got %r" % (scope,))
+        names = calib.table_tensors(self.backbone, scope)
         if not self.merged_heads:
             raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
         batches = list(batches)
@@ -426,6 +497,7 @@ class Model:
         saved = (self._int8, self.parallel_heads, self.training)
         self._int8, self.parallel_heads, self.training = None, False, False
         self._calib_hook = col.observe
+        self._calib_net = scope == "network"
         images = 0
         try:
             with torch.no_grad():
@@ -442,7 +514,8 @@ class Model:
         finally:
             self._int8, self.parallel_heads, self.training = saved
             self._calib_hook = None
-        t = calib.make_table(self.backbone, self.classes, self.num_anchors, method, images, col.scales(method))
+            self._calib_net = False
+        t = calib.make_table(self.backbone, self.classes, self.num_anchors, method, images, col.scales(method, names), scope)
         if table is not None:
             calib.save_table(t, table)
         return t
@@ -545,8 +618,13 @@ class Model:
         P = self._packed
         outs = {}
         blocks = P["blocks"]
+        net8 = self._int8.get("net") if (self._int8 is not None and not self.training) else None
+        hook = self._calib_hook if self._calib_net else None     # network-scope calibration: layer3 / layer4 tensors
         z_next = None                 # conv1 of THIS block, already computed by the previous block's fused tail (GEMM3)
         for bi, blk in enumerate(blocks):
+            if net8 is not None and blk["level"] >= 4:
+                return self._features_s8(outs[3], net8)
+            tap = hook if blk["level"] >= 4 else None
             cs = blk["convs"]
             dn = blk["down"]
             z_in, z_next = z_next, None
@@ -566,7 +644,9 @@ class Model:
                     outs[blk["level"]] = x
                 continue
             identity = x if dn is None else dn(x)
-            if (self.fused_bneck and len(cs) == 3 and cs[1].stride == 1 and cs[1].groups == 1 and cs[1].ks == 3 and
+            if tap is not None and dn is not None:
+                tap(blk["name"] + ".downsample", identity)
+            if (self.fused_bneck and tap is None and len(cs) == 3 and cs[1].stride == 1 and cs[1].groups == 1 and cs[1].ks == 3 and
                     cs[1].cin in (64, 128) and cs[1].cout == cs[1].cin and cs[2].cin == cs[1].cin and cs[2].cout % 128 == 0 and
                     cs[2].cout <= 512):
                 # conv2 (3x3) + conv3 (1x1) + identity + ReLU in one kernel: the 3x3's output never leaves the SM
@@ -585,12 +665,62 @@ class Model:
                     x = engine.bottleneck_tail(out, cs[1].w, cs[1].b, cs[2].w, cs[2].b, identity, relu=True)
             else:
                 out = z_in if z_in is not None else x
-                for c in (cs[1:-1] if z_in is not None else cs[:-1]):
+                for k, c in enumerate(cs[1:-1] if z_in is not None else cs[:-1]):
                     out = c(out, relu=True)
+                    if tap is not None:
+                        tap("%s.conv%d" % (blk["name"], k + 1), out)
                 x = cs[-1](out, relu=True, residual=identity)
+            if tap is not None:
+                tap(blk["name"], x)
             if blk["last"]:
                 outs[blk["level"]] = x
+        if hook is not None:
+            hook("backbones.%s.features.layer2" % self.backbone, outs[3])
         return self._fpn(outs[3], outs[4], outs[5])
+
+    def _conv8(self, L, x, relu=False, out=None, **addends):
+        """One network-scope s8 convolution (a layer of _pack_int8_net) of NHWC int8 x (or an int8 AtlasView)."""
+        n, h, w, cin = x.shape
+        oh, ow = ((h - 1) // 2 + 1, (w - 1) // 2 + 1) if L["stride"] == 2 else (h, w)
+        engine.STATS["conv_flops"] += 2 * n * oh * ow * L["cout"] * L["ks"] * L["ks"] * cin
+        return engine.conv2d_s8(x, L["w"], L["alpha"], L["b"], L["cout"], L["ks"], relu=relu, out=out,
+                                inv_out_scale=L["inv_out"], stride=L["stride"], **addends)
+
+    def _features_s8(self, c3, N):
+        """Network scope from layer2's fp16 output C3: one quantisation, then layer3, layer4 (residual added in the last
+        convolution's epilogue) and the FPN on s8."""
+        x = c3q = engine.quantize_f16_s8(c3, N["inv_c3"])
+        taps = []
+        for blk in N["blocks"]:
+            identity = x if blk["down"] is None else self._conv8(blk["down"], x)
+            t = x
+            for L in blk["convs"][:-1]:
+                t = self._conv8(L, t, relu=True)
+            x = self._conv8(blk["convs"][-1], t, relu=True, residual=identity, res_scale=blk["res_scale"])
+            taps.append(x)
+        nl3 = RESNET_LAYERS[self.backbone][1][2]
+        return self._fpn_s8(c3q, taps[nl3 - 1], taps[-1], N)
+
+    def _fpn_s8(self, c3, c4, c5, N):
+        """FPN on s8 taps: the laterals add the top-down path in their epilogue, smooth3/4/5 and pyramid6/7 write the s8
+        pyramid atlas the INT8 heads read."""
+        if not self.merged_heads:
+            raise ValueError("INT8 network scope writes the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
+        p5 = self._conv8(N["lateral5"], c5)
+        p4 = self._conv8(N["lateral4"], c4, upsample=p5, up_scale=N["lateral4"]["up_scale"])
+        p3 = self._conv8(N["lateral3"], c3, upsample=p4, up_scale=N["lateral3"]["up_scale"])
+        n = c5.shape[0]
+        h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
+        sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
+                 ((h6 - 1) // 2 + 1, (w6 - 1) // 2 + 1))
+        at = self._atlas_for(n, sizes, c5.device)
+        v = [engine.AtlasView(self._atlas_s8(at)[0], r, h, w) for r, (h, w) in zip(at["rows"], sizes)]
+        self._conv8(N["smooth3"], p3, out=v[0])
+        self._conv8(N["smooth4"], p4, out=v[1])
+        self._conv8(N["smooth5"], p5, out=v[2])
+        self._conv8(N["pyramid6"], c5, out=v[3])
+        self._conv8(N["pyramid7"], engine.relu_from_view_s8(v[3]), out=v[4])
+        return v
 
     def _fpn(self, c3, c4, c5):
         """FPN (odtk/backbones/fpn.py:45-61) on the three backbone taps."""
@@ -598,6 +728,9 @@ class Model:
         p5 = P["lateral5"](c5)
         p4 = P["lateral4"](c4, upsample=p5)
         p3 = P["lateral3"](c3, upsample=p4)
+        if self._calib_net:
+            for k, t in ((5, p5), (4, p4), (3, p3)):
+                self._calib_hook("backbones.%s.lateral%d" % (self.backbone, k), t)
         if self.merged_heads and c5.shape[3] % 64 == 0:
             # pyramid atlas: the five levels stacked in ONE zero-separated NHWC buffer, so that every head-tower layer is
             # one launch over all levels instead of five
@@ -638,6 +771,14 @@ class Model:
                   "buf": [torch.zeros((n, ha, wa, 256), dtype=torch.float16, device=device) for _ in range(5)]}
             self._atlas[key] = at
         return at
+
+    @staticmethod
+    def _atlas_s8(at):
+        """The five int8 buffers of an atlas geometry (INT8 heads), zero-initialised on first use."""
+        if "buf8" not in at:
+            buf = at["buf"][0]
+            at["buf8"] = [torch.zeros(buf.shape, dtype=torch.int8, device=buf.device) for _ in range(5)]
+        return at["buf8"]
 
     def _heads(self, features, sigmoid=True, sinks=None):
         """Class / box heads on the five levels (odtk/model.py:134-135).  The ten conv chains are
@@ -729,10 +870,10 @@ class Model:
 
         i8 = self._int8 if not self.training else None
         if i8 is not None:
-            # INT8: the fp16 atlas is quantised once (main stream, before the fork); towers and final layers run on s8
-            if "buf8" not in at:
-                at["buf8"] = [torch.zeros(atlas0.shape, dtype=torch.int8, device=atlas0.device) for _ in range(5)]
-            q_in = engine.quantize_f16_s8(atlas0, i8["inv_in"], out=at["buf8"][0])
+            # INT8: the fp16 atlas is quantised once (main stream, before the fork) -- in network scope the FPN wrote the s8
+            # atlas itself; towers and final layers run on s8
+            buf8 = self._atlas_s8(at)
+            q_in = atlas0 if atlas0.dtype == torch.int8 else engine.quantize_f16_s8(atlas0, i8["inv_in"], out=buf8[0])
 
             def tower8(head, bufs, final_mode, use_sinks):
                 t = q_in
@@ -750,7 +891,7 @@ class Model:
                     outs.append(engine.conv2d_s8(lv, last["w"], last["alpha"], last["b"], last["cout"], 3, out_mode=mode, sink=sink))
                 return outs
 
-            tower, bufs = tower8, at["buf8"]
+            tower, bufs = tower8, buf8
         else:
             bufs = at["buf"]
 

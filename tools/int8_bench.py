@@ -9,7 +9,13 @@ Reports, as one JSON line:
   * the quantise launch of the INT8 path;
   * the INT8 vs fp16 detection match rate (same class, every box coordinate within 2 px, score within 0.02);
   * the card name and power limit (read-only nvidia-smi query).
---dump-outputs DIR writes both precisions' detections as float32 .npy."""
+--scope network adds a third arm, INT8 network scope (ResNet layer3, layer4 and the FPN on s8 too), and reports:
+  * fp16, INT8-heads and INT8-network img/s from CUDA graphs timed in the same process, alternating;
+  * per-launch times of the layer3 / layer4 / FPN convolutions in fp16 and in INT8-network, with achieved TOPS against the
+    989 / 1979 data-sheet peaks;
+  * the C3 quantise launch (CUDA events over repeated launches on a C3-shaped tensor);
+  * the INT8-network vs fp16 detection match rate.
+--dump-outputs DIR writes every arm's detections as float32 .npy."""
 import argparse
 import ctypes
 import json
@@ -25,7 +31,7 @@ import torch  # noqa: E402
 
 from oracle import model_ref  # noqa: E402
 from retinanet_examples_b200 import _lib, engine, synth  # noqa: E402
-from retinanet_examples_b200.model import Model, make_state_dict  # noqa: E402
+from retinanet_examples_b200.model import RESNET_LAYERS, Model, make_state_dict  # noqa: E402
 
 PEAK_TOPS = {"fp16": 989.0, "int8": 1979.0}
 CONV_KINDS = ("conv1x1", "conv3x3", "stem7x7", "stem_pool", "bneck_tail", "conv1x1_s8", "conv3x3_s8")
@@ -68,6 +74,67 @@ def head_launches(model, x):
     return heads, qms
 
 
+def region_launches(model, x, names):
+    """Per-launch ms and trace entry of the layer3 / layer4 / FPN convolutions (`names`, forward order) of one eager,
+    single-stream forward: the len(names) convolution launches before the 18 head convolutions."""
+    lib = _lib.lib()
+    model.parallel_heads = False
+    engine.STATS["trace"] = []
+    lib.odtk_prof_reset()
+    lib.odtk_prof_enable(1)
+    model.forward(x)
+    torch.cuda.synchronize()
+    lib.odtk_prof_enable(0)
+    trace, engine.STATS["trace"] = engine.STATS["trace"], None
+    model.parallel_heads = True
+    convs = [t for t in trace if t["kind"] in CONV_KINDS]
+    buf = (ctypes.c_float * len(convs))()
+    assert lib.odtk_prof_get_list(3, buf, len(convs)) == len(convs)
+    rows = list(zip(convs, buf))[-18 - len(names):-18]
+    return [{"layer": n, "kind": t["kind"], "ms": float(v), "flops": t["flops"]} for n, (t, v) in zip(names, rows)]
+
+
+def region_names(backbone):
+    """The convolutions of layer3, layer4 and the FPN in launch order (downsample first in a block's first launch)."""
+    block, layers = RESNET_LAYERS[backbone]
+    f, out = "layer", []
+    for li in (3, 4):
+        for b in range(layers[li - 1]):
+            p = "%s%d.%d." % (f, li, b)
+            out += ([p + "downsample"] if b == 0 else []) + [p + "conv%d" % k for k in range(1, 4 if block == "bottleneck" else 3)]
+    return out + ["lateral5", "lateral4", "lateral3", "smooth3", "smooth4", "smooth5", "pyramid6", "pyramid7"]
+
+
+def region_table(rows16, rows8):
+    table = []
+    for a, b in zip(rows16, rows8):
+        assert a["layer"] == b["layer"] and a["flops"] == b["flops"], (a, b)
+        table.append({"layer": a["layer"], "gflop": round(a["flops"] / 1e9, 2),
+                      "fp16_us": round(a["ms"] * 1e3, 1), "fp16_tops": round(a["flops"] / a["ms"] / 1e9, 1),
+                      "int8_us": round(b["ms"] * 1e3, 1), "int8_tops": round(b["flops"] / b["ms"] / 1e9, 1),
+                      "speedup": round(a["ms"] / b["ms"], 2)})
+    tot16, tot8 = sum(r["ms"] for r in rows16), sum(r["ms"] for r in rows8)
+    fl = sum(r["flops"] for r in rows16)
+    return {"launches": table, "fp16_ms": round(tot16, 3), "int8_ms": round(tot8, 3),
+            "fp16_share_of_peak": round(fl / tot16 / 1e9 / PEAK_TOPS["fp16"], 3),
+            "int8_share_of_peak": round(fl / tot8 / 1e9 / PEAK_TOPS["int8"], 3)}
+
+
+def quantize_ms(c3_shape, dev, reps=50):
+    """One C3 quantise launch (odtk_quantize_f16_s8), CUDA events over `reps` launches after a warm-up."""
+    t = torch.randn(c3_shape, generator=torch.Generator().manual_seed(7)).half().to(dev)
+    out = torch.empty(c3_shape, dtype=torch.int8, device=dev)
+    for _ in range(5):
+        engine.quantize_f16_s8(t, 10.0, out=out)
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    for _ in range(reps):
+        engine.quantize_f16_s8(t, 10.0, out=out)
+    t1.record()
+    t1.synchronize()
+    return t0.elapsed_time(t1) / reps
+
+
 def summarize(heads, precision):
     groups = {"tower": heads[0:4] + heads[9:13], "cls_final": heads[4:9], "box_final": heads[13:18]}
     out = {}
@@ -105,6 +172,7 @@ def main():
     ap.add_argument("--calib-batches", type=int, default=2)
     ap.add_argument("--calib-batch-size", type=int, default=8)
     ap.add_argument("--method", default="entropy", choices=("entropy", "max"))
+    ap.add_argument("--scope", default="heads", choices=("heads", "network"))
     ap.add_argument("--dump-outputs", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -120,13 +188,21 @@ def main():
     m8 = Model(backbone, classes=80).load_state_dict(sd).cuda(0)
     calib_x = [torch.randn((args.calib_batch_size, 3, H, W), generator=torch.Generator().manual_seed(2000 + i))
                for i in range(args.calib_batches)]
-    table = m8.calibrate(calib_x, method=args.method)
+    table = m8.calibrate(calib_x, method=args.method, scope=args.scope)
     m8.set_precision("int8", table)
     models = {"fp16": m16, "int8": m8}
+    if args.scope == "network":
+        mn = Model(backbone, classes=80).load_state_dict(sd).cuda(0)
+        mn.set_precision("int8", table, scope="network")
+        models["int8_network"] = mn
 
-    heads = {p: head_launches(m, x) for p, m in models.items()}
+    heads = {p: head_launches(m, x) for p, m in models.items() if p != "int8_network"}
     outs = {p: [t.clone().cpu().numpy() for t in m.forward(x)] for p, m in models.items()}
     rate, ndet = match_rate(outs["int8"], outs["fp16"])
+    if args.scope == "network":
+        names = region_names(backbone)
+        region = region_table(region_launches(m16, x, names), region_launches(models["int8_network"], x, names))
+        rate_net, _ = match_rate(outs["int8_network"], outs["fp16"])
     if args.dump_outputs:
         os.makedirs(args.dump_outputs, exist_ok=True)
         for p, o in outs.items():
@@ -148,18 +224,26 @@ def main():
             t1.record()
             t1.synchronize()
             windows[p].append(t0.elapsed_time(t1))
-    res = {"workload": "%s batch %d 3x%dx%d, heads fp16 vs INT8 (%s calibration, %d x %d images)" % (
-        backbone, args.batch, H, W, args.method, args.calib_batches, args.calib_batch_size)}
+    res = {"workload": "%s batch %d 3x%dx%d, %s (%s calibration, %d x %d images)" % (
+        backbone, args.batch, H, W, "heads fp16 vs INT8" if args.scope == "heads" else "fp16 vs INT8 heads vs INT8 network",
+        args.method, args.calib_batches, args.calib_batch_size)}
     res.update(gpu_info())
     for p in models:
         ms = float(np.median(windows[p])) / args.steps
         res["%s_img_s" % p] = round(args.batch * 1000.0 / ms, 1)
         res["%s_ms_per_step" % p] = round(ms, 3)
-        res["%s_heads" % p] = summarize(heads[p][0], p)
+        if p in heads:
+            res["%s_heads" % p] = summarize(heads[p][0], p)
     res["int8_speedup"] = round(res["int8_img_s"] / res["fp16_img_s"], 3)
     res["int8_quantize_ms"] = round(heads["int8"][1], 4) if heads["int8"][1] is not None else None
     res["match_rate_int8_vs_fp16"] = round(rate, 4)
     res["detections_compared"] = ndet
+    if args.scope == "network":
+        res["int8_network_speedup"] = round(res["int8_network_img_s"] / res["fp16_img_s"], 3)
+        res["int8_network_vs_heads"] = round(res["int8_network_img_s"] / res["int8_img_s"], 3)
+        res["layer3_layer4_fpn"] = region
+        res["c3_quantize_ms"] = round(quantize_ms((args.batch, H // 8, W // 8, 512), dev), 4)
+        res["match_rate_int8_network_vs_fp16"] = round(rate_net, 4)
     res["scales"] = table["scales"]
     print(json.dumps(res))
 

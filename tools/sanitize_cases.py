@@ -6,7 +6,8 @@ Shapes are tiny (the tools slow kernels down 10-100x) but chosen to reach each v
 mbarrier rings: conv modes 0 / 1 / 2 / 3 with N tiles 64 and 128, ragged M and N tiles, residual / upsample / ReLU6 /
 fp32 / sigmoid / candidate epilogues, the fused stem + pool (stem.cu: halo rows at the image edges), the fused bottleneck
 tail (bottleneck.cu: C1 64 / 128, projected identity, GEMM3 with 64 / 128 outputs -- shared-memory A operands written
-by the epilogues), the s8 instantiation of the conv kernel and the INT8 heads of the model, decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
+by the epilogues), the s8 instantiation of the conv kernel (stride 2 in modes 3 and 1, residual / upsample addends, level-view
+input and output) and the INT8 heads and network scope of the model, decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
 iou, target assignment, the cooperative loss kernel."""
 import os
 import sys
@@ -90,6 +91,28 @@ def main():
                              relu=mode == engine.OUT_NHWC_S8, out_mode=mode, inv_out_scale=0.1)
             torch.cuda.synchronize()
             print("conv_s8 %s -> plan %s" % ((n, h, w, cin, cout, ks), {k: v for k, v in engine.last_plan().items() if v}), flush=True)
+        # s8 network-scope paths: stride 2 (parity split / element-strided boxes), residual and upsample addends, s8 atlas
+        # level views in and out, ReLU copy of a level
+        for n, h, w, cin, cout, ks, stride, add in ((2, 16, 24, 256, 256, 3, 2, ""), (2, 16, 24, 512, 256, 1, 2, ""),
+                                                    (2, 13, 20, 256, 256, 3, 2, ""), (2, 16, 24, 256, 512, 1, 1, "res"),
+                                                    (2, 16, 24, 256, 256, 3, 1, "res"), (2, 16, 24, 256, 256, 1, 1, "up")):
+            xq = engine.quantize_f16_s8(rnd(n, h, w, cin), 20.0)
+            oh, ow = ((h - 1) // 2 + 1, (w - 1) // 2 + 1) if stride == 2 else (h, w)
+            wq, s_w = engine.pack_weight_s8(torch.randn((cout, cin, ks, ks), generator=g) * 0.05)
+            kw = {"residual": engine.quantize_f16_s8(rnd(n, oh, ow, cout), 20.0), "res_scale": 0.05} if add == "res" else \
+                 {"upsample": engine.quantize_f16_s8(rnd(n, oh // 2, ow // 2, cout), 20.0), "up_scale": 0.05} if add == "up" else {}
+            engine.conv2d_s8(xq, wq.to(DEV), (s_w * 0.05).to(DEV), torch.randn(cout, generator=g).to(DEV), cout, ks, relu=True,
+                             inv_out_scale=0.1, stride=stride, **kw)
+            torch.cuda.synchronize()
+            print("conv_s8_ex %s -> plan %s" % ((n, h, w, cin, cout, ks, stride, add), {k: v for k, v in engine.last_plan().items() if v}), flush=True)
+        at = torch.zeros((2, 56, 24, 256), dtype=torch.int8, device=DEV)
+        at[:, :32] = engine.quantize_f16_s8(rnd(2, 32, 24, 256), 20.0)
+        wq, s_w = engine.pack_weight_s8(torch.randn((256, 256, 3, 3), generator=g) * 0.05)
+        engine.conv2d_s8(engine.AtlasView(at, 0, 32, 24), wq.to(DEV), (s_w * 0.05).to(DEV), None, 256, 3, relu=True, stride=2,
+                         out=engine.AtlasView(at, 40, 16, 12), inv_out_scale=0.1)
+        engine.relu_from_view_s8(engine.AtlasView(at, 40, 16, 12))
+        torch.cuda.synchronize()
+        print("conv_s8_ex atlas views ok", flush=True)
     if only in ("", "model"):
         for rotated in (False, True):
             classes, na = 4, 27 if rotated else 9
@@ -104,6 +127,10 @@ def main():
             out = m(x)
             torch.cuda.synchronize()
             print("model int8 rotated=%s detections=%d" % (rotated, int((out[0] > 0).sum())), flush=True)
+            m.set_precision("int8", m.calibrate([x], method="max", scope="network"), scope="network")   # layer3/4 + FPN on s8
+            out = m(x)
+            torch.cuda.synchronize()
+            print("model int8 network rotated=%s detections=%d" % (rotated, int((out[0] > 0).sum())), flush=True)
     if only in ("", "postproc"):
         cls, deltas = synth.head_outputs(1, seed=0)
         anchors = [box.generate_anchors(s, box.DEFAULT_RATIOS, box.DEFAULT_SCALES).reshape(-1).tolist() for s in synth.LEVEL_STRIDES]
