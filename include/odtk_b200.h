@@ -420,6 +420,31 @@ int odtk_snap_to_anchors(const float *targets, int batch, int max_boxes, int hei
 int odtk_preprocess_u8(const void *x, void *y, int n, int h, int w, int hs, int ws, const float *mean,
                        const float *std, odtk_stream_t stream);
 
+/* One image of odtk_preprocess_resize_u8: its uint8 HWC RGB pixels (contiguous) start `offset` bytes into x, and
+ * it is resized from src_h x src_w to dst_h x dst_w.                                                          */
+typedef struct {
+  long long offset;
+  int src_h, src_w, dst_h, dst_w;
+} odtk_resize_image_t;
+
+/* The whole input side of `odtk infer` for images of any size (odtk/data.py:55-60, 113-123, collate_fn
+ * :154-176): each image is resized with Pillow's 8-bit Image.BILINEAR resampling (triangle filter, support
+ * widened by the downscale factor, weights in IEEE double normalised by their sum, 22-bit fixed point,
+ * horizontal pass rounded to uint8 before the vertical one; bit-exact), normalised with the operations of
+ * odtk_preprocess_u8 and written at the top left of one canvas of the fp16 NHWC4 stem buffer
+ * [n, canvas_h+6, canvas_w+8, 4].  Everything outside an image's dst rectangle is 0.  One fused kernel, no
+ * intermediate image.
+ *   images      host table of the n images: validated here, never read by the kernel;
+ *   images_dev  device copy of the same table, read by the kernel.  Under a CUDA graph the caller may
+ *               rewrite it (and x) before each replay with other sizes that fit the canvas;
+ *   x_bytes     bytes readable from x: every image must lie in [x, x + x_bytes).
+ * Two-phase: y == NULL returns the bytes y must hold.  ODTK_E_INVALID: a size <= 0, a dst larger than the
+ * canvas, an odd canvas side, an image outside [x, x + x_bytes).  mean / std: 3 host floats.
+ * Axes shrunk by more than 7x take a slower path that recomputes the filter taps per pixel.                  */
+long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                    const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w, void *y,
+                                    const float *mean, const float *std, odtk_stream_t stream);
+
 /* ---- per-kernel timing (H100-native addition; the reference has only a wall-clock
  * Profiler without CUDA sync, odtk/utils.py:140-167) ------------------------------
  * When enabled, every launch of a tagged kernel is bracketed by CUDA events on the

@@ -85,6 +85,8 @@ SIGNATURES = {
     "odtk_snap_to_anchors": (ctypes.c_int, [ctypes.c_void_p] + [ctypes.c_int] * 5 + [_c_f32p, ctypes.c_int, ctypes.c_int,
                                             ctypes.c_float, ctypes.c_float] + [ctypes.c_void_p] * 5),
     "odtk_preprocess_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [_c_f32p, _c_f32p, ctypes.c_void_p]),
+    "odtk_preprocess_resize_u8": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p] +
+                                  [ctypes.c_int] * 3 + [ctypes.c_void_p, _c_f32p, _c_f32p, ctypes.c_void_p]),
     "odtk_prof_enable": (None, [ctypes.c_int]),
     "odtk_prof_reset": (None, []),
     "odtk_prof_get_list": (ctypes.c_longlong, [ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.c_longlong]),
@@ -126,6 +128,12 @@ class BneckDesc(ctypes.Structure):
                 ("n", ctypes.c_int), ("h", ctypes.c_int), ("width", ctypes.c_int), ("c1", ctypes.c_int), ("c2", ctypes.c_int),
                 ("relu", ctypes.c_int), ("xproj", ctypes.c_void_p), ("wproj", ctypes.c_void_p),
                 ("w_next", ctypes.c_void_p), ("b_next", ctypes.c_void_p), ("z", ctypes.c_void_p), ("c_next", ctypes.c_int)]
+
+
+class ResizeImage(ctypes.Structure):
+    """odtk_resize_image_t (include/odtk_b200.h)."""
+    _fields_ = [("offset", ctypes.c_longlong), ("src_h", ctypes.c_int), ("src_w", ctypes.c_int), ("dst_h", ctypes.c_int),
+                ("dst_w", ctypes.c_int)]
 
 
 class CandSink(ctypes.Structure):

@@ -150,6 +150,16 @@ __global__ void pad_input_rows_kernel(const __half *__restrict__ x, __half *__re
   }
 }
 
+// One RGB pixel of odtk infer's input normalisation (reference odtk/data.py:118-121) as the stem's 8-byte NHWC4 pixel:
+// same operation order as the reference: float(u8) / 255, then - mean, then / std, fp32, one fp16 rounding.
+__device__ __forceinline__ uint2 normalize_rgb_u8(unsigned r8, unsigned g8, unsigned b8, float m0, float m1, float m2,
+                                                  float s0, float s1, float s2) {
+  float r = ((float)r8 / 255.0f - m0) / s0, g = ((float)g8 / 255.0f - m1) / s1, b = ((float)b8 / 255.0f - m2) / s2;
+  __half2 rg = __floats2half2_rn(r, g);
+  __half2 bz = __floats2half2_rn(b, 0.0f);
+  return make_uint2(*reinterpret_cast<unsigned *>(&rg), *reinterpret_cast<unsigned *>(&bz));
+}
+
 // Input side of odtk infer (reference odtk/data.py:113-123): uint8 HWC image -> /255 -> (x - mean) / std
 // -> zero padding to a multiple of the model stride, fused with the stem's own zero padding and the
 // RGB -> NHWC4 widening: one 8-byte store per padded pixel, the fp32 full-image pass disappears.
@@ -166,14 +176,174 @@ __global__ void preprocess_u8_kernel(const unsigned char *__restrict__ x, __half
     uint2 v = make_uint2(0u, 0u);
     if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
       const unsigned char *s = x + (((long long)n * H + ih) * W + iw) * 3;
-      // same operation order as the reference: float(u8) / 255, then - mean, then / std
-      float r = ((float)s[0] / 255.0f - m0) / s0, g = ((float)s[1] / 255.0f - m1) / s1, b = ((float)s[2] / 255.0f - m2) / s2;
-      __half2 rg = __floats2half2_rn(r, g);
-      __half2 bz = __floats2half2_rn(b, 0.0f);
-      v.x = *reinterpret_cast<unsigned *>(&rg);
-      v.y = *reinterpret_cast<unsigned *>(&bz);
+      v = normalize_rgb_u8(s[0], s[1], s[2], m0, m1, m2, s0, s1, s2);
     }
     reinterpret_cast<uint2 *>(y)[i] = v;
+  }
+}
+
+// ---- Pillow-exact bilinear resize (PIL Image.resize(..., BILINEAR) on 8-bit RGB, the resize of odtk/data.py:60) ----
+// Separable triangle filter.  Per output position o of an axis (in -> out samples): scale = in / out, the support is
+// max(scale, 1), the window is [int(center - support + 0.5), int(center + support + 0.5)) clamped to the input, each tap
+// weighs triangle((i - center + 0.5) / max(scale, 1)), the weights are divided by their sum and turned into 22-bit fixed
+// point (rounding half away from zero).  Every double operation is an explicit round-to-nearest intrinsic, so no FMA
+// contraction can change a bit against the C original.  Pixels accumulate in int32 from 1 << 21, >> 22, clamp to
+// [0, 255]; the horizontal result is rounded to uint8 before the vertical pass reads it.  An axis whose lengths match
+// gets weights (1, 0): the identity, like the pass Pillow skips.
+constexpr int RS_BITS = 22;
+constexpr int RS_TW = 32, RS_TH = 64, RS_ROWS = 8;   // 32 x 64 output tile per block of 32 x 8 threads
+constexpr int RS_KMAX = 16;            // taps per position kept in shared memory (axes shrunk up to 7x)
+
+struct ResampleAxis {
+  double center, ss, ww;
+  int lo, count;
+};
+
+__device__ __forceinline__ double resample_scale(int in_size, int out_size) {
+  return __ddiv_rn((double)in_size, (double)out_size);
+}
+
+__device__ __forceinline__ int resample_ksize(int in_size, int out_size) {
+  const double s = resample_scale(in_size, out_size);
+  return (int)ceil(s < 1.0 ? 1.0 : s) * 2 + 1;
+}
+
+__device__ __forceinline__ double resample_tap(const ResampleAxis &a, int j) {
+  double t = __dmul_rn(__dadd_rn(__dadd_rn((double)(a.lo + j), -a.center), 0.5), a.ss);
+  if (t < 0.0) t = -t;
+  return t < 1.0 ? __dadd_rn(1.0, -t) : 0.0;
+}
+
+__device__ ResampleAxis resample_axis(int o, int in_size, int out_size) {
+  ResampleAxis a;
+  const double scale = resample_scale(in_size, out_size);
+  const double support = scale < 1.0 ? 1.0 : scale;          // filter support 1 x max(scale, 1)
+  a.center = __dadd_rn(0.0, __dmul_rn(__dadd_rn((double)o, 0.5), scale));
+  a.ss = __ddiv_rn(1.0, support);
+  a.lo = max(__double2int_rz(__dadd_rn(__dadd_rn(a.center, -support), 0.5)), 0);
+  a.count = min(__double2int_rz(__dadd_rn(__dadd_rn(a.center, support), 0.5)), in_size) - a.lo;
+  double ww = 0.0;
+  for (int j = 0; j < a.count; j++) ww = __dadd_rn(ww, resample_tap(a, j));
+  a.ww = ww;
+  return a;
+}
+
+__device__ __forceinline__ int resample_weight(const ResampleAxis &a, int j) {
+  double k = resample_tap(a, j);
+  if (a.ww != 0.0) k = __ddiv_rn(k, a.ww);
+  const double f = __dmul_rn(k, (double)(1 << RS_BITS));
+  return k < 0.0 ? __double2int_rz(__dadd_rn(-0.5, f)) : __double2int_rz(__dadd_rn(0.5, f));
+}
+
+__device__ __forceinline__ unsigned resample_clip8(int acc) { return (unsigned)min(max(acc >> RS_BITS, 0), 255); }
+
+// grid (ceil((canvas_w + 8) / 32), ceil((canvas_h + 6) / 64), n), 256 threads = 32 columns x 8 rows, each thread writes
+// the 8-byte NHWC4 pixels of one column of the 32 x 64 tile, every 8th row.  A tile that meets the image first puts the
+// fixed-point taps of its 32 columns and 64 rows into shared memory (one thread per column / row, in parallel), then every
+// pixel sums taps x source bytes (sources come through L1).  The taps' double arithmetic is the latency every block waits
+// for once, hence the tall tile.
+__device__ __forceinline__ int resample_acc_init() { return 1 << (RS_BITS - 1); }
+
+__global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kernel(
+    const unsigned char *__restrict__ x, const odtk_resize_image_t *__restrict__ tab, __half *__restrict__ y, int HS, int WS,
+    float m0, float m1, float m2, float s0, float s1, float s2) {
+  __shared__ int s_wx[RS_KMAX][RS_TW], s_wy[RS_TH][RS_KMAX];     // column taps tap-major: lanes read consecutive words
+  __shared__ int s_lox[RS_TW], s_nx[RS_TW], s_loy[RS_TH], s_ny[RS_TH];
+  __shared__ uint2 s_norm[256];   // normalize_rgb_u8(v, v, v): channel c of a pixel is its value's channel c
+  const int HP = HS + 6, WP = WS + 8;
+  const int n = blockIdx.z;
+  const odtk_resize_image_t im = tab[n];
+  const int tx = threadIdx.x % RS_TW, ty = threadIdx.x / RS_TW;
+  const int x0 = blockIdx.x * RS_TW - 3, y0 = blockIdx.y * RS_TH - 3;     // tile origin in image coordinates
+  const int ox = x0 + tx, xp = ox + 3;
+  const bool meets = x0 + RS_TW > 0 && x0 < im.dst_w && y0 + RS_TH > 0 && y0 < im.dst_h;                       // block-uniform
+  const bool tables = meets && resample_ksize(im.src_w, im.dst_w) <= RS_KMAX && resample_ksize(im.src_h, im.dst_h) <= RS_KMAX;
+  if (meets) {
+    for (int v = threadIdx.x; v < 256; v += RS_TW * RS_ROWS) s_norm[v] = normalize_rgb_u8(v, v, v, m0, m1, m2, s0, s1, s2);
+    if (!tables) __syncthreads();
+  }
+  if (tables && threadIdx.x >= RS_TW + RS_TH) {
+    // while the tap threads work, the other warps prefetch the tile's source window into L1 (every row then hits; without
+    // it each of a thread's 8 rows waits for its own miss).  A float estimate widened by the filter support + 2, clamped
+    // to the image: a hint only, the exact windows come from the taps.
+    const float sy = (float)im.src_h / im.dst_h, sx = (float)im.src_w / im.dst_w;
+    const float hy = fmaxf(sy, 1.0f) + 2.0f, hx = fmaxf(sx, 1.0f) + 2.0f;
+    const int r0 = max((int)((float)max(y0, 0) * sy - hy), 0), r1 = min((int)((float)(y0 + RS_TH) * sy + hy) + 1, im.src_h);
+    const int c0 = max((int)((float)max(x0, 0) * sx - hx), 0), c1 = min((int)((float)(x0 + RS_TW) * sx + hx) + 1, im.src_w);
+    const unsigned char *src = x + im.offset;
+    const long long pitch = (long long)im.src_w * 3;
+    const uintptr_t b0 = (uintptr_t)(src + (long long)c0 * 3) & ~(uintptr_t)127;
+    const int lines = (int)(((uintptr_t)(src + (long long)c1 * 3 - 1) - b0) / 128) + 1;
+    for (int i = threadIdx.x - (RS_TW + RS_TH); i < (r1 - r0) * lines; i += RS_TW * RS_ROWS - (RS_TW + RS_TH)) {
+      const int r = r0 + i / lines, l = i % lines;
+      const unsigned char *p = src + (long long)r * pitch + (long long)c0 * 3;
+      const unsigned char *q = reinterpret_cast<const unsigned char *>(b0 + (uintptr_t)l * 128) + (long long)r * pitch;
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(q > p ? q : p));
+    }
+  }
+  if (tables) {
+    if (threadIdx.x < RS_TW) {
+      const int o = x0 + threadIdx.x;
+      if (o >= 0 && o < im.dst_w) {
+        const ResampleAxis a = resample_axis(o, im.src_w, im.dst_w);
+        s_lox[threadIdx.x] = a.lo;
+        s_nx[threadIdx.x] = a.count;
+        for (int j = 0; j < a.count; j++) s_wx[j][threadIdx.x] = resample_weight(a, j);
+      }
+    } else if (threadIdx.x < RS_TW + RS_TH) {
+      const int r = threadIdx.x - RS_TW, o = y0 + r;
+      if (o >= 0 && o < im.dst_h) {
+        const ResampleAxis a = resample_axis(o, im.src_h, im.dst_h);
+        s_loy[r] = a.lo;
+        s_ny[r] = a.count;
+        for (int j = 0; j < a.count; j++) s_wy[r][j] = resample_weight(a, j);
+      }
+    }
+    __syncthreads();
+  }
+  const unsigned char *src = x + im.offset;
+  const long long pitch = (long long)im.src_w * 3;
+  for (int r = ty; r < RS_TH; r += RS_ROWS) {
+    const int oy = y0 + r, yp = oy + 3;
+    if (yp >= HP) break;
+    uint2 v = make_uint2(0u, 0u);
+    if (meets && ox >= 0 && ox < im.dst_w && oy >= 0 && oy < im.dst_h) {
+      int acc[3] = {resample_acc_init(), resample_acc_init(), resample_acc_init()};
+      if (tables) {
+        const int lox = s_lox[tx], nx = s_nx[tx], loy = s_loy[r], ny = s_ny[r];
+        for (int j = 0; j < ny; j++) {
+          const unsigned char *row = src + (long long)(loy + j) * pitch + lox * 3;
+          int h[3] = {resample_acc_init(), resample_acc_init(), resample_acc_init()};
+          for (int i = 0; i < nx; i++) {
+            const int k = s_wx[i][tx];
+#pragma unroll
+            for (int c = 0; c < 3; c++) h[c] += (int)__ldg(row + i * 3 + c) * k;
+          }
+          const int kv = s_wy[r][j];
+#pragma unroll
+          for (int c = 0; c < 3; c++) acc[c] += (int)resample_clip8(h[c]) * kv;
+        }
+      } else {
+        // strong downscale: the windows do not fit the shared tables, every pixel evaluates its own taps
+        const ResampleAxis ax = resample_axis(ox, im.src_w, im.dst_w), ay = resample_axis(oy, im.src_h, im.dst_h);
+        for (int j = 0; j < ay.count; j++) {
+          const unsigned char *row = src + (long long)(ay.lo + j) * pitch + ax.lo * 3;
+          int h[3] = {resample_acc_init(), resample_acc_init(), resample_acc_init()};
+          for (int i = 0; i < ax.count; i++) {
+            const int k = resample_weight(ax, i);
+#pragma unroll
+            for (int c = 0; c < 3; c++) h[c] += (int)__ldg(row + i * 3 + c) * k;
+          }
+          const int kv = resample_weight(ay, j);
+#pragma unroll
+          for (int c = 0; c < 3; c++) acc[c] += (int)resample_clip8(h[c]) * kv;
+        }
+      }
+      // the normalisation is per channel: take r from the red value's entry, g from the green one's, b from the blue one's
+      v = make_uint2(__byte_perm(s_norm[resample_clip8(acc[0])].x, s_norm[resample_clip8(acc[1])].x, 0x7610),
+                     s_norm[resample_clip8(acc[2])].y);
+    }
+    if (xp < WP) reinterpret_cast<uint2 *>(y)[((long long)n * HP + yp) * WP + xp] = v;
   }
 }
 
@@ -299,6 +469,26 @@ extern "C" int odtk_preprocess_u8(const void *x, void *y, int n, int h, int w, i
   OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
   preprocess_u8_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream_>>>(
       (const unsigned char *)x, (__half *)y, n, h, w, hs, ws, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                               const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w,
+                                               void *y, const float *mean, const float *std, odtk_stream_t stream_) {
+  if (!images || n <= 0 || n > 65535 || canvas_h <= 0 || canvas_w <= 0 || (canvas_h % 2) || (canvas_w % 2)) return ODTK_E_INVALID;
+  for (int i = 0; i < n; i++) {
+    const odtk_resize_image_t &im = images[i];
+    if (im.src_h <= 0 || im.src_w <= 0 || im.dst_h <= 0 || im.dst_w <= 0) return ODTK_E_INVALID;
+    if (im.dst_h > canvas_h || im.dst_w > canvas_w) return ODTK_E_INVALID;
+    if (im.offset < 0 || (unsigned long long)im.offset + (unsigned long long)im.src_h * im.src_w * 3 > x_bytes) return ODTK_E_INVALID;
+  }
+  const long long bytes = (long long)n * (canvas_h + 6) * (canvas_w + 8) * 8;
+  if (!y) return bytes;
+  if (!x || !images_dev || !mean || !std) return ODTK_E_INVALID;
+  const dim3 grid((canvas_w + 8 + RS_TW - 1) / RS_TW, (canvas_h + 6 + RS_TH - 1) / RS_TH, n);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  preprocess_resize_u8_kernel<<<grid, RS_TW * RS_ROWS, 0, (cudaStream_t)stream_>>>(
+      (const unsigned char *)x, images_dev, (__half *)y, canvas_h, canvas_w, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 

@@ -342,6 +342,145 @@ def preprocess_u8(images, stride=128, mean=IMAGENET_MEAN, std=IMAGENET_STD):
     return xp, hs, ws
 
 
+def resize_ratio(h, w, resize, max_size):
+    """The inference resize of odtk/data.py:55-60 with the same Python float expressions: ratio = resize / shorter side,
+    lowered to max_size / longer side when the longer side would exceed max_size.  Returns (ratio, dst_h, dst_w)."""
+    ratio = resize / min(h, w)
+    if ratio * max(h, w) > max_size:
+        ratio = max_size / max(h, w)
+    return ratio, int(ratio * h), int(ratio * w)
+
+
+class ResizePlan:
+    """Sizes of one batch of raw images for odtk_preprocess_resize_u8: `table` (odtk_resize_image_t[n], offsets into the
+    packed uint8 bytes of the images in order), `nbytes` (packed size), `ratios` (float32 [n], what odtk/data.py's
+    collate returns), `canvas` (hs, ws): the batch maximum of each stride-padded dst size (collate_fn, odtk/data.py:154-176),
+    or the caller's canvas."""
+
+    def __init__(self, shapes, resize, max_size, stride=128, canvas=None):
+        n = len(shapes)
+        if n == 0:
+            raise ValueError("no images")
+        self.table = (_lib.ResizeImage * n)()
+        ratios, off, hs, ws = [], 0, 0, 0
+        for i, (h, w) in enumerate(shapes):
+            ratio, dh, dw = resize_ratio(h, w, resize, max_size)
+            if dh <= 0 or dw <= 0:
+                raise ValueError("image %d (%dx%d) resizes to %dx%d" % (i, h, w, dh, dw))
+            t = self.table[i]
+            t.offset, t.src_h, t.src_w, t.dst_h, t.dst_w = off, h, w, dh, dw
+            off += h * w * 3
+            ratios.append(ratio)
+            hs, ws = max(hs, -(-dh // stride) * stride), max(ws, -(-dw // stride) * stride)
+        if canvas is not None:
+            ch, cw = int(canvas[0]), int(canvas[1])
+            if ch % stride or cw % stride or ch < hs or cw < ws:
+                raise ValueError("canvas %dx%d must be a multiple of %d and hold the batch's %dx%d" % (ch, cw, stride, hs, ws))
+            hs, ws = ch, cw
+        self.n, self.nbytes, self.canvas = n, off, (hs, ws)
+        self.ratios = torch.tensor(ratios, dtype=torch.float32)
+
+    def table_bytes(self):
+        return torch.frombuffer(bytearray(bytes(self.table)), dtype=torch.uint8)
+
+
+def image_shapes(images):
+    """[(h, w)] of a list of uint8 [h, w, 3] images; ValueError for anything else."""
+    shapes = []
+    for i, im in enumerate(images):
+        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[-1] != 3:
+            raise ValueError("image %d: expected a uint8 [h, w, 3] tensor, got %s %s" % (i, im.dtype, tuple(im.shape)))
+        shapes.append((im.shape[0], im.shape[1]))
+    return shapes
+
+
+TABLE_ALIGN = 256
+
+
+def table_pad(n):
+    """Bytes the size table of n images takes at the front of a staging buffer (the pixels start 256-byte aligned)."""
+    return -(-n * ctypes.sizeof(_lib.ResizeImage) // TABLE_ALIGN) * TABLE_ALIGN
+
+
+def stage_images(images, plan, buf):
+    """Copy the plan's size table and the images (uint8 [h, w, 3], CPU or CUDA) into the device buffer `buf`, laid out
+    [table | pixels packed one after another], on the current stream.  CPU images go through one pinned buffer: table
+    and pixels leave in ONE H2D copy.  Returns (table view, pixel view) of buf."""
+    tpad = table_pad(plan.n)
+    assert buf.dtype == torch.uint8 and buf.numel() >= tpad + plan.nbytes
+    tb = plan.table_bytes()
+    if all(not im.is_cuda for im in images):
+        pinned = torch.empty(tpad + plan.nbytes, dtype=torch.uint8, pin_memory=True)
+        pinned[:tb.numel()].copy_(tb)
+        torch.cat([im.reshape(-1) for im in images], out=pinned[tpad:])
+        buf[:tpad + plan.nbytes].copy_(pinned, non_blocking=True)
+    else:
+        buf[:tb.numel()].copy_(tb.pin_memory(), non_blocking=True)
+        torch.cat([im.to(buf.device).reshape(-1) for im in images], out=buf[tpad:tpad + plan.nbytes])
+    return buf[:tpad], buf[tpad:]
+
+
+def resize_launch(x_dev, x_bytes, plan, table_dev, out=None, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """odtk_preprocess_resize_u8 over already staged bytes: returns the stem buffer [n, hs+6, ws+8, 4] fp16 (or writes
+    `out`)."""
+    hs, ws = plan.canvas
+    L = _lib.lib()
+    nbytes = _lib.check(L.odtk_preprocess_resize_u8(None, x_bytes, ctypes.byref(plan.table), None, plan.n, hs, ws, None, None,
+                                                    None, None), "preprocess_resize_u8")
+    if out is None:
+        out = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=torch.float16, device=x_dev.device)
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.numel() * 2 == nbytes
+    m = (ctypes.c_float * 3)(*mean)
+    s = (ctypes.c_float * 3)(*std)
+    _lib.check(L.odtk_preprocess_resize_u8(ctypes.c_void_p(x_dev.data_ptr()), x_bytes, ctypes.byref(plan.table),
+                                           ctypes.c_void_p(table_dev.data_ptr()), plan.n, hs, ws, ctypes.c_void_p(out.data_ptr()),
+                                           m, s, _stream()), "preprocess_resize_u8")
+    STATS["launches"] += 1
+    _trace("preprocess_resize_u8", 0, resize_bytes(plan), n=plan.n, h=hs, w=ws, cin=3)
+    return out
+
+
+def resize_bytes(plan):
+    """Algorithmic HBM bytes of one odtk_preprocess_resize_u8 launch: every source byte read once, the size table, the
+    whole fp16 NHWC4 canvas written once."""
+    hs, ws = plan.canvas
+    return plan.nbytes + ctypes.sizeof(plan.table) + plan.n * (hs + 6) * (ws + 8) * 8
+
+
+def preprocess_resize_u8(images, resize, max_size, stride=128, canvas=None, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """Input side of `odtk infer` for a list of raw uint8 [h_i, w_i, 3] RGB images of any sizes (odtk/data.py:55-60,
+    113-123, collate_fn :154-176): Pillow-exact BILINEAR resize by the reference's ratio, normalisation, stride and batch
+    padding, written straight into the stem's zero-bordered NHWC4 fp16 buffer [n, hs+6, ws+8, 4] by one kernel.  CPU
+    images are staged through pinned memory with one H2D copy; CUDA images are read in place.  `canvas` (hs, ws): a fixed
+    batch canvas (multiples of `stride`); default the batch maximum of the stride-padded sizes.  Returns (xp, hs, ws,
+    ratios float32 [n])."""
+    plan = ResizePlan(image_shapes(images), resize, max_size, stride, canvas)
+    dev = next((im.device for im in images if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
+    if all(im.is_cuda and im.is_contiguous() for im in images):
+        # in place: offsets from the lowest image address (one flat device address space)
+        base = min(im.data_ptr() for im in images)
+        for t, im in zip(plan.table, images):
+            t.offset = im.data_ptr() - base
+        x_bytes = max(im.data_ptr() + im.numel() for im in images) - base
+        table_dev = plan.table_bytes().pin_memory().to(dev, non_blocking=True)
+        x_dev = _DevPtr(base, dev)
+    else:
+        table_dev, x_dev = stage_images(images, plan, torch.empty(table_pad(plan.n) + plan.nbytes, dtype=torch.uint8, device=dev))
+        x_bytes = plan.nbytes
+    xp = resize_launch(x_dev, x_bytes, plan, table_dev, mean=mean, std=std)
+    return xp, plan.canvas[0], plan.canvas[1], plan.ratios
+
+
+class _DevPtr:
+    """A raw device address with the two tensor attributes resize_launch reads."""
+
+    def __init__(self, ptr, device):
+        self.ptr, self.device = ptr, device
+
+    def data_ptr(self):
+        return self.ptr
+
+
 def stem_conv_padded(xp, h, wd, w, bias, cout, relu=True):
     """Stem over an already padded NHWC4 buffer [N, h+6, wd+8, 4] (from preprocess_u8)."""
     n = xp.shape[0]

@@ -59,6 +59,29 @@ def infer(model, path, detections_file=None, resize=None, max_size=None, batch_s
     return gather_detections(*unpack_detections(packed), world=max(world, 1))
 
 
+def infer_images(model, batches, resize=800, max_size=1333, world=0):
+    """The per-batch loop of `infer` over lists of raw uint8 [h, w, 3] RGB images of any sizes (the reference's PIL data
+    loader path, odtk/data.py:55-60, 113-123, 154-176): Model.forward_images resizes, normalises and pads each batch on
+    the GPU.  Returns (scores [N, D], boxes [N, D, nbox] in resized coordinates, classes [N, D], ratios float32 [N]) for the
+    images of ALL ranks, rank-major like `infer`; detections_to_coco(scores, boxes, classes, ratios) gives odtk infer's
+    output."""
+    results, ratios = [], []
+    with torch.no_grad():
+        for images in batches:
+            (scores, boxes, classes), r = model.forward_images(images, resize, max_size)
+            results.append(pack_detections(scores, boxes, classes))
+            ratios.append(r)
+    packed = torch.cat(results, dim=0)
+    ratios = torch.cat(ratios)
+    world = max(world, 1)
+    if world > 1:
+        r = ratios.to(packed.device)
+        out = torch.empty(world * r.numel(), dtype=r.dtype, device=r.device)
+        dist.all_gather_into_tensor(out, r)
+        ratios = out.cpu()
+    return gather_detections(*unpack_detections(packed), world=world) + (ratios,)
+
+
 def detections_to_coco(scores, boxes, classes, ratios, image_ids=None, category_ids=None):
     """Output side of `odtk infer` (odtk/infer.py:104-148, axis-aligned branch): keep score > 0, undo the
     resize ratio, convert (x1, y1, x2, y2) to COCO (x, y, w, h) with the +1 width convention.

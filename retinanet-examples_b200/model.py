@@ -961,6 +961,9 @@ class Model:
         else:
             width = x.shape[-1]
             features = self._features(self._stem(self._to_nhwc_half(x)))
+        return self._detect_fused(features, width)
+
+    def _detect_fused(self, features, width):
         sizes = tuple((f.shape[1], f.shape[2]) for f in features)
         batch = features[0].shape[0]
         key = (batch, sizes, width, self.threshold, self.top_n, self.rotated_bbox)
@@ -1049,9 +1052,70 @@ class Model:
         if self.exporting:
             self.strides = [width // c.shape[-1] for c in cls_heads]
             return cls_heads, box_heads
+        return self._detect_dense(cls_heads, box_heads, width)
+
+    def _detect_dense(self, cls_heads, box_heads, width):
         strides, anchors = self._level_anchors([c.shape[-1] for c in cls_heads], width)
         decoded = _C.decode_levels(cls_heads, box_heads, anchors, strides, self.threshold, self.top_n, self.rotated_bbox)
         return self._nms(decoded)
+
+    # ---- raw images of any size (the PIL data loader of `odtk infer`, odtk/data.py:55-60, 113-123, 154-176) ------------
+    def _forward_padded(self, xp, hs, width):
+        """Detections from the stem's padded NHWC4 input buffer: the fused-candidate or the dense route of forward()."""
+        features = self._features(self._stem(padded=(xp, hs, width)))
+        if self.fused_candidates:
+            return self._detect_fused(features, width)
+        return self._detect_dense(*self._heads(features), width)
+
+    def forward_images(self, images, resize=800, max_size=1333, canvas=None):
+        """Inference on a list of raw uint8 [h_i, w_i, 3] RGB images of any sizes (CPU or CUDA tensors): each image is
+        resized by the reference's ratio with Pillow-exact BILINEAR resampling, normalised and padded into one batch
+        canvas by one kernel (engine.preprocess_resize_u8), then the network runs as forward() does.  `canvas` (hs, ws):
+        a fixed canvas (multiples of 128) shared by every batch, hence one CUDA graph; default the reference collate's
+        batch maximum.  Returns ((scores, boxes, classes), ratios): boxes in resized coordinates, as the reference model
+        returns them; ratios float32 [n] (divide by them for original coordinates, infer.detections_to_coco).
+        With enable_cuda_graph() one graph per (n, canvas) is replayed; its staging buffers grow (and the graph is
+        captured again) when a batch has more bytes than they hold."""
+        if self._packed is None:
+            raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
+        if self.training or self.exporting:
+            raise RuntimeError("forward_images runs inference: call .eval() and leave exporting off")
+        plan = engine.ResizePlan(engine.image_shapes(images), resize, max_size, self.stride, canvas)
+        hs, ws = plan.canvas
+        if getattr(self, "_graphs", None) is None:
+            xp, _, _, ratios = engine.preprocess_resize_u8(images, resize, max_size, self.stride, (hs, ws))
+            return self._forward_padded(xp, hs, ws), ratios
+        key = ("images", plan.n, hs, ws)
+        entry = self._graphs.get(key)
+        if entry is None or entry["capacity"] < plan.nbytes:
+            entry = self._graphs[key] = self._capture_images(images, plan, max(plan.nbytes, 2 * entry["capacity"] if entry else 0))
+        engine.stage_images(images, plan, entry["buf"])
+        entry["graph"].replay()
+        if self.gather is not None:
+            self.gather.steps += 1
+        return entry["out"], plan.ratios
+
+    def _capture_images(self, images, plan, capacity):
+        """CUDA graph of resize + network over static device buffers: [size table | packed pixels] of `capacity` bytes and
+        the stem buffer.  The kernel reads the sizes from the device table, so any batch that fits the canvas replays it."""
+        dev = self._packed["stem"].w_stem.device
+        tpad = engine.table_pad(plan.n)
+        buf = torch.empty(tpad + capacity, dtype=torch.uint8, device=dev)
+        hs, ws = plan.canvas
+        xp = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=torch.float16, device=dev)
+
+        def run():
+            engine.resize_launch(buf[tpad:], capacity, plan, buf[:tpad], out=xp)
+            return self._forward_padded(xp, hs, ws)
+
+        engine.stage_images(images, plan, buf)
+        for _ in range(2):                      # warm-up: lazy attribute set-up, allocator, anchors
+            run()
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = run()
+        return {"graph": graph, "buf": buf, "xp": xp, "out": out, "capacity": capacity}
 
     # ---- CUDA graph replay ---------------------------------------------------------------------
     def enable_cuda_graph(self, enabled=True):

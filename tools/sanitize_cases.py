@@ -149,6 +149,15 @@ def main():
         loss.retina_loss([c], [b], [ci], [bt], 3, with_grad=True)
         torch.cuda.synchronize()
         print("loss ok", flush=True)
+    if only in ("", "resize"):
+        # raw-image resize into the stem buffer: an upscale, a downscale within the shared tap tables, one beyond them
+        # (per-pixel taps), a same-size image and a tiny one, ragged in one canvas; CPU (staged) and CUDA (in place) input
+        imgs = [torch.randint(0, 256, s, dtype=torch.uint8, generator=g) for s in ((30, 40, 3), (300, 170, 3), (900, 41, 3),
+                                                                                    (64, 100, 3), (3, 5, 3))]
+        engine.preprocess_resize_u8(imgs, 64, 100)
+        engine.preprocess_resize_u8([i.to(DEV) for i in imgs], 64, 100, canvas=(256, 128))
+        torch.cuda.synchronize()
+        print("resize ok", flush=True)
 
 
 if __name__ == "__main__":
