@@ -445,6 +445,63 @@ long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, const odtk_re
                                     const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w, void *y,
                                     const float *mean, const float *std, odtk_stream_t stream);
 
+/* ---- baseline JPEG decode (the Image.open(path).convert("RGB") of odtk/data.py:50, on the GPU) ------------------
+ * One image of odtk_decode_jpeg: a baseline sequential Huffman-coded 8-bit JPEG (SOF0 / SOF1), grayscale or YCbCr
+ * with luma sampling 1x1 (4:4:4), 2x1 (4:2:2) or 2x2 (4:2:0) and 1x1 chroma.  Byte offsets are from the start of
+ * the input buffer `in`; the sums (seg_base, blk_base, pix_base) run over the images in order.                  */
+typedef struct {
+  long long scan_offset;   /* entropy-coded data of the scan, RSTn markers included, EOI excluded              */
+  long long blk_base;      /* first 8x8 block of the image in the workspace (all components, Y then Cb, Cr)    */
+  long long pix_base;      /* sum of height x width of the images before this one                              */
+  int scan_bytes, height, width;
+  int ncomp;               /* 1 (grayscale) or 3 (YCbCr)                                                        */
+  int hmax, vmax;          /* luma sampling factors; 1, 1 for grayscale                                         */
+  int restart_interval;    /* MCUs per restart segment, 0 = no restart markers                                  */
+  int nseg;                /* restart segments: ceil(MCUs / restart_interval), 1 without DRI                    */
+  int seg_base;            /* first segment of the image in the batch                                           */
+  int quant[3];            /* per component: offset of 64 uint16 quantisation steps, row-major, 16-byte aligned */
+  int dc[3], ac[3];        /* per component: offsets of its odtk_jpeg_huff_t DC and AC tables, 16-byte aligned */
+} odtk_jpeg_image_t;
+
+/* One Huffman table (T.81 annex C canonical code) as the decoder reads it. */
+typedef struct {
+  unsigned short look[256]; /* next 8 bits -> (code length << 8) | symbol; 0 when the code is longer than 8 bits   */
+  int maxcode[18];          /* largest code of each length 1..16, -1 when there is none; [17] = INT_MAX           */
+  int valoff[18];           /* val index of a code of length l = code + valoff[l]                                  */
+  unsigned char val[256];   /* the symbols in code order                                                           */
+} odtk_jpeg_huff_t;
+
+/* Status bits per image (int32 status[n]; 0 = decoded).                                                      */
+#define ODTK_JPEG_BAD_CODE 1       /* a bit pattern that is no code of the Huffman table                        */
+#define ODTK_JPEG_BAD_INDEX 2      /* a run of zeros past coefficient 63                                        */
+#define ODTK_JPEG_TRUNCATED 4      /* a restart segment ran out of entropy-coded data                           */
+#define ODTK_JPEG_BAD_RESTART 8    /* the scan does not hold nseg - 1 restart markers                            */
+
+/* Decode n baseline JPEGs bit-exactly as libjpeg(-turbo) does by default (Huffman decode, dequantisation, the
+ * JDCT_ISLOW integer IDCT with its range limit, "fancy" triangle-filter chroma upsampling, the fixed-point table
+ * YCbCr -> RGB conversion) into uint8 HWC RGB images; grayscale is replicated to three channels.  Four kernels:
+ * restart-marker scan (one block per image), entropy decode (one thread per image and restart segment), IDCT (one
+ * thread per 8x8 block), upsampling + colour conversion (one thread per pixel).
+ *   in, in_bytes   device buffer [odtk_jpeg_image_t[n] | ... tables ... | entropy-coded bytes]; the descriptor
+ *                  table at offset 0 is what the kernels read;
+ *   images         host copy of that descriptor table: validated here, never read by a kernel;
+ *   outs, outs_dev host table / its device copy: image i is written at y + outs[i].offset, src_h x src_w must be
+ *                  its height x width (dst_h / dst_w are not read);
+ *   workspace      restart segment bounds, int16 coefficient blocks, uint8 component planes; the kernels place
+ *                  these regions from the totals of the device descriptor table, not from this call's host table;
+ *   status         int32 [n] device: ODTK_JPEG_* bits of each image.  A corrupt stream never faults: its decoder
+ *                  stops, sets the bits and the other images are unaffected.
+ * Sizes come from the device tables, so a CUDA graph may replay the call after the caller rewrote `in` and
+ * outs_dev with another batch of n images that the host tables validated and whose totals fit the buffers (its
+ * workspace need, from the size query, at most workspace_bytes), even when it has more blocks or restart segments
+ * than the batch the graph was captured with.  An image of more than INT32_MAX pixels is ODTK_E_UNSUPPORTED.
+ * Two-phase: workspace == NULL returns the workspace bytes.  ODTK_E_INVALID: a size <= 0, inconsistent sums, an
+ * offset outside its buffer; ODTK_E_UNSUPPORTED: a component count or sampling factors outside the above;
+ * ODTK_E_WORKSPACE: workspace_bytes too small.                                                                */
+long long odtk_decode_jpeg(const void *in, size_t in_bytes, const odtk_jpeg_image_t *images, int n,
+                           const odtk_resize_image_t *outs, const odtk_resize_image_t *outs_dev, void *workspace,
+                           size_t workspace_bytes, void *y, size_t y_bytes, int *status, odtk_stream_t stream);
+
 /* ---- per-kernel timing (H100-native addition; the reference has only a wall-clock
  * Profiler without CUDA sync, odtk/utils.py:140-167) ------------------------------
  * When enabled, every launch of a tagged kernel is bracketed by CUDA events on the

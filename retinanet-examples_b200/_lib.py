@@ -87,6 +87,9 @@ SIGNATURES = {
     "odtk_preprocess_u8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [_c_f32p, _c_f32p, ctypes.c_void_p]),
     "odtk_preprocess_resize_u8": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p] +
                                   [ctypes.c_int] * 3 + [ctypes.c_void_p, _c_f32p, _c_f32p, ctypes.c_void_p]),
+    "odtk_decode_jpeg": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
+                                             ctypes.c_void_p, ctypes.c_void_p]),
     "odtk_prof_enable": (None, [ctypes.c_int]),
     "odtk_prof_reset": (None, []),
     "odtk_prof_get_list": (ctypes.c_longlong, [ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.c_longlong]),
@@ -134,6 +137,19 @@ class ResizeImage(ctypes.Structure):
     """odtk_resize_image_t (include/odtk_b200.h)."""
     _fields_ = [("offset", ctypes.c_longlong), ("src_h", ctypes.c_int), ("src_w", ctypes.c_int), ("dst_h", ctypes.c_int),
                 ("dst_w", ctypes.c_int)]
+
+
+class JpegImage(ctypes.Structure):
+    """odtk_jpeg_image_t (include/odtk_b200.h)."""
+    _fields_ = [("scan_offset", ctypes.c_longlong), ("blk_base", ctypes.c_longlong), ("pix_base", ctypes.c_longlong)] + \
+               [(f, ctypes.c_int) for f in ("scan_bytes", "height", "width", "ncomp", "hmax", "vmax", "restart_interval", "nseg",
+                                            "seg_base")] + [(f, ctypes.c_int * 3) for f in ("quant", "dc", "ac")]
+
+
+class JpegHuff(ctypes.Structure):
+    """odtk_jpeg_huff_t (include/odtk_b200.h)."""
+    _fields_ = [("look", ctypes.c_uint16 * 256), ("maxcode", ctypes.c_int * 18), ("valoff", ctypes.c_int * 18),
+                ("val", ctypes.c_uint8 * 256)]
 
 
 class CandSink(ctypes.Structure):

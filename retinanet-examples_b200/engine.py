@@ -471,6 +471,59 @@ def preprocess_resize_u8(images, resize, max_size, stride=128, canvas=None, mean
     return xp, plan.canvas[0], plan.canvas[1], plan.ratios
 
 
+def jpeg_launch(batch, buf, outs, workspace, y, status):
+    """odtk_decode_jpeg over a staged batch (jpeg.JpegBatch.stage): `buf` the staging buffer (its odtk_resize_image_t
+    copy at batch.resize_off is the device output table), `outs` the host output table, `y` the packed uint8 pixels,
+    `status` int32 [n].  workspace=None returns the workspace bytes the batch needs (and validates the tables)."""
+    L = _lib.lib()
+    ws_ptr = ctypes.c_void_p(workspace.data_ptr()) if workspace is not None else None
+    rc = _lib.check(L.odtk_decode_jpeg(ctypes.c_void_p(buf.data_ptr()) if workspace is not None else None, buf.numel(),
+                                       ctypes.byref(batch.images), batch.n, ctypes.byref(outs),
+                                       ctypes.c_void_p(buf.data_ptr() + batch.resize_off), ws_ptr,
+                                       workspace.numel() if workspace is not None else 0,
+                                       ctypes.c_void_p(y.data_ptr()), y.numel(),
+                                       ctypes.c_void_p(status.data_ptr()) if status is not None else None, _stream()),
+                    "decode_jpeg")
+    if workspace is not None:
+        STATS["launches"] += 4
+        _trace("decode_jpeg", 0, jpeg_bytes(batch), n=batch.n, h=0, w=0, cin=3)
+    return rc
+
+
+def jpeg_bytes(batch):
+    """Algorithmic HBM bytes of one odtk_decode_jpeg call: the staged input read once (the marker scan and the entropy
+    decode each read the scan bytes), coefficients written and read (128 B per block), planes written and read (64 B per
+    block, chroma read up to 4 times by the colour kernel, counted once), RGB pixels written."""
+    return batch.nbytes + sum(t.scan_bytes for t in batch.images) + batch.blocks * (256 + 128) + batch.pixels * 3
+
+
+def _output_table(shapes):
+    """odtk_resize_image_t[n] packing uint8 [h, w, 3] images one after another (dst = src) and the total bytes."""
+    outs = (_lib.ResizeImage * len(shapes))()
+    off = 0
+    for t, (h, w) in zip(outs, shapes):
+        t.offset, t.src_h, t.src_w, t.dst_h, t.dst_w = off, h, w, h, w
+        off += h * w * 3
+    return outs, off
+
+
+def decode_jpeg(datas, device=None):
+    """Decode a list of baseline JPEG streams (bytes-like) on the GPU, bit-exact to Pillow's
+    np.asarray(Image.open(f).convert("RGB")).  The host parses headers and stages the batch with one pinned H2D copy.
+    Returns (list of uint8 [h, w, 3] CUDA views into one packed buffer, status int32 [n] CUDA: 0 or ODTK_JPEG_* bits).
+    ValueError names the image and the reason for a stream the decoder does not take (progressive, CMYK, ...)."""
+    from . import jpeg
+    batch = jpeg.JpegBatch(datas)
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    outs, nbytes = _output_table(batch.shapes)
+    buf = batch.stage(outs, torch.empty(batch.nbytes, dtype=torch.uint8, device=dev))
+    y = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    workspace = torch.empty(batch.workspace_bytes(), dtype=torch.uint8, device=dev)
+    status = torch.empty(batch.n, dtype=torch.int32, device=dev)
+    jpeg_launch(batch, buf, outs, workspace, y, status)
+    return [y[t.offset:t.offset + h * w * 3].view(h, w, 3) for t, (h, w) in zip(outs, batch.shapes)], status
+
+
 class _DevPtr:
     """A raw device address with the two tensor attributes resize_launch reads."""
 

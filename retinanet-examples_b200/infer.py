@@ -82,6 +82,33 @@ def infer_images(model, batches, resize=800, max_size=1333, world=0):
     return gather_detections(*unpack_detections(packed), world=world) + (ratios,)
 
 
+def infer_jpeg(model, batches, resize=800, max_size=1333, world=0):
+    """infer_images over lists of baseline JPEG streams (bytes-like): Model.forward_jpeg decodes them on the GPU, bit-exact
+    to the reference loader's Image.open(path).convert("RGB") (odtk/data.py:50), then resizes, normalises and pads.
+    Returns (scores, boxes, classes, ratios, status int32 [N]) for the images of ALL ranks, rank-major like `infer`;
+    status is 0 for a decoded image and ODTK_JPEG_* bits for a corrupt one."""
+    results, ratios, status = [], [], []
+    with torch.no_grad():
+        for datas in batches:
+            (scores, boxes, classes), r, s = model.forward_jpeg(datas, resize, max_size)
+            results.append(pack_detections(scores, boxes, classes))
+            ratios.append(r)
+            status.append(s.clone())
+    packed = torch.cat(results, dim=0)
+    ratios = torch.cat(ratios)
+    status = torch.cat(status)
+    world = max(world, 1)
+    if world > 1:
+        r = ratios.to(packed.device)
+        out = torch.empty(world * r.numel(), dtype=r.dtype, device=r.device)
+        dist.all_gather_into_tensor(out, r)
+        ratios = out.cpu()
+        s = torch.empty(world * status.numel(), dtype=status.dtype, device=status.device)
+        dist.all_gather_into_tensor(s, status)
+        status = s
+    return gather_detections(*unpack_detections(packed), world=world) + (ratios, status.cpu())
+
+
 def detections_to_coco(scores, boxes, classes, ratios, image_ids=None, category_ids=None):
     """Output side of `odtk infer` (odtk/infer.py:104-148, axis-aligned branch): keep score > 0, undo the
     resize ratio, convert (x1, y1, x2, y2) to COCO (x, y, w, h) with the +1 width convention.

@@ -1117,6 +1117,79 @@ class Model:
             out = run()
         return {"graph": graph, "buf": buf, "xp": xp, "out": out, "capacity": capacity}
 
+    # ---- JPEG streams (the Image.open(path).convert("RGB") of odtk/data.py:50, then the raw-image path) ------------------
+    def forward_jpeg(self, datas, resize=800, max_size=1333, canvas=None):
+        """Inference on a list of baseline JPEG streams (bytes-like, e.g. open(path, "rb").read()): the GPU decodes them
+        bit-exactly as Pillow's Image.open(f).convert("RGB") does (engine.decode_jpeg), then they go through
+        forward_images' resize + network path.  Returns ((scores, boxes, classes), ratios, status): status int32 [n]
+        CUDA, 0 or the ODTK_JPEG_* bits of an image whose scan is corrupt (its detections are then meaningless, the
+        other images are unaffected).  A stream the decoder does not take (progressive, CMYK, ...) raises ValueError
+        naming the image: decode it with Pillow and use forward_images.
+        With enable_cuda_graph() one graph per (n, canvas) covers decode, resize and network; its staging, workspace
+        and pixel buffers grow (and the graph is captured again) when a batch needs more than they hold."""
+        from . import jpeg
+        if self._packed is None:
+            raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
+        if self.training or self.exporting:
+            raise RuntimeError("forward_jpeg runs inference: call .eval() and leave exporting off")
+        batch = jpeg.JpegBatch(datas)
+        plan = engine.ResizePlan(batch.shapes, resize, max_size, self.stride, canvas)
+        hs, ws = plan.canvas
+        need = (batch.nbytes, batch.workspace_bytes(), plan.nbytes)
+        if getattr(self, "_graphs", None) is None:
+            bufs = self._jpeg_buffers(plan.n, need)
+            batch.stage(plan.table, bufs["buf"])
+            xp = self._jpeg_decode_resize(batch, plan, bufs)
+            return self._forward_padded(xp, hs, ws), plan.ratios, bufs["status"]
+        key = ("jpeg", plan.n, hs, ws)
+        entry = self._graphs.get(key)
+        if entry is None or any(a > b for a, b in zip(need, entry["capacity"])):
+            cap = tuple(max(a, 2 * b) for a, b in zip(need, entry["capacity"])) if entry else need
+            entry = self._graphs[key] = self._capture_jpeg(batch, plan, cap)
+        else:
+            bufs = entry["bufs"]
+            engine.jpeg_launch(batch, bufs["buf"], plan.table, None, bufs["pixels"], None)    # validate the host tables
+            batch.stage(plan.table, bufs["buf"])
+        entry["graph"].replay()
+        if self.gather is not None:
+            self.gather.steps += 1
+        return entry["out"], plan.ratios, entry["bufs"]["status"]
+
+    def _jpeg_buffers(self, n, capacity):
+        dev = self._packed["stem"].w_stem.device
+        staging, workspace, pixels = capacity
+        return {"buf": torch.empty(staging, dtype=torch.uint8, device=dev),
+                "workspace": torch.empty(workspace, dtype=torch.uint8, device=dev),
+                "pixels": torch.empty(pixels, dtype=torch.uint8, device=dev),
+                "status": torch.empty(n, dtype=torch.int32, device=dev)}
+
+    def _jpeg_decode_resize(self, batch, plan, bufs, xp=None):
+        """Decode into the packed pixel buffer at the resize plan's offsets, then resize it into the stem buffer; the
+        resize kernel reads the size table staged with the batch."""
+        engine.jpeg_launch(batch, bufs["buf"], plan.table, bufs["workspace"], bufs["pixels"], bufs["status"])
+        return engine.resize_launch(bufs["pixels"], bufs["pixels"].numel(), plan, bufs["buf"][batch.resize_off:], out=xp)
+
+    def _capture_jpeg(self, batch, plan, capacity):
+        """CUDA graph of decode + resize + network over static buffers of `capacity` (staging, workspace, pixel bytes)
+        and the stem buffer.  Every kernel reads its sizes from the staged tables, so any batch of n JPEGs that fits the
+        canvas and the buffers replays it."""
+        bufs = self._jpeg_buffers(plan.n, capacity)
+        hs, ws = plan.canvas
+        xp = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=torch.float16, device=bufs["buf"].device)
+
+        def run():
+            self._jpeg_decode_resize(batch, plan, bufs, xp)
+            return self._forward_padded(xp, hs, ws)
+
+        batch.stage(plan.table, bufs["buf"])
+        for _ in range(2):                      # warm-up: lazy attribute set-up, allocator, anchors
+            run()
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            out = run()
+        return {"graph": graph, "bufs": bufs, "xp": xp, "out": out, "capacity": capacity}
+
     # ---- CUDA graph replay ---------------------------------------------------------------------
     def enable_cuda_graph(self, enabled=True):
         """Capture the whole forward (≈125 kernel launches, no host sync anywhere on the path) into a

@@ -158,6 +158,17 @@ def main():
         engine.preprocess_resize_u8([i.to(DEV) for i in imgs], 64, 100, canvas=(256, 128))
         torch.cuda.synchronize()
         print("resize ok", flush=True)
+    if only in ("", "jpeg"):
+        # JPEG decode kernels (restart scan, entropy decode, IDCT, upsample + colour): every sampling, grayscale, restart
+        # intervals, a 640x480 image, then a batch with a truncated stream (its decoder runs out of data and stops)
+        import numpy as np
+        fx = np.load(os.path.join(ROOT, "tests", "golden", "jpeg_pil.npz"))
+        datas = [fx[n + "_jpeg"].tobytes() for n in ("420_q75", "422_restart_rows", "444_restart3", "gray_q100", "420_640x480",
+                                                     "420_1x1")]
+        engine.decode_jpeg(datas)
+        _, status = engine.decode_jpeg(datas[:2] + [fx["truncated_jpeg"].tobytes()])
+        torch.cuda.synchronize()
+        print("jpeg ok status=%s" % status.cpu().tolist(), flush=True)
 
 
 if __name__ == "__main__":
