@@ -267,6 +267,49 @@ int odtk_conv2d_s8_ex(const odtk_conv_s8_ex_t *desc, odtk_stream_t stream);
  * everything a multiple of 16, 16-byte aligned): the input of FPN pyramid7, ReLU(P6), from a level of the s8 atlas. */
 int odtk_relu_copy_rows_s8(const void *x, void *y, int n, int rows, int row_elems, long long x_img_pitch,
                            long long x_row_pitch, long long y_img_pitch, long long y_row_pitch, odtk_stream_t stream);
+/* Full-precision convolution (the reference's --full-precision, odtk/main.py:192-195, odtk/infer.py:54-58): fp32
+ * activations, fp32 weights split on the host into two tf32-valued halves w_hi = rna_tf32(w), w_lo = rna_tf32(w - w_hi)
+ * (low 13 bits zero, [cout, ksize*ksize*cin], tap-major / channel-minor).  The kernel splits the activations the same way
+ * and accumulates a_hi*b_lo + a_lo*b_hi + a_hi*b_hi on the tf32 tensor cores into fp32 ("3xTF32"): the operand error per
+ * product is about 3 * 2^-22 |a||b| instead of 2^-11 for one TF32 pass.  Then + bias, + residual, + upsample (fp32 adds),
+ * ReLU, and one output mode:
+ *     ODTK_OUT_NHWC_F32          y: NHWC fp32 [n, oh, ow, ldy] (or a level view of an fp32 atlas)
+ *     ODTK_OUT_NCHW_F32[_SIGMOID], ODTK_OUT_CANDIDATES   as for odtk_conv2d
+ * ksize 1 / 3 with cin % 32 == 0, stride 1 / 2 (pad ksize/2), the views and tile tables of odtk_conv_t; or ksize 7,
+ * stride 2, cin 3: the ResNet stem (pad 3) over x = the NHWC4 fp32 image [n, h+6, width+8, 4] of odtk_pad_input_f32, with
+ * w packed [cout, 224] as k = r*32 + s*4 + c (zero for s = 7 or c = 3); any h and width.  NHWC outputs need cout even.  Addends and output
+ * views need ODTK_OUT_NHWC_F32; views and tile tables are 3x3 without addends; upsample needs stride 1 and even h, width.
+ * Anything else returns ODTK_E_UNSUPPORTED.                                                                           */
+#define ODTK_OUT_NHWC_F32 5
+typedef struct {
+  const void *x;        /* NHWC fp32 [n, h, width, cin] (stem: NHWC4 fp32 [n, h+6, width+8, 4])   */
+  const void *w_hi;     /* fp32 [cout, ksize*ksize*cin], tf32-valued                             */
+  const void *w_lo;     /* fp32, same shape: rna_tf32(w - w_hi)                                  */
+  const float *bias;    /* fp32 [cout] or NULL                                                   */
+  const void *residual; /* NHWC fp32 [n, oh, ow, ldr] or NULL                                   */
+  const void *upsample; /* NHWC fp32 [n, h/2, width/2, cout] (nearest-2x, stride 1) or NULL     */
+  void *y;
+  int n, h, width, cin, cout, ksize, stride, relu /* 0 / 1 */, out_mode, ldy, ldr;
+  const odtk_cand_sink_t *sink;
+  int x_rows, x_width;
+  int y_rows, y_row_off, y_width;
+  const void *tile_tab;
+  int tab_tiles;
+} odtk_conv_f32_t;
+int odtk_conv2d_f32(const odtk_conv_f32_t *desc, odtk_stream_t stream);
+/* fp32 twins of the small layers around the convolutions (full-precision mode), same geometry as the fp16 calls:
+ *   odtk_pad_input_f32          NHWC fp32 RGB [n, h, w, 3] -> zero-bordered NHWC4 fp32 [n, h+6, w+8, 4]
+ *   odtk_preprocess_u8_f32      as odtk_preprocess_u8, the normalised fp32 values without the fp16 rounding
+ *   odtk_preprocess_resize_u8_f32   (declared after odtk_preprocess_resize_u8) the same resize, y NHWC4 fp32
+ *   odtk_maxpool3x3s2_f32      NHWC fp32, c % 4 == 0
+ *   odtk_relu_copy_rows_f32     y = max(x, 0) over n x rows runs of row_elems floats (pitches in elements, multiples of
+ *                               4, 16-byte aligned): pyramid7's input ReLU(P6) from a level of the fp32 atlas        */
+int odtk_pad_input_f32(const void *x, void *y, int n, int h, int w, odtk_stream_t stream);
+int odtk_preprocess_u8_f32(const void *x, void *y, int n, int h, int w, int hs, int ws, const float *mean,
+                           const float *std, odtk_stream_t stream);
+int odtk_maxpool3x3s2_f32(const void *x, void *y, int n, int h, int w, int c, odtk_stream_t stream);
+int odtk_relu_copy_rows_f32(const void *x, void *y, int n, int rows, int row_elems, long long x_img_pitch,
+                            long long x_row_pitch, long long y_img_pitch, long long y_row_pitch, odtk_stream_t stream);
 /* y[i] = clamp(rint((float)x[i] * inv_scale), -127, 127): fp16 -> s8, n % 8 == 0, 16-byte aligned x, 8-byte aligned y. */
 int odtk_quantize_f16_s8(const void *x, void *y, long long n, float inv_scale, odtk_stream_t stream);
 /* Introspection (tests): the kernel variant the last odtk_conv2d / odtk_stem_conv call of the calling host thread
@@ -444,6 +487,11 @@ typedef struct {
 long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
                                     const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w, void *y,
                                     const float *mean, const float *std, odtk_stream_t stream);
+/* The same resize into the fp32 NHWC4 stem buffer of the full-precision mode: the normalised fp32 values without the
+ * fp16 rounding.  Same arguments and checks; y == NULL returns the (fp32) bytes.                                 */
+long long odtk_preprocess_resize_u8_f32(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                        const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w, void *y,
+                                        const float *mean, const float *std, odtk_stream_t stream);
 
 /* ---- baseline JPEG decode (the Image.open(path).convert("RGB") of odtk/data.py:50, on the GPU) ------------------
  * One image of odtk_decode_jpeg: a baseline sequential Huffman-coded 8-bit JPEG (SOF0 / SOF1), grayscale or YCbCr

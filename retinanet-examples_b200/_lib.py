@@ -55,6 +55,14 @@ SIGNATURES = {
     "odtk_conv2d_s8_ex": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     "odtk_relu_copy_rows_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int] +
                                [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
+    "odtk_conv2d_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_pad_input_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "odtk_preprocess_u8_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [_c_f32p, _c_f32p, ctypes.c_void_p]),
+    "odtk_preprocess_resize_u8_f32": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p] +
+                                      [ctypes.c_int] * 3 + [ctypes.c_void_p, _c_f32p, _c_f32p, ctypes.c_void_p]),
+    "odtk_maxpool3x3s2_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 4 + [ctypes.c_void_p]),
+    "odtk_relu_copy_rows_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int] +
+                                [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     "odtk_quantize_f16_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_longlong, ctypes.c_float, ctypes.c_void_p]),
     "odtk_conv_last_plan": (ctypes.c_int, [ctypes.c_void_p]),
     "odtk_conv_map_cache_stats": (ctypes.c_int, [ctypes.POINTER(ctypes.c_longlong), ctypes.POINTER(ctypes.c_longlong)]),

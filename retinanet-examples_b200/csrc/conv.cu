@@ -27,6 +27,11 @@
 // Only Cin % 64 != 0 callers (RGB stems other than the 7x7) are first lowered to GEMM rows by layers.cu and run as mode 0.
 // INT8 (odtk_conv2d_s8 / _ex): the same kernel instantiated on s8 operands -- 128-channel K blocks, wgmma m64nNk32 with s32
 // accumulators, a dequantising epilogue (+ s8 residual / upsample addends) -- in modes 0, 1 (incl. s2) and 3.
+// FP32 (odtk_conv2d_f32): instantiated on fp32 operands with split-TF32 ("3xTF32") products -- 32-channel K blocks (one
+// 128-byte swizzle row), weights as two tf32-valued halves (w_hi, w_lo) that both stream through every stage; each consumer
+// warpgroup splits its own 64 A rows in shared memory (hi rounded in place, lo into a side buffer) and issues three wgmma
+// m64nNk8 tf32 MMAs per k8 step, a_hi*b_lo + a_lo*b_hi + a_hi*b_hi, into fp32 accumulators; fp32 NHWC epilogue (+ fp32
+// residual / upsample addends) -- in modes 0, 1 (incl. s2 and tile tables), 2 (stem over an NHWC4 fp32 image) and 3.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <math.h>
@@ -49,6 +54,22 @@ constexpr int kThreads = 384;
 constexpr int kMaxStages = 8;
 constexpr int kPipeBytes = 192 * 1024;   // 6 stages at BN = 128 (32 KB each), 8 at BN = 64
 constexpr int kSmemBytes = kPipeBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+// FP32 instances: after the stages, the A_lo side buffers, 2 per consumer warpgroup (64 rows x 128 B each, double-buffered:
+// the previous K block's MMAs may still read one while the next block is split into the other)
+constexpr int kLoBytes = 64 * 128;
+constexpr int kSplitBytes = 2 * 2 * kLoBytes;
+constexpr int kSmemBytesF32 = kPipeBytes + kSplitBytes + 1024 + 256;
+static_assert(kSmemBytesF32 <= 227 * 1024, "fp32 instance exceeds the opt-in shared memory");
+
+// operand types of conv_gemm_kernel
+enum ConvOp { kOpF16 = 0, kOpS8 = 1, kOpTF32x3 = 2 };
+
+// round to the nearest tf32 value, ties away from zero (low 13 bits cleared)
+__device__ __forceinline__ float tf32_rna(float x) {
+  uint32_t r;
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+  return __uint_as_float(r);
+}
 
 struct Barriers {
   uint64_t full[kMaxStages];
@@ -57,18 +78,22 @@ struct Barriers {
 static_assert(sizeof(Barriers) <= 256, "barrier block too small");
 
 // ---------------------------------------------------------------------------------- kernel
-// S8: int8 operands (odtk_conv2d_s8).  A K block is then one 128-byte swizzle row of 128 channels instead of 64, the MMAs
-// are the integer m64nNk32 form with exact s32 accumulators, and the epilogue dequantises with fmaf(acc, alpha, bias).
-template <int BN, bool S8>
+// OP kOpS8: int8 operands (odtk_conv2d_s8).  A K block is then one 128-byte swizzle row of 128 channels instead of 64, the
+// MMAs are the integer m64nNk32 form with exact s32 accumulators, and the epilogue dequantises with fmaf(acc, alpha, bias).
+// OP kOpTF32x3: fp32 operands (odtk_conv2d_f32).  A K block is one 128-byte row of 32 channels; a stage holds A, then
+// B_hi and B_lo (tmB / tmB2); the MMAs are three m64nNk8 tf32 products per k8 step (see the file comment).
+template <int BN, int OP>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
                  const __grid_constant__ ConvParams p) {
+  constexpr bool S8 = OP == kOpS8, F32 = OP == kOpTF32x3;
+  constexpr int BR = F32 ? 2 * BN : BN;   // B rows per stage: fp32 carries w_hi and w_lo
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  Barriers *bars = reinterpret_cast<Barriers *>(smem + kPipeBytes);
+  Barriers *bars = reinterpret_cast<Barriers *>(smem + kPipeBytes + (F32 ? kSplitBytes : 0));
   const int kStages = p.nstages, rb = p.row_bytes;
-  const int stage_bytes = (128 + BN) * rb;
+  const int stage_bytes = (128 + BR) * rb;
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0), tid = threadIdx.x & 127;
 
   if (threadIdx.x == 0) {
@@ -101,17 +126,17 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (wg == 0) {
     // ===================================== TMA producer =====================================
     if (tid != 0) return;
-    const uint32_t a_bytes = (uint32_t)((p.mode == 0 ? 128 : p.TH * p.TW) * rb), b_bytes = (uint32_t)(BN * rb);
-    const int kelems = S8 ? rb : rb >> 1;   // K elements per block: 64 (SW128) or 32 (SW64); s8: 128
+    const uint32_t a_bytes = (uint32_t)((p.mode == 0 ? 128 : p.TH * p.TW) * rb), b_bytes = (uint32_t)(BR * rb);
+    const int kelems = S8 ? rb : F32 ? rb >> 2 : rb >> 1;   // K elements per block: 64 (SW128) or 32 (SW64); s8: 128; fp32: 32
     int stage = 0;
     uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       int m_tile, n_tile, img, h0, w0, hlim, wlim;
       tile_origin(tile, m_tile, n_tile, img, h0, w0, hlim, wlim);
       const int n0 = n_tile * BN;
-      // K order: 64-channel (s8: 128-channel) chunk outer, tap inner
+      // K order: 64-channel (s8: 128-channel, fp32: 32-channel) chunk outer, tap inner
       for (int kb = 0; kb < p.kblocks_per_tap; kb++) {
-        const int kch = p.grouped ? n0 : kb * (S8 ? 128 : 64);   // input-channel coordinate: grouped convs read their own chunk only
+        const int kch = p.grouped ? n0 : kb * (S8 ? 128 : F32 ? 32 : 64);   // input-channel coordinate: grouped convs read their own chunk only
         for (int tap = 0; tap < p.taps; tap++) {
           const int dy = tap / p.kw - p.pad, dx = tap % p.kw - p.pad;
           mbar_wait(&bars->empty[stage], phase ^ 1u);
@@ -130,6 +155,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             tma_load_5d(sa, &tmA, &bars->full[stage], 0, w0, tap, h0, img);   // stem: filter row `tap`
           }
           tma_load_2d(sb, &tmB, &bars->full[stage], (tap * p.kblocks_per_tap + kb) * kelems, n0);
+          if constexpr (F32) tma_load_2d(sb + BN * rb, &tmB2, &bars->full[stage], (tap * p.kblocks_per_tap + kb) * kelems, n0);
           if (++stage == kStages) { stage = 0; phase ^= 1u; }
         }
       }
@@ -162,16 +188,47 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int brb = kb < kb_main ? rb : 128;
       const uint32_t sa = smem_u32(smem + stage * stage_bytes);
       const uint64_t da = wgmma_desc(sa + (uint32_t)(cw * 64 * brb), brb), db = wgmma_desc(sa + (uint32_t)(128 * brb), brb);
-      wgmma_fence();
-      if constexpr (S8) {
+      if constexpr (F32) {
+        // split this warpgroup's 64 A rows: hi = rna_tf32(a) in place, lo = rna_tf32(a - hi) (a - hi is exact) into the side
+        // buffer of this K block's parity.  Elementwise, so the swizzle does not matter: 16 bytes per thread and pass.
+        unsigned char *a_own = smem + stage * stage_bytes + cw * 64 * 128;
+        unsigned char *a_lo = smem + kPipeBytes + (2 * cw + (kb & 1)) * kLoBytes;
 #pragma unroll
-        for (int k = 0; k < 4; k++) WgmmaS8<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
-      } else if (brb == 128) {
+        for (int i = 0; i < kLoBytes / (128 * 16); i++) {
+          const int off = (tid + 128 * i) * 16;
+          float4 v = *reinterpret_cast<const float4 *>(a_own + off), lo;
+          float *vv = reinterpret_cast<float *>(&v), *ll = reinterpret_cast<float *>(&lo);
 #pragma unroll
-        for (int k = 0; k < 4; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+          for (int e = 0; e < 4; e++) {
+            const float hi = tf32_rna(vv[e]);
+            ll[e] = tf32_rna(vv[e] - hi);
+            vv[e] = hi;
+          }
+          *reinterpret_cast<float4 *>(a_own + off) = v;
+          *reinterpret_cast<float4 *>(a_lo + off) = lo;
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> async-proxy wgmma reads
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+        const uint64_t dlo = wgmma_desc(smem_u32(a_lo), 128), dbl = db + (uint64_t)((BN * 128) >> 4);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; k++) {   // small terms first
+          WgmmaTF32<BN>::mma(acc, da + (uint64_t)(2 * k), dbl + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+          WgmmaTF32<BN>::mma(acc, dlo + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+          WgmmaTF32<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), 1);
+        }
       } else {
+        wgmma_fence();
+        if constexpr (S8) {
 #pragma unroll
-        for (int k = 0; k < 2; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+          for (int k = 0; k < 4; k++) WgmmaS8<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+        } else if (brb == 128) {
+#pragma unroll
+          for (int k = 0; k < 4; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+        } else {
+#pragma unroll
+          for (int k = 0; k < 2; k++) Wgmma<BN>::mma(acc, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) ? 1 : 0);
+        }
       }
       wgmma_commit();
       // the previous K block's MMAs have finished reading their stage once at most one group is in flight
@@ -238,7 +295,29 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           continue;
         }
       }
-      if (!S8 && p.out_mode == ODTK_OUT_NHWC_F16) {
+      if constexpr (F32) {
+        if (p.out_mode == ODTK_OUT_NHWC_F32) {
+          // fp32 activations: + bias, + residual, + upsample (fp32 adds in this order), ReLU
+          if (!valid) continue;
+          const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
+          float *o = reinterpret_cast<float *>(p.out) + opix * p.ldy;
+          const float *res = p.res32 ? p.res32 + m * p.ldr : nullptr;
+          const float *up = p.up32 ? p.up32 + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
+#pragma unroll
+          for (int j = 0; j < BN / 8; j++) {
+            const int col = n0 + 8 * j + 2 * q;
+            if (col >= p.Cout) continue;   // Cout even: both columns of the pair are in range or neither
+            float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+            if (p.bias) { v0 += __ldg(p.bias + col); v1 += __ldg(p.bias + col + 1); }
+            if (res) { const float2 r = *reinterpret_cast<const float2 *>(res + col); v0 += r.x; v1 += r.y; }
+            if (up) { const float2 u = *reinterpret_cast<const float2 *>(up + col); v0 += u.x; v1 += u.y; }
+            if (p.relu) { v0 = fmaxf(v0, 0.0f); v1 = fmaxf(v1, 0.0f); }
+            *reinterpret_cast<float2 *>(o + col) = make_float2(v0, v1);
+          }
+          continue;
+        }
+      }
+      if (OP == kOpF16 && p.out_mode == ODTK_OUT_NHWC_F16) {
         if (!valid) continue;
         const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
         __half *o = reinterpret_cast<__half *>(p.out) + opix * p.ldy;
@@ -405,20 +484,20 @@ void choose_patch(int H, int W, int &TH, int &TW) {
 
 namespace {
 
-template <int BN, bool S8>
+template <int BN, int OP>
 void launch_bn(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
                const CUtensorMap &tmB2, const ConvParams &p) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
+  cfg.dynamicSmemBytes = OP == kOpTF32x3 ? kSmemBytesF32 : kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = odtk_pdl_on() ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, S8>, tmA, tmB, tmA2, tmB2, p);
+  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, OP>, tmA, tmB, tmA2, tmB2, p);
 }
 
 // Per-device state (one process may drive several GPUs): the > 48 KB dynamic-shared-memory opt-in of every kernel
@@ -432,10 +511,12 @@ bool device_ready() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return false;
   std::lock_guard<std::mutex> lk(g_dev_mu);
   if (g_dev_ready[dev]) return true;
-  if (cudaFuncSetAttribute(conv_gemm_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
+  if (cudaFuncSetAttribute(conv_gemm_kernel<64, kOpF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<64, kOpS8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpS8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<64, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess)
     return false;
   g_dev_ready[dev] = true;
   return true;
@@ -443,25 +524,28 @@ bool device_ready() {
 
 thread_local odtk_conv_plan_t g_last_plan;
 
-void set_stages(ConvParams &p, int BN) {
-  p.nstages = kPipeBytes / ((128 + BN) * p.row_bytes);
+void set_stages(ConvParams &p, int BN, int op = kOpF16) {
+  p.nstages = kPipeBytes / ((128 + (op == kOpTF32x3 ? 2 * BN : BN)) * p.row_bytes);
   if (p.nstages > kMaxStages) p.nstages = kMaxStages;
 }
 
 int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
-           const CUtensorMap &tmB2, cudaStream_t stream, bool s8 = false) {
+           const CUtensorMap &tmB2, cudaStream_t stream, int op = kOpF16) {
   const int total = p.num_m_tiles * p.num_n_tiles;
   const int sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
   const int grid = total < sms ? total : sms;
   g_last_plan = odtk_conv_plan_t{p.mode, 0, BN, p.num_m_tiles, p.num_n_tiles, p.nstages, 0, 0, 0, 0, 0, 0, p.TH, p.TW, grid, 0};
   {
     OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    if (s8) {
-      if (BN == 64) launch_bn<64, true>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-      else          launch_bn<128, true>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    if (op == kOpS8) {
+      if (BN == 64) launch_bn<64, kOpS8>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      else          launch_bn<128, kOpS8>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    } else if (op == kOpTF32x3) {
+      if (BN == 64) launch_bn<64, kOpTF32x3>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      else          launch_bn<128, kOpTF32x3>(grid, stream, tmA, tmB, tmA2, tmB2, p);
     } else {
-      if (BN == 64) launch_bn<64, false>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-      else          launch_bn<128, false>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      if (BN == 64) launch_bn<64, kOpF16>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      else          launch_bn<128, kOpF16>(grid, stream, tmA, tmB, tmA2, tmB2, p);
     }
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
@@ -480,11 +564,12 @@ int set_sink(ConvParams &p, const odtk_cand_sink_t *k, int cout, int h, int widt
 }
 
 // A operand of a 1x1 / 3x3, stride 1 / 2 launch: the mode, the output patch and tile grid, and the tensor map of x (the
-// top-left h x width rectangle of images xH x xW pixels apart).  es: bytes per element, 2 (fp16) or 1 (s8); a K block is
-// one 128-byte swizzle row of channels either way.  Shared by odtk_conv2d and odtk_conv2d_s8_ex.
+// top-left h x width rectangle of images xH x xW pixels apart).  es: bytes per element, 2 (fp16), 1 (s8) or 4 (fp32); a K
+// block is one 128-byte swizzle row of channels either way.  Shared by odtk_conv2d, odtk_conv2d_s8_ex and odtk_conv2d_f32.
 int a_operand(ConvParams &p, CUtensorMap &tmA, const void *x, int n, int h, int width, int cin, int ksize, int stride,
               uint64_t xH, uint64_t xW, bool x_view, const void *tile_tab, int tab_tiles, bool upsample, int es) {
-  const CUtensorMapDataType dt = es == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = es == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                : es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const uint32_t kc = 128 / es;   // channels per K block
   const uint64_t C = (uint64_t)cin, W = (uint64_t)width, H = (uint64_t)h;
   if (stride == 2 && ((h & 1) || (width & 1) || x_view)) {
@@ -718,7 +803,107 @@ int conv_run_s8(const odtk_conv_s8_ex_t *e, cudaStream_t stream) {
     uint32_t box[2] = {128, (uint32_t)BN};
     if (!encode_map(&tmB, d->w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
   }
-  return launch(p, BN, tmA, tmB, tmA, tmB, stream, true);
+  return launch(p, BN, tmA, tmB, tmA, tmB, stream, kOpS8);
+}
+
+// odtk_conv2d_f32: the kernel on fp32 operands (split TF32).  1x1 / 3x3 with the geometry of odtk_conv2d (dense, atlas views,
+// tile tables, stride 2 on either view), plus ksize 7 / stride 2 / cin 3: the ResNet stem over the NHWC4 fp32 image
+// [n, h+6, width+8, 4] (mode 2, any h and width).  NHWC fp32 outputs may add an fp32 residual and / or upsample addend and
+// may land in a level view of an fp32 atlas.
+int conv_run_f32(const odtk_conv_f32_t *d, cudaStream_t stream) {
+  if (!d || !d->x || !d->w_hi || !d->w_lo) return ODTK_E_INVALID;
+  if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
+  if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
+  if (d->out_mode != ODTK_OUT_NHWC_F32 && d->out_mode != ODTK_OUT_NCHW_F32 && d->out_mode != ODTK_OUT_NCHW_F32_SIGMOID &&
+      d->out_mode != ODTK_OUT_CANDIDATES)
+    return ODTK_E_INVALID;
+  const int stride = d->stride > 1 ? d->stride : 1;
+  const bool stem = d->ksize == 7;
+  if (stem ? (d->cin != 3 || stride != 2) : ((d->ksize != 1 && d->ksize != 3) || d->cin % 32)) return ODTK_E_UNSUPPORTED;
+  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
+  if (d->relu != 0 && d->relu != 1) return ODTK_E_UNSUPPORTED;
+  if (d->out_mode == ODTK_OUT_NHWC_F32 && (d->cout % 2)) return ODTK_E_UNSUPPORTED;   // float2 stores
+  if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  if (((uintptr_t)d->x | (uintptr_t)d->w_hi | (uintptr_t)d->w_lo | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15)
+    return ODTK_E_INVALID;
+  const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
+  const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
+  const bool y_view = d->y_rows > 0 || d->y_width > 0 || d->y_row_off > 0;
+  const bool addend = d->residual || d->upsample;
+  // as odtk_conv2d_s8_ex: addends and output views need NHWC fp32, views and tile tables are 3x3 without addends
+  if ((addend || y_view) && d->out_mode != ODTK_OUT_NHWC_F32) return ODTK_E_UNSUPPORTED;
+  if ((x_view || y_view || d->tile_tab) && (d->ksize != 3 || addend)) return ODTK_E_UNSUPPORTED;
+  if (stem && addend) return ODTK_E_UNSUPPORTED;
+  if (d->upsample && stride != 1) return ODTK_E_UNSUPPORTED;
+  if (d->tile_tab && (d->tab_tiles <= 0 || x_view || y_view || stride != 1)) return ODTK_E_INVALID;
+  if ((((uintptr_t)d->residual | (uintptr_t)d->upsample) & 7) || (d->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
+  if (!device_ready()) return ODTK_E_CUDA;
+  const int sms = odtk_sm_count();
+  ConvParams p;
+  memset(&p, 0, sizeof p);
+  p.N = d->n; p.H = d->h; p.W = d->width; p.Cin = d->cin; p.Cout = d->cout;
+  p.row_bytes = 128;
+  p.M = (long long)d->n * d->h * d->width;
+  p.bias = d->bias;
+  p.out = d->y;
+  p.relu = d->relu;
+  p.out_mode = d->out_mode;
+  p.ldy = d->ldy > 0 ? d->ldy : d->cout;
+  p.ldr = d->ldr > 0 ? d->ldr : d->cout;
+  p.res32 = (const float *)d->residual;
+  p.up32 = (const float *)d->upsample;
+  p.up_h = d->h / 2; p.up_w = d->width / 2;
+  if ((p.out_mode == ODTK_OUT_NHWC_F32 && (p.ldy & 1)) || (p.res32 && (p.ldr & 1))) return ODTK_E_INVALID;   // float2 accesses
+  if (p.out_mode == ODTK_OUT_CANDIDATES) {
+    const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
+    if (rc != ODTK_OK) return rc;
+  }
+  CUtensorMap tmA, tmB, tmB2;
+  uint64_t K;
+  if (stem) {
+    // NHWC4 window rows as in odtk_stem_conv, in fp32: 8 pixels x 4 channels = 32 floats = one 128-byte swizzle row
+    const int OH = (d->h - 1) / 2 + 1, OW = (d->width - 1) / 2 + 1;
+    const uint64_t HP = (uint64_t)d->h + 6, WP = (uint64_t)d->width + 8;
+    p.mode = 2;
+    p.H = OH; p.W = OW; p.Cin = 4;
+    p.kw = 1; p.taps = 7; p.pad = 0; p.kblocks_per_tap = 1;
+    p.M = (long long)d->n * OH * OW;
+    choose_patch(OH, OW, p.TH, p.TW);
+    p.tiles_h = (OH + p.TH - 1) / p.TH;
+    p.tiles_w = (OW + p.TW - 1) / p.TW;
+    p.num_m_tiles = d->n * p.tiles_h * p.tiles_w;
+    uint64_t dims[5] = {32, (uint64_t)OW, 7, (uint64_t)OH, (uint64_t)d->n};
+    uint64_t str[4] = {32, WP * 16, WP * 32, HP * WP * 16};
+    uint32_t box[5] = {32, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
+    if (!encode_map(&tmA, d->x, 5, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32))
+      return ODTK_E_UNSUPPORTED;
+    K = 224;
+  } else {
+    p.kw = d->ksize; p.taps = d->ksize * d->ksize; p.pad = d->ksize / 2;
+    p.kblocks_per_tap = d->cin / 32;
+    const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
+                             d->tab_tiles, d->upsample != nullptr, 4);
+    if (rc != ODTK_OK) return rc;
+    K = (uint64_t)p.taps * d->cin;
+  }
+  p.oH = d->y_rows > 0 ? d->y_rows : p.H;
+  p.oR = d->y_row_off > 0 ? d->y_row_off : 0;
+  p.oW = d->y_width > 0 ? d->y_width : p.W;
+  if ((long long)d->n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
+  // N tile as for odtk_conv2d
+  int BN = d->cout <= 64 ? 64 : 128;
+  if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
+  p.num_n_tiles = (d->cout + BN - 1) / BN;
+  set_stages(p, BN, kOpTF32x3);
+  {
+    uint64_t dims[2] = {K, (uint64_t)d->cout};
+    uint64_t str[1] = {K * 4};
+    uint32_t box[2] = {32, (uint32_t)BN};
+    if (!encode_map(&tmB, d->w_hi, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32) ||
+        !encode_map(&tmB2, d->w_lo, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32))
+      return ODTK_E_CUDA;
+  }
+  return launch(p, BN, tmA, tmB, tmA, tmB2, stream, kOpTF32x3);
 }
 
 // bias operand: [cout, 64] fp16 with (hi, lo, 0, ...): hi + lo == bias to 2^-22 relative
@@ -751,6 +936,10 @@ extern "C" int odtk_conv2d_s8(const odtk_conv_s8_t *d, odtk_stream_t stream_) {
 
 extern "C" int odtk_conv2d_s8_ex(const odtk_conv_s8_ex_t *e, odtk_stream_t stream_) {
   return conv_run_s8(e, (cudaStream_t)stream_);
+}
+
+extern "C" int odtk_conv2d_f32(const odtk_conv_f32_t *d, odtk_stream_t stream_) {
+  return conv_run_f32(d, (cudaStream_t)stream_);
 }
 
 // ResNet stem: 7x7 stride-2 pad-3 convolution of the RGB image, im2col-free.  `xp` is the image

@@ -51,4 +51,7 @@ struct ConvParams {
   // pixel, upsample [N, up_h, up_w, Cout] at (h >> 1, w >> 1); NULL when absent
   const int8_t *res8, *up8;
   float res_scale, up_scale;
+  // fp32 addends of ODTK_OUT_NHWC_F32 (odtk_conv2d_f32): residual [M, ldr] at the output pixel, upsample
+  // [N, up_h, up_w, Cout] at (h >> 1, w >> 1); NULL when absent
+  const float *res32, *up32;
 };

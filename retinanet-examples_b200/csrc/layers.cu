@@ -6,6 +6,8 @@
 // Reference call sites: odtk/backbones/resnet.py:25-28, odtk/backbones/fpn.py:54-55.
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "prof.cuh"
 
@@ -150,14 +152,23 @@ __global__ void pad_input_rows_kernel(const __half *__restrict__ x, __half *__re
   }
 }
 
-// One RGB pixel of odtk infer's input normalisation (reference odtk/data.py:118-121) as the stem's 8-byte NHWC4 pixel:
-// same operation order as the reference: float(u8) / 255, then - mean, then / std, fp32, one fp16 rounding.
+// One channel of odtk infer's input normalisation (reference odtk/data.py:118-121), same operation order as the
+// reference: float(u8) / 255, then - mean, then / std, fp32.
+__device__ __forceinline__ float normalize_u8(unsigned v, float m, float s) { return ((float)v / 255.0f - m) / s; }
+
+// One RGB pixel of it as the stem's 8-byte NHWC4 pixel: one fp16 rounding.
 __device__ __forceinline__ uint2 normalize_rgb_u8(unsigned r8, unsigned g8, unsigned b8, float m0, float m1, float m2,
                                                   float s0, float s1, float s2) {
-  float r = ((float)r8 / 255.0f - m0) / s0, g = ((float)g8 / 255.0f - m1) / s1, b = ((float)b8 / 255.0f - m2) / s2;
+  float r = normalize_u8(r8, m0, s0), g = normalize_u8(g8, m1, s1), b = normalize_u8(b8, m2, s2);
   __half2 rg = __floats2half2_rn(r, g);
   __half2 bz = __floats2half2_rn(b, 0.0f);
   return make_uint2(*reinterpret_cast<unsigned *>(&rg), *reinterpret_cast<unsigned *>(&bz));
+}
+
+// The same pixel as the 16-byte fp32 NHWC4 pixel of the full-precision stem (no rounding after the fp32 arithmetic).
+__device__ __forceinline__ float4 normalize_rgb_u8_f32(unsigned r8, unsigned g8, unsigned b8, float m0, float m1, float m2,
+                                                       float s0, float s1, float s2) {
+  return make_float4(normalize_u8(r8, m0, s0), normalize_u8(g8, m1, s1), normalize_u8(b8, m2, s2), 0.0f);
 }
 
 // Input side of odtk infer (reference odtk/data.py:113-123): uint8 HWC image -> /255 -> (x - mean) / std
@@ -244,12 +255,16 @@ __device__ __forceinline__ unsigned resample_clip8(int acc) { return (unsigned)m
 // for once, hence the tall tile.
 __device__ __forceinline__ int resample_acc_init() { return 1 << (RS_BITS - 1); }
 
+// F32: the full-precision stem buffer, 16-byte fp32 NHWC4 pixels (normalize_rgb_u8_f32) instead of 8-byte fp16 ones.
+template <bool F32>
 __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kernel(
-    const unsigned char *__restrict__ x, const odtk_resize_image_t *__restrict__ tab, __half *__restrict__ y, int HS, int WS,
+    const unsigned char *__restrict__ x, const odtk_resize_image_t *__restrict__ tab,
+    typename std::conditional<F32, float4, uint2>::type *__restrict__ y, int HS, int WS,
     float m0, float m1, float m2, float s0, float s1, float s2) {
+  using Pix = typename std::conditional<F32, float4, uint2>::type;
   __shared__ int s_wx[RS_KMAX][RS_TW], s_wy[RS_TH][RS_KMAX];     // column taps tap-major: lanes read consecutive words
   __shared__ int s_lox[RS_TW], s_nx[RS_TW], s_loy[RS_TH], s_ny[RS_TH];
-  __shared__ uint2 s_norm[256];   // normalize_rgb_u8(v, v, v): channel c of a pixel is its value's channel c
+  __shared__ Pix s_norm[256];   // normalize_rgb_u8(v, v, v): channel c of a pixel is its value's channel c
   const int HP = HS + 6, WP = WS + 8;
   const int n = blockIdx.z;
   const odtk_resize_image_t im = tab[n];
@@ -259,7 +274,10 @@ __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kerne
   const bool meets = x0 + RS_TW > 0 && x0 < im.dst_w && y0 + RS_TH > 0 && y0 < im.dst_h;                       // block-uniform
   const bool tables = meets && resample_ksize(im.src_w, im.dst_w) <= RS_KMAX && resample_ksize(im.src_h, im.dst_h) <= RS_KMAX;
   if (meets) {
-    for (int v = threadIdx.x; v < 256; v += RS_TW * RS_ROWS) s_norm[v] = normalize_rgb_u8(v, v, v, m0, m1, m2, s0, s1, s2);
+    for (int v = threadIdx.x; v < 256; v += RS_TW * RS_ROWS) {
+      if constexpr (F32) s_norm[v] = normalize_rgb_u8_f32(v, v, v, m0, m1, m2, s0, s1, s2);
+      else s_norm[v] = normalize_rgb_u8(v, v, v, m0, m1, m2, s0, s1, s2);
+    }
     if (!tables) __syncthreads();
   }
   if (tables && threadIdx.x >= RS_TW + RS_TH) {
@@ -306,7 +324,9 @@ __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kerne
   for (int r = ty; r < RS_TH; r += RS_ROWS) {
     const int oy = y0 + r, yp = oy + 3;
     if (yp >= HP) break;
-    uint2 v = make_uint2(0u, 0u);
+    Pix v;
+    if constexpr (F32) v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    else v = make_uint2(0u, 0u);
     if (meets && ox >= 0 && ox < im.dst_w && oy >= 0 && oy < im.dst_h) {
       int acc[3] = {resample_acc_init(), resample_acc_init(), resample_acc_init()};
       if (tables) {
@@ -340,10 +360,13 @@ __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kerne
         }
       }
       // the normalisation is per channel: take r from the red value's entry, g from the green one's, b from the blue one's
-      v = make_uint2(__byte_perm(s_norm[resample_clip8(acc[0])].x, s_norm[resample_clip8(acc[1])].x, 0x7610),
-                     s_norm[resample_clip8(acc[2])].y);
+      if constexpr (F32)
+        v = make_float4(s_norm[resample_clip8(acc[0])].x, s_norm[resample_clip8(acc[1])].y, s_norm[resample_clip8(acc[2])].z, 0.0f);
+      else
+        v = make_uint2(__byte_perm(s_norm[resample_clip8(acc[0])].x, s_norm[resample_clip8(acc[1])].x, 0x7610),
+                       s_norm[resample_clip8(acc[2])].y);
     }
-    if (xp < WP) reinterpret_cast<uint2 *>(y)[((long long)n * HP + yp) * WP + xp] = v;
+    if (xp < WP) y[((long long)n * HP + yp) * WP + xp] = v;
   }
 }
 
@@ -412,6 +435,89 @@ __global__ void relu_copy_rows_s8_kernel(const int8_t *__restrict__ x, int8_t *_
   }
 }
 
+// ---- fp32 twins (full-precision mode, odtk_conv2d_f32) ----
+// RGB NHWC3 fp32 -> zero-padded NHWC4 fp32 [n, h+6, w+8, 4], the border of pad_input_kernel.  One 16-byte pixel per thread.
+__global__ void pad_input_f32_kernel(const float *__restrict__ x, float4 *__restrict__ y, int N, int H, int W) {
+  const int HP = H + 6, WP = W + 8;
+  const long long total = (long long)N * HP * WP;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int xp = (int)(i % WP);
+    long long t = i / WP;
+    int yp = (int)(t % HP);
+    int n = (int)(t / HP);
+    int ih = yp - 3, iw = xp - 3;
+    float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
+      const float *s = x + (((long long)n * H + ih) * W + iw) * 3;
+      v = make_float4(__ldg(s), __ldg(s + 1), __ldg(s + 2), 0.0f);
+    }
+    y[i] = v;
+  }
+}
+
+// preprocess_u8_kernel into the fp32 NHWC4 stem buffer
+__global__ void preprocess_u8_f32_kernel(const unsigned char *__restrict__ x, float4 *__restrict__ y, int N, int H, int W,
+                                         int HS, int WS, float m0, float m1, float m2, float s0, float s1, float s2) {
+  const int HP = HS + 6, WP = WS + 8;
+  const long long total = (long long)N * HP * WP;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int xp = (int)(i % WP);
+    long long t = i / WP;
+    int yp = (int)(t % HP);
+    int n = (int)(t / HP);
+    int ih = yp - 3, iw = xp - 3;
+    float4 v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+    if (ih >= 0 && ih < H && iw >= 0 && iw < W) {
+      const unsigned char *s = x + (((long long)n * H + ih) * W + iw) * 3;
+      v = normalize_rgb_u8_f32(s[0], s[1], s[2], m0, m1, m2, s0, s1, s2);
+    }
+    y[i] = v;
+  }
+}
+
+// 3x3 stride-2 pad-1 max-pool on NHWC fp32, 4 channels (16 bytes) per thread
+__global__ void maxpool3x3s2_f32_kernel(const float *__restrict__ x, float *__restrict__ y, int N, int H, int W, int C,
+                                        int OH, int OW) {
+  const int c4n = C >> 2;
+  const long long total = (long long)N * OH * OW * c4n;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    int c4 = (int)(i % c4n);
+    long long m = i / c4n;
+    int ow = (int)(m % OW);
+    long long t = m / OW;
+    int oh = (int)(t % OH);
+    int n = (int)(t / OH);
+    float4 best = make_float4(-INFINITY, -INFINITY, -INFINITY, -INFINITY);
+#pragma unroll
+    for (int dy = 0; dy < 3; dy++) {
+      int ih = oh * 2 + dy - 1;
+      if (ih < 0 || ih >= H) continue;
+#pragma unroll
+      for (int dx = 0; dx < 3; dx++) {
+        int iw = ow * 2 + dx - 1;
+        if (iw < 0 || iw >= W) continue;
+        const float4 v = __ldg(reinterpret_cast<const float4 *>(x + (((long long)n * H + ih) * W + iw) * C) + c4);
+        best.x = fmaxf(best.x, v.x); best.y = fmaxf(best.y, v.y); best.z = fmaxf(best.z, v.z); best.w = fmaxf(best.w, v.w);
+      }
+    }
+    reinterpret_cast<float4 *>(y + m * C)[c4] = best;
+  }
+}
+
+// 3-D strided copy of fp32 rows with ReLU, 16 bytes per thread (pyramid7's input ReLU(P6) from the fp32 atlas)
+__global__ void relu_copy_rows_f32_kernel(const float *__restrict__ x, float *__restrict__ y, int n, int rows, int row4,
+                                          long long x_img, long long x_row, long long y_img, long long y_row) {
+  const long long total = (long long)n * rows * row4;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % row4);
+    const long long t = i / row4;
+    const int r = (int)(t % rows), im = (int)(t / rows);
+    float4 v = __ldg(reinterpret_cast<const float4 *>(x + im * x_img + r * x_row) + c);
+    v.x = fmaxf(v.x, 0.0f); v.y = fmaxf(v.y, 0.0f); v.z = fmaxf(v.z, 0.0f); v.w = fmaxf(v.w, 0.0f);
+    reinterpret_cast<float4 *>(y + im * y_img + r * y_row)[c] = v;
+  }
+}
+
 inline int grid_for(long long total, int threads) {
   long long b = (total + threads - 1) / threads;
   long long cap = (long long)odtk_sm_count() * 16;
@@ -472,9 +578,10 @@ extern "C" int odtk_preprocess_u8(const void *x, void *y, int n, int h, int w, i
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 
-extern "C" long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
-                                               const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w,
-                                               void *y, const float *mean, const float *std, odtk_stream_t stream_) {
+namespace {
+template <bool F32>
+long long preprocess_resize(const void *x, size_t x_bytes, const odtk_resize_image_t *images, const odtk_resize_image_t *images_dev,
+                            int n, int canvas_h, int canvas_w, void *y, const float *mean, const float *std, odtk_stream_t stream_) {
   if (!images || n <= 0 || n > 65535 || canvas_h <= 0 || canvas_w <= 0 || (canvas_h % 2) || (canvas_w % 2)) return ODTK_E_INVALID;
   for (int i = 0; i < n; i++) {
     const odtk_resize_image_t &im = images[i];
@@ -482,13 +589,65 @@ extern "C" long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, co
     if (im.dst_h > canvas_h || im.dst_w > canvas_w) return ODTK_E_INVALID;
     if (im.offset < 0 || (unsigned long long)im.offset + (unsigned long long)im.src_h * im.src_w * 3 > x_bytes) return ODTK_E_INVALID;
   }
-  const long long bytes = (long long)n * (canvas_h + 6) * (canvas_w + 8) * 8;
+  const long long bytes = (long long)n * (canvas_h + 6) * (canvas_w + 8) * (F32 ? 16 : 8);
   if (!y) return bytes;
   if (!x || !images_dev || !mean || !std) return ODTK_E_INVALID;
   const dim3 grid((canvas_w + 8 + RS_TW - 1) / RS_TW, (canvas_h + 6 + RS_TH - 1) / RS_TH, n);
   OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
-  preprocess_resize_u8_kernel<<<grid, RS_TW * RS_ROWS, 0, (cudaStream_t)stream_>>>(
-      (const unsigned char *)x, images_dev, (__half *)y, canvas_h, canvas_w, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
+  preprocess_resize_u8_kernel<F32><<<grid, RS_TW * RS_ROWS, 0, (cudaStream_t)stream_>>>(
+      (const unsigned char *)x, images_dev, (typename std::conditional<F32, float4, uint2>::type *)y, canvas_h, canvas_w,
+      mean[0], mean[1], mean[2], std[0], std[1], std[2]);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+}  // namespace
+
+extern "C" long long odtk_preprocess_resize_u8(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                               const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w,
+                                               void *y, const float *mean, const float *std, odtk_stream_t stream_) {
+  return preprocess_resize<false>(x, x_bytes, images, images_dev, n, canvas_h, canvas_w, y, mean, std, stream_);
+}
+
+extern "C" long long odtk_preprocess_resize_u8_f32(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                                   const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w,
+                                                   void *y, const float *mean, const float *std, odtk_stream_t stream_) {
+  return preprocess_resize<true>(x, x_bytes, images, images_dev, n, canvas_h, canvas_w, y, mean, std, stream_);
+}
+
+extern "C" int odtk_pad_input_f32(const void *x, void *y, int n, int h, int w, odtk_stream_t stream_) {
+  if (!x || !y || n <= 0 || h <= 0 || w <= 0 || ((uintptr_t)y & 15)) return ODTK_E_INVALID;
+  const long long total = (long long)n * (h + 6) * (w + 8);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  pad_input_f32_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream_>>>((const float *)x, (float4 *)y, n, h, w);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_preprocess_u8_f32(const void *x, void *y, int n, int h, int w, int hs, int ws, const float *mean,
+                                      const float *std, odtk_stream_t stream_) {
+  if (!x || !y || !mean || !std || n <= 0 || h <= 0 || w <= 0 || hs < h || ws < w || ((uintptr_t)y & 15)) return ODTK_E_INVALID;
+  const long long total = (long long)n * (hs + 6) * (ws + 8);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  preprocess_u8_f32_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream_>>>(
+      (const unsigned char *)x, (float4 *)y, n, h, w, hs, ws, mean[0], mean[1], mean[2], std[0], std[1], std[2]);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_maxpool3x3s2_f32(const void *x, void *y, int n, int h, int w, int c, odtk_stream_t stream_) {
+  if (!x || !y || n <= 0 || h <= 0 || w <= 0 || c <= 0 || (c % 4) || (((uintptr_t)x | (uintptr_t)y) & 15)) return ODTK_E_INVALID;
+  const int oh = (h - 1) / 2 + 1, ow = (w - 1) / 2 + 1;
+  const long long total = (long long)n * oh * ow * (c / 4);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  maxpool3x3s2_f32_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream_>>>((const float *)x, (float *)y, n, h, w, c, oh, ow);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_relu_copy_rows_f32(const void *x, void *y, int n, int rows, int row_elems, long long x_img_pitch,
+                                       long long x_row_pitch, long long y_img_pitch, long long y_row_pitch, odtk_stream_t stream_) {
+  if (!x || !y || n <= 0 || rows <= 0 || row_elems <= 0 || (row_elems % 4)) return ODTK_E_INVALID;
+  if ((x_img_pitch | x_row_pitch | y_img_pitch | y_row_pitch) % 4 || (((uintptr_t)x | (uintptr_t)y) & 15)) return ODTK_E_INVALID;
+  const long long total = (long long)n * rows * (row_elems / 4);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  relu_copy_rows_f32_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream_>>>((const float *)x, (float *)y, n, rows, row_elems / 4,
+                                                                                     x_img_pitch, x_row_pitch, y_img_pitch, y_row_pitch);
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 

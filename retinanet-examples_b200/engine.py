@@ -6,7 +6,7 @@ import torch
 
 from . import _lib
 
-OUT_NHWC_F16, OUT_NCHW_F32, OUT_NCHW_F32_SIGMOID, OUT_CANDIDATES, OUT_NHWC_S8 = 0, 1, 2, 3, 4
+OUT_NHWC_F16, OUT_NCHW_F32, OUT_NCHW_F32_SIGMOID, OUT_CANDIDATES, OUT_NHWC_S8, OUT_NHWC_F32 = 0, 1, 2, 3, 4, 5
 
 # host-side accounting of what was launched (bench.py reads it): kernels launched by this
 # module and algorithmic convolution FLOPs (2 * pixels * Cout * taps * Cin, unpadded)
@@ -48,6 +48,15 @@ class ConvS8ExDesc(ctypes.Structure):
     _fields_ = [("base", ConvS8Desc), ("stride", ctypes.c_int), ("residual", ctypes.c_void_p), ("res_scale", ctypes.c_float),
                 ("upsample", ctypes.c_void_p), ("up_scale", ctypes.c_float), ("y_rows", ctypes.c_int),
                 ("y_row_off", ctypes.c_int), ("y_width", ctypes.c_int)]
+
+
+class ConvF32Desc(ctypes.Structure):
+    """odtk_conv_f32_t (include/odtk_b200.h)."""
+    _fields_ = [("x", ctypes.c_void_p), ("w_hi", ctypes.c_void_p), ("w_lo", ctypes.c_void_p), ("bias", ctypes.c_void_p),
+                ("residual", ctypes.c_void_p), ("upsample", ctypes.c_void_p), ("y", ctypes.c_void_p)] + \
+               [(f, ctypes.c_int) for f in ("n", "h", "width", "cin", "cout", "ksize", "stride", "relu", "out_mode", "ldy", "ldr")] + \
+               [("sink", ctypes.c_void_p), ("x_rows", ctypes.c_int), ("x_width", ctypes.c_int), ("y_rows", ctypes.c_int),
+                ("y_row_off", ctypes.c_int), ("y_width", ctypes.c_int), ("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int)]
 
 
 def _stream():
@@ -447,13 +456,13 @@ def resize_bytes(plan):
     return plan.nbytes + ctypes.sizeof(plan.table) + plan.n * (hs + 6) * (ws + 8) * 8
 
 
-def preprocess_resize_u8(images, resize, max_size, stride=128, canvas=None, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+def preprocess_resize_u8(images, resize, max_size, stride=128, canvas=None, mean=IMAGENET_MEAN, std=IMAGENET_STD, f32=False):
     """Input side of `odtk infer` for a list of raw uint8 [h_i, w_i, 3] RGB images of any sizes (odtk/data.py:55-60,
     113-123, collate_fn :154-176): Pillow-exact BILINEAR resize by the reference's ratio, normalisation, stride and batch
     padding, written straight into the stem's zero-bordered NHWC4 fp16 buffer [n, hs+6, ws+8, 4] by one kernel.  CPU
     images are staged through pinned memory with one H2D copy; CUDA images are read in place.  `canvas` (hs, ws): a fixed
     batch canvas (multiples of `stride`); default the batch maximum of the stride-padded sizes.  Returns (xp, hs, ws,
-    ratios float32 [n])."""
+    ratios float32 [n]).  f32: the fp32 stem buffer of the full-precision mode (resize_launch_f32)."""
     plan = ResizePlan(image_shapes(images), resize, max_size, stride, canvas)
     dev = next((im.device for im in images if im.is_cuda), torch.device("cuda", torch.cuda.current_device()))
     if all(im.is_cuda and im.is_contiguous() for im in images):
@@ -467,7 +476,7 @@ def preprocess_resize_u8(images, resize, max_size, stride=128, canvas=None, mean
     else:
         table_dev, x_dev = stage_images(images, plan, torch.empty(table_pad(plan.n) + plan.nbytes, dtype=torch.uint8, device=dev))
         x_bytes = plan.nbytes
-    xp = resize_launch(x_dev, x_bytes, plan, table_dev, mean=mean, std=std)
+    xp = (resize_launch_f32 if f32 else resize_launch)(x_dev, x_bytes, plan, table_dev, mean=mean, std=std)
     return xp, plan.canvas[0], plan.canvas[1], plan.ratios
 
 
@@ -650,3 +659,178 @@ def pad_input(x):
 def stem_pool(x, w, bias, cout, relu=True):
     """NHWC fp16 RGB batch [N,H,W,3] -> zero-pad to NHWC4 (one small kernel) -> fused stem + max-pool."""
     return stem_pool_padded(pad_input(x), x.shape[1], x.shape[2], w, bias, cout, relu)
+
+
+# ---- full precision: fp32 activations, split-TF32 convolutions (odtk_conv2d_f32) ------------------------------------
+def tf32_rna(x):
+    """Round fp32 values to the nearest tf32 value, ties away from zero, as cvt.rna.tf32.f32 does: the low 13 bits of the
+    magnitude are rounded off (finite inputs)."""
+    b = x.float().contiguous().view(torch.int32)
+    return ((b + 0x1000) & ~0x1FFF).view(torch.float32)
+
+
+def pack_weight_tf32x2(weight, kpad=None):
+    """[Cout, Cin, kh, kw] fp32 -> (hi, lo): fp32 [Cout, kh*kw*Cin (zero padded to kpad)] in the K order of pack_weight,
+    hi = rna_tf32(w), lo = rna_tf32(w - hi), both tf32-valued (low 13 bits zero); |w - hi - lo| <= 2^-22 |w|."""
+    cout, cin, kh, kw = weight.shape
+    w = weight.float().permute(0, 2, 3, 1).reshape(cout, kh * kw * cin)
+    if kpad is not None and kpad > w.shape[1]:
+        w = torch.cat([w, w.new_zeros(cout, kpad - w.shape[1])], dim=1)
+    return split_tf32x2(w)
+
+
+def split_tf32x2(w):
+    """(hi, lo) = (rna_tf32(w), rna_tf32(w - hi)) of an fp32 tensor, contiguous."""
+    hi = tf32_rna(w)
+    return hi.contiguous(), tf32_rna(w.float() - hi).contiguous()
+
+
+def pack_stem_weight_tf32x2(weight):
+    """[Cout, 3, 7, 7] fp32 -> (hi, lo) fp32 [Cout, 224] in the K order of pack_stem_weight (k = r*32 + s*4 + c)."""
+    cout = weight.shape[0]
+    w = weight.new_zeros((cout, 7, 8, 4))
+    w[:, :, :7, :3] = weight.float().permute(0, 2, 3, 1)
+    return split_tf32x2(w.reshape(cout, 224))
+
+
+def conv2d_f32(x, w_hi, w_lo, bias, cout, ksize, relu=False, residual=None, upsample=None, out_mode=OUT_NHWC_F32, out=None,
+               stride=1, sink=None, tile_tab=None):
+    """Full-precision convolution (odtk_conv2d_f32): x NHWC fp32 [N,H,W,Cin] (or an fp32 AtlasView); w_hi / w_lo from
+    pack_weight_tf32x2; bias fp32 [Cout] or None; stride 1 / 2, pad ksize//2.  Returns NHWC fp32 [N,OH,OW,Cout]
+    (OUT_NHWC_F32, + residual NHWC fp32 [N,OH,OW,Cout] and / or upsample NHWC fp32 [N,H/2,W/2,Cout] before ReLU) or NCHW
+    fp32 [N,Cout,OH,OW]; `out` may be an fp32 AtlasView; tile_tab as for conv2d."""
+    xv = x if isinstance(x, AtlasView) else None
+    assert (xv.atlas if xv is not None else x).dtype == torch.float32
+    assert xv is not None or (x.is_cuda and x.is_contiguous())
+    assert w_hi.dtype == torch.float32 and w_lo.dtype == torch.float32
+    n, h, wd, cin = x.shape
+    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
+    if out_mode == OUT_CANDIDATES:
+        assert sink is not None
+    elif out is None:
+        if out_mode == OUT_NHWC_F32:
+            out = torch.empty((n, oh, ow, cout), dtype=torch.float32, device=x.device)
+        else:
+            out = torch.empty((n, cout, oh, ow), dtype=torch.float32, device=x.device)
+    for t in (residual, upsample):
+        assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+    d = ConvF32Desc()
+    d.x, d.w_hi, d.w_lo, d.y = x.data_ptr(), w_hi.data_ptr(), w_lo.data_ptr(), (out.data_ptr() if out is not None else None)
+    d.bias = bias.data_ptr() if bias is not None else None
+    d.residual = residual.data_ptr() if residual is not None else None
+    d.upsample = upsample.data_ptr() if upsample is not None else None
+    if xv is not None:
+        d.x_rows, d.x_width = xv.atlas.shape[1], xv.atlas.shape[2]
+    if isinstance(out, AtlasView):
+        d.y_rows, d.y_row_off, d.y_width = out.atlas.shape[1], 0, out.atlas.shape[2]     # data_ptr() already points at the level
+    if tile_tab is not None:
+        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    d.sink = ctypes.addressof(sink) if sink is not None else None
+    d.n, d.h, d.width, d.cin, d.cout, d.ksize, d.stride = n, h, wd, cin, cout, ksize, int(stride)
+    d.relu, d.out_mode = int(relu), out_mode
+    _lib.check(_lib.lib().odtk_conv2d_f32(ctypes.byref(d), _stream()), "conv2d_f32")
+    STATS["launches"] += 1
+    if STATS["trace"] is not None:
+        # 4-byte operands: activations read once (atlas launches: the pixels of the levels; 1x1 stride 2: the pixels it
+        # samples), both weight halves, the output, the addends
+        px = n * oh * ow if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
+        obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * 4
+        xbytes = px * cin * 4 if (tile_tab is not None or (ksize == 1 and stride == 2)) else n * h * wd * cin * 4
+        _trace("conv%dx%d_f32" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin,
+               xbytes + (w_hi.numel() + w_lo.numel()) * 4 + obytes + (px * cout * 4 if residual is not None else 0)
+               + (px * cout if upsample is not None else 0),
+               n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
+               upsample=upsample is not None, out_mode=out_mode)
+    return out
+
+
+def stem_conv_f32(xp, h, wd, w_hi, w_lo, bias, cout, relu=True):
+    """7x7 stride-2 pad-3 stem over the NHWC4 fp32 image [N, h+6, wd+8, 4] (pad_input_f32 / preprocess_u8_f32):
+    odtk_conv2d_f32 with ksize 7.  Returns NHWC fp32 [N, (h-1)/2+1, (wd-1)/2+1, cout]."""
+    assert xp.dtype == torch.float32 and xp.is_contiguous() and xp.shape[1:] == (h + 6, wd + 8, 4)
+    n = xp.shape[0]
+    out = torch.empty((n, (h - 1) // 2 + 1, (wd - 1) // 2 + 1, cout), dtype=torch.float32, device=xp.device)
+    d = ConvF32Desc()
+    d.x, d.w_hi, d.w_lo, d.y = xp.data_ptr(), w_hi.data_ptr(), w_lo.data_ptr(), out.data_ptr()
+    d.bias = bias.data_ptr() if bias is not None else None
+    d.n, d.h, d.width, d.cin, d.cout, d.ksize, d.stride = n, h, wd, 3, cout, 7, 2
+    d.relu, d.out_mode = int(relu), OUT_NHWC_F32
+    _lib.check(_lib.lib().odtk_conv2d_f32(ctypes.byref(d), _stream()), "conv2d_f32")
+    STATS["launches"] += 1
+    _trace("stem7x7_f32", 2 * out.numel() * 147, xp.numel() * 4 + (w_hi.numel() + w_lo.numel()) * 4 + out.numel() * 4,
+           n=n, h=h, w=wd, cin=3, cout=cout, stride=2)
+    return out
+
+
+def pad_input_f32(x):
+    """NHWC fp32 RGB batch [N,H,W,3] -> zero-bordered NHWC4 fp32 [N, H+6, W+8, 4] (odtk_pad_input_f32)."""
+    n, h, wd, c = x.shape
+    assert c == 3 and x.dtype == torch.float32 and x.is_contiguous()
+    xp = torch.empty((n, h + 6, wd + 8, 4), dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().odtk_pad_input_f32(ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(xp.data_ptr()), n, h, wd, _stream()),
+               "pad_input_f32")
+    STATS["launches"] += 1
+    _trace("pad_input_f32", 0, x.numel() * 4 + xp.numel() * 4, n=n, h=h, w=wd, cin=3)
+    return xp
+
+
+def preprocess_u8_f32(images, stride=128, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """preprocess_u8 into the fp32 NHWC4 stem buffer [N, Hs+6, Ws+8, 4] (odtk_preprocess_u8_f32): the normalised values
+    without the fp16 rounding.  Returns (buffer, Hs, Ws)."""
+    assert images.is_cuda and images.dtype == torch.uint8 and images.is_contiguous() and images.shape[-1] == 3
+    n, h, w, _ = images.shape
+    hs, ws = (h + stride - 1) // stride * stride, (w + stride - 1) // stride * stride
+    xp = torch.empty((n, hs + 6, ws + 8, 4), dtype=torch.float32, device=images.device)
+    m = (ctypes.c_float * 3)(*mean)
+    s = (ctypes.c_float * 3)(*std)
+    _lib.check(_lib.lib().odtk_preprocess_u8_f32(ctypes.c_void_p(images.data_ptr()), ctypes.c_void_p(xp.data_ptr()), n, h, w,
+                                                 hs, ws, m, s, _stream()), "preprocess_u8_f32")
+    STATS["launches"] += 1
+    _trace("preprocess_u8_f32", 0, images.numel() + xp.numel() * 4, n=n, h=h, w=w, cin=3)
+    return xp, hs, ws
+
+
+def resize_launch_f32(x_dev, x_bytes, plan, table_dev, out=None, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """resize_launch into the fp32 NHWC4 stem buffer [n, hs+6, ws+8, 4] (odtk_preprocess_resize_u8_f32)."""
+    hs, ws = plan.canvas
+    L = _lib.lib()
+    nbytes = _lib.check(L.odtk_preprocess_resize_u8_f32(None, x_bytes, ctypes.byref(plan.table), None, plan.n, hs, ws, None,
+                                                        None, None, None), "preprocess_resize_u8_f32")
+    if out is None:
+        out = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=torch.float32, device=x_dev.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.numel() * 4 == nbytes
+    m = (ctypes.c_float * 3)(*mean)
+    s = (ctypes.c_float * 3)(*std)
+    _lib.check(L.odtk_preprocess_resize_u8_f32(ctypes.c_void_p(x_dev.data_ptr()), x_bytes, ctypes.byref(plan.table),
+                                               ctypes.c_void_p(table_dev.data_ptr()), plan.n, hs, ws,
+                                               ctypes.c_void_p(out.data_ptr()), m, s, _stream()), "preprocess_resize_u8_f32")
+    STATS["launches"] += 1
+    _trace("preprocess_resize_u8_f32", 0, resize_bytes(plan) + plan.n * (hs + 6) * (ws + 8) * 8, n=plan.n, h=hs, w=ws, cin=3)
+    return out
+
+
+def maxpool3x3s2_f32(x):
+    """3x3 stride-2 pad-1 max-pool of NHWC fp32 [N,H,W,C] (odtk_maxpool3x3s2_f32)."""
+    n, h, w, c = x.shape
+    assert x.dtype == torch.float32 and x.is_contiguous()
+    out = torch.empty((n, (h - 1) // 2 + 1, (w - 1) // 2 + 1, c), dtype=torch.float32, device=x.device)
+    _lib.check(_lib.lib().odtk_maxpool3x3s2_f32(ctypes.c_void_p(x.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w, c,
+                                                _stream()), "maxpool3x3s2_f32")
+    STATS["launches"] += 1
+    _trace("maxpool_f32", 0, x.numel() * 4 + out.numel() * 4, n=n, h=h, w=w, cin=c)
+    return out
+
+
+def relu_from_view_f32(view):
+    """ReLU of a level of the fp32 atlas into a new dense fp32 tensor [N, h, w, C] (odtk_relu_copy_rows_f32): pyramid7's
+    input ReLU(P6) in full precision."""
+    n, h, w, c = view.shape
+    a = view.atlas
+    assert a.dtype == torch.float32
+    out = torch.empty((n, h, w, c), dtype=torch.float32, device=a.device)
+    _lib.check(_lib.lib().odtk_relu_copy_rows_f32(ctypes.c_void_p(view.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w * c,
+                                                  a.shape[1] * a.shape[2] * c, a.shape[2] * c, h * w * c, w * c, _stream()),
+               "relu_copy_rows_f32")
+    STATS["launches"] += 1
+    _trace("relu_f32", 0, out.numel() * 8, n=n, h=h, w=w, cin=c)
+    return out

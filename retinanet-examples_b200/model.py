@@ -32,6 +32,8 @@ RESNEXT = {"ResNeXt50_32x4dFPN": (32, 4), "ResNeXt101_32x8dFPN": (32, 8)}
 MOBILENET = {"MobileNetV2FPN": [(1, 16, 1, 1), (6, 24, 2, 2), (6, 32, 3, 2), (6, 64, 4, 2), (6, 96, 3, 1), (6, 160, 3, 2), (6, 320, 1, 1)]}
 MOBILENET_TAPS = (6, 13, 17)
 BACKBONES = tuple(RESNET_LAYERS) + tuple(MOBILENET)
+# backbones of the full-precision mode (set_precision("fp32")): the plain ResNets (no grouped or depthwise convolutions)
+FP32_BACKBONES = tuple(b for b in RESNET_LAYERS if b not in RESNEXT)
 
 
 def mobilenet_blocks(backbone):
@@ -239,6 +241,7 @@ class Model:
         self.int8_scope = "heads"     # "heads" or "network" (layer3, layer4 and the FPN in INT8 as well)
         self._calib_hook = None
         self._calib_net = False       # calibration also records the network scope's tensors
+        self._f32 = None              # full precision: split-TF32 weights of every layer (packed on first use)
 
     def __repr__(self):
         return '\n'.join(['     model: {}'.format(self.name), '  backbone: {}'.format(self.backbone),
@@ -296,6 +299,7 @@ class Model:
             raise RuntimeError("missing keys in state_dict: %s" % missing[:4])
         self._sd = {k: v.detach().float().cpu() for k, v in sd.items() if torch.is_tensor(v)}
         self._packed = None
+        self._f32 = None
         return self
 
     def cuda(self, device=None):
@@ -327,6 +331,7 @@ class Model:
     def _pack(self):
         sd, dev = self._sd, self.device
         P = {}
+        self._f32 = None
 
         def conv_bn(prefix_conv, prefix_bn, stride=1, groups=1):
             w, b = engine.fold_bn(sd[prefix_conv + ".weight"], sd[prefix_bn + ".weight"], sd[prefix_bn + ".bias"],
@@ -446,14 +451,76 @@ class Model:
         N["pyramid7"] = plain("pyramid7", s32("heads.input"), "heads.input", 2)
         return N
 
+    def _pack_f32(self):
+        """Full precision: every convolution of the ResNet backbone, the FPN and the heads with BatchNorm folded in fp32 (as
+        _pack does), its weights split into two tf32-valued halves (engine.pack_weight_tf32x2), the fp32 bias and the
+        geometry."""
+        sd, dev = self._sd, self.device
+        block, layers = RESNET_LAYERS[self.backbone]
+        f, n = "backbones.%s.features." % self.backbone, "backbones.%s." % self.backbone
+
+        def layer(w, b, stride=1, stem=False):
+            hi, lo = engine.pack_stem_weight_tf32x2(w) if stem else engine.pack_weight_tf32x2(w)
+            return {"hi": hi.to(dev), "lo": lo.to(dev), "b": b.float().contiguous().to(dev) if b is not None else None,
+                    "cout": w.shape[0], "ks": w.shape[2], "stride": stride}
+
+        def folded(pc, pb, stride=1, stem=False):
+            w, b = engine.fold_bn(sd[pc + ".weight"], sd[pb + ".weight"], sd[pb + ".bias"], sd[pb + ".running_mean"],
+                                  sd[pb + ".running_var"])
+            return layer(w, b, stride, stem)
+
+        def plain(name, stride=1):
+            return layer(sd[n + name + ".weight"], sd.get(n + name + ".bias"), stride)
+
+        F = {"stem": folded(f + "conv1", f + "bn1", 2, stem=True), "blocks": []}
+        for li, nblocks in enumerate(layers):
+            for b in range(nblocks):
+                stride = 2 if (b == 0 and li > 0) else 1
+                p = f + "layer%d.%d." % (li + 1, b)
+                if block == "bottleneck":       # torchvision v1.5: the 3x3 carries the stride
+                    convs = [folded(p + "conv1", p + "bn1"), folded(p + "conv2", p + "bn2", stride), folded(p + "conv3", p + "bn3")]
+                else:
+                    convs = [folded(p + "conv1", p + "bn1", stride), folded(p + "conv2", p + "bn2")]
+                down = folded(p + "downsample.0", p + "downsample.1", stride) if (p + "downsample.0.weight") in sd else None
+                F["blocks"].append({"convs": convs, "down": down, "level": li + 2, "last": b == nblocks - 1})
+        for k in ("lateral3", "lateral4", "lateral5", "smooth3", "smooth4", "smooth5"):
+            F[k] = plain(k)
+        F["pyramid6"] = plain("pyramid6", 2)
+        F["pyramid7"] = plain("pyramid7", 2)
+        for head in ("cls_head", "box_head"):
+            F[head] = [layer(sd["%s.%d.weight" % (head, i)], sd.get("%s.%d.bias" % (head, i))) for i in (0, 2, 4, 6, 8)]
+        return F
+
+    def _full_precision(self):
+        """True when the inference forward runs in fp32 (set_precision("fp32")); the training-mode forward stays fp16."""
+        return self.precision == "fp32" and not self.training
+
+    def _f32_layers(self):
+        if self._f32 is None:
+            self._f32 = self._pack_f32()
+        return self._f32
+
     def set_precision(self, precision, table=None, scope="heads"):
-        """"fp16" (default) or "int8": the head towers and the two final head layers run on the s8 tensor cores with the
+        """"fp16" (default), "fp32" or "int8".  "fp32" (full precision, the reference's --full-precision): fp32
+        activations end to end and every convolution on split-TF32 tensor-core products (odtk_conv2d_f32); its head outputs
+        are within 1e-4 - 2.3e-4 * max|ref| of fp32 PyTorch (measured on the H100) instead of fp16's 1.4e-3 - 2.1e-3 --
+        ResNet18/34/50/101/152FPN (not ResNeXt or
+        MobileNetV2), over the pyramid atlas (ODTK_MERGED_HEADS=1); the fused stem-pool and bottleneck kernels are not
+        used, and the split weights are packed on the first fp32 forward.  "int8": the head towers and the two final head layers run on the s8 tensor cores with the
         activation scales of `table` (a path or a dict, from `calibrate`).  scope "heads" (default): the backbone and the
         FPN stay fp16; "network" (a table from calibrate(..., scope="network")): ResNet layer3, layer4 and the FPN run in
         INT8 too, from layer2's output quantised once, and the FPN writes the s8 atlas the heads read -- the stem, layer1 and
         layer2 stay fp16 (ResNet18/34/50/101/152 backbones; ResNeXt and MobileNetV2 take "heads" only).  The training-mode
         forward stays fp16.  INT8 needs the pyramid atlas (ODTK_MERGED_HEADS=1).  Captured CUDA graphs are dropped."""
         if precision == "fp16":
+            self._int8_table = None
+            self._int8 = None
+            self.int8_scope = "heads"
+        elif precision == "fp32":
+            if self.backbone not in FP32_BACKBONES:
+                raise ValueError("full precision covers %s, not %s" % (", ".join(FP32_BACKBONES), self.backbone))
+            if not self.merged_heads:
+                raise ValueError("full precision runs the heads over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
             self._int8_table = None
             self._int8 = None
             self.int8_scope = "heads"
@@ -469,7 +536,9 @@ class Model:
             if self._packed is not None:
                 self._pack_int8()
         else:
-            raise ValueError("precision must be 'fp16' or 'int8', got %r" % (precision,))
+            raise ValueError("precision must be 'fp16', 'fp32' or 'int8', got %r" % (precision,))
+        if precision != "fp32":
+            self._f32 = None
         self.precision = precision
         if getattr(self, "_graphs", None):
             self._graphs = {}
@@ -494,8 +563,9 @@ class Model:
             raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
         batches = list(batches)
         col = calib.Collector()
-        saved = (self._int8, self.parallel_heads, self.training)
+        saved = (self._int8, self.parallel_heads, self.training, self.precision)
         self._int8, self.parallel_heads, self.training = None, False, False
+        self.precision = "fp16" if self.precision == "fp32" else self.precision
         self._calib_hook = col.observe
         self._calib_net = scope == "network"
         images = 0
@@ -512,7 +582,7 @@ class Model:
                         images += x.shape[0] if phase == 0 else 0
             torch.cuda.synchronize()
         finally:
-            self._int8, self.parallel_heads, self.training = saved
+            self._int8, self.parallel_heads, self.training, self.precision = saved
             self._calib_hook = None
             self._calib_net = False
         t = calib.make_table(self.backbone, self.classes, self.num_anchors, method, images, col.scales(method, names), scope)
@@ -722,6 +792,54 @@ class Model:
         self._conv8(N["pyramid7"], engine.relu_from_view_s8(v[3]), out=v[4])
         return v
 
+    def _conv32(self, L, x, relu=False, out=None, valid_px=None, **kw):
+        """One full-precision convolution (a layer of _pack_f32) of NHWC fp32 x (or an fp32 AtlasView)."""
+        n, h, w, cin = x.shape
+        oh, ow = ((h - 1) // 2 + 1, (w - 1) // 2 + 1) if L["stride"] == 2 else (h, w)
+        px = n * oh * ow if valid_px is None else valid_px
+        engine.STATS["conv_flops"] += 2 * px * L["cout"] * L["ks"] * L["ks"] * cin
+        return engine.conv2d_f32(x, L["hi"], L["lo"], L["b"], L["cout"], L["ks"], relu=relu, out=out, stride=L["stride"], **kw)
+
+    def _input_f32(self, x):
+        """NCHW float batch -> the fp32 NHWC4 stem buffer (xp, h, w)."""
+        if x.dim() != 4:
+            raise ValueError("expected a [B, 3, H, W] batch")
+        return engine.pad_input_f32(x.permute(0, 2, 3, 1).contiguous().float()), x.shape[2], x.shape[3]
+
+    def _features_f32(self, xp, h, w):
+        """Full precision from the fp32 NHWC4 stem buffer [N, h+6, w+8, 4]: stem convolution (+ ReLU) and max-pool, the
+        ResNet blocks as their 1x1 / 3x3 launches with the residual added in the last one's epilogue, then the FPN into
+        the fp32 atlas.  Returns the five level views."""
+        F = self._f32_layers()
+        st = F["stem"]
+        engine.STATS["conv_flops"] += 2 * xp.shape[0] * ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1) * st["cout"] * 49 * 3
+        x = engine.maxpool3x3s2_f32(engine.stem_conv_f32(xp, h, w, st["hi"], st["lo"], st["b"], st["cout"], relu=True))
+        outs = {}
+        for blk in F["blocks"]:
+            identity = x if blk["down"] is None else self._conv32(blk["down"], x)
+            t = x
+            for L in blk["convs"][:-1]:
+                t = self._conv32(L, t, relu=True)
+            x = self._conv32(blk["convs"][-1], t, relu=True, residual=identity)
+            if blk["last"]:
+                outs[blk["level"]] = x
+        c3, c4, c5 = outs[3], outs[4], outs[5]
+        p5 = self._conv32(F["lateral5"], c5)
+        p4 = self._conv32(F["lateral4"], c4, upsample=p5)
+        p3 = self._conv32(F["lateral3"], c3, upsample=p4)
+        n = c5.shape[0]
+        h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
+        sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
+                 ((h6 - 1) // 2 + 1, (w6 - 1) // 2 + 1))
+        at = self._atlas_for(n, sizes, c5.device)
+        v = [engine.AtlasView(self._atlas_f32(at)[0], r, lh, lw) for r, (lh, lw) in zip(at["rows"], sizes)]
+        self._conv32(F["smooth3"], p3, out=v[0])
+        self._conv32(F["smooth4"], p4, out=v[1])
+        self._conv32(F["smooth5"], p5, out=v[2])
+        self._conv32(F["pyramid6"], c5, out=v[3])
+        self._conv32(F["pyramid7"], engine.relu_from_view_f32(v[3]), out=v[4])
+        return v
+
     def _fpn(self, c3, c4, c5):
         """FPN (odtk/backbones/fpn.py:45-61) on the three backbone taps."""
         P = self._packed
@@ -779,6 +897,14 @@ class Model:
             buf = at["buf"][0]
             at["buf8"] = [torch.zeros(buf.shape, dtype=torch.int8, device=buf.device) for _ in range(5)]
         return at["buf8"]
+
+    @staticmethod
+    def _atlas_f32(at):
+        """The five fp32 buffers of an atlas geometry (full precision), zero-initialised on first use."""
+        if "buf32" not in at:
+            buf = at["buf"][0]
+            at["buf32"] = [torch.zeros(buf.shape, dtype=torch.float32, device=buf.device) for _ in range(5)]
+        return at["buf32"]
 
     def _heads(self, features, sigmoid=True, sinks=None):
         """Class / box heads on the five levels (odtk/model.py:134-135).  The ten conv chains are
@@ -892,6 +1018,24 @@ class Model:
                 return outs
 
             tower, bufs = tower8, buf8
+        elif self._full_precision():
+            # full precision: the FPN wrote the fp32 atlas; towers and final layers on split-TF32 products
+            f32 = self._f32_layers()
+
+            def tower32(head, bufs, final_mode, use_sinks):
+                t = atlas0
+                for i, L in enumerate(f32[head][:-1]):
+                    nxt = bufs[i & 1]
+                    self._conv32(L, t, relu=True, out=nxt, tile_tab=at["tab"], valid_px=at["px"])
+                    t = nxt
+                outs = []
+                for l, v in enumerate(views):
+                    lv = engine.AtlasView(t, at["rows"][l], v.h, v.w)
+                    mode, sink = (engine.OUT_CANDIDATES, use_sinks[l]) if use_sinks is not None else (final_mode, None)
+                    outs.append(self._conv32(f32[head][-1], lv, out_mode=mode, sink=sink))
+                return outs
+
+            tower, bufs = tower32, self._atlas_f32(at)
         else:
             bufs = at["buf"]
 
@@ -927,6 +1071,9 @@ class Model:
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
         P = self._packed
+        if self._full_precision():
+            xp, hs, ws = engine.preprocess_u8_f32(images, self.stride)
+            return self._heads(self._features_f32(xp, hs, ws), sigmoid), (hs, ws)
         xp, hs, ws = engine.preprocess_u8(images, self.stride)
         return self._heads(self._features(self._stem(padded=(xp, hs, ws))), sigmoid), (hs, ws)
 
@@ -935,6 +1082,8 @@ class Model:
         (sigmoid) class maps [B, A*C, H, W] and box maps [B, A*4|6, H, W], fp32 NCHW."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
+        if self._full_precision():
+            return self._heads(self._features_f32(*self._input_f32(x)), sigmoid)
         return self._heads(self._features(self._stem(self._to_nhwc_half(x))), sigmoid)
 
     def _level_anchors(self, widths, width):
@@ -955,7 +1104,14 @@ class Model:
         of odtk/model.py:140 are never written or re-read.  Same detections as the dense route."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
-        if x.dtype == torch.uint8:
+        if self._full_precision():
+            if x.dtype == torch.uint8:
+                xp, hs, width = engine.preprocess_u8_f32(x, self.stride)
+                features = self._features_f32(xp, hs, width)
+            else:
+                width = x.shape[-1]
+                features = self._features_f32(*self._input_f32(x))
+        elif x.dtype == torch.uint8:
             xp, hs, width = engine.preprocess_u8(x, self.stride)
             features = self._features(self._stem(padded=(xp, hs, width)))
         else:
@@ -1061,8 +1217,12 @@ class Model:
 
     # ---- raw images of any size (the PIL data loader of `odtk infer`, odtk/data.py:55-60, 113-123, 154-176) ------------
     def _forward_padded(self, xp, hs, width):
-        """Detections from the stem's padded NHWC4 input buffer: the fused-candidate or the dense route of forward()."""
-        features = self._features(self._stem(padded=(xp, hs, width)))
+        """Detections from the stem's padded NHWC4 input buffer (fp32 in full precision): the fused-candidate or the dense
+        route of forward()."""
+        if self._full_precision():
+            features = self._features_f32(xp, hs, width)
+        else:
+            features = self._features(self._stem(padded=(xp, hs, width)))
         if self.fused_candidates:
             return self._detect_fused(features, width)
         return self._detect_dense(*self._heads(features), width)
@@ -1083,7 +1243,8 @@ class Model:
         plan = engine.ResizePlan(engine.image_shapes(images), resize, max_size, self.stride, canvas)
         hs, ws = plan.canvas
         if getattr(self, "_graphs", None) is None:
-            xp, _, _, ratios = engine.preprocess_resize_u8(images, resize, max_size, self.stride, (hs, ws))
+            xp, _, _, ratios = engine.preprocess_resize_u8(images, resize, max_size, self.stride, (hs, ws),
+                                                           f32=self._full_precision())
             return self._forward_padded(xp, hs, ws), ratios
         key = ("images", plan.n, hs, ws)
         entry = self._graphs.get(key)
@@ -1102,10 +1263,10 @@ class Model:
         tpad = engine.table_pad(plan.n)
         buf = torch.empty(tpad + capacity, dtype=torch.uint8, device=dev)
         hs, ws = plan.canvas
-        xp = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=torch.float16, device=dev)
+        xp = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=self._stem_dtype(), device=dev)
 
         def run():
-            engine.resize_launch(buf[tpad:], capacity, plan, buf[:tpad], out=xp)
+            self._resize_launch(buf[tpad:], capacity, plan, buf[:tpad], out=xp)
             return self._forward_padded(xp, hs, ws)
 
         engine.stage_images(images, plan, buf)
@@ -1116,6 +1277,13 @@ class Model:
         with torch.cuda.graph(graph):
             out = run()
         return {"graph": graph, "buf": buf, "xp": xp, "out": out, "capacity": capacity}
+
+    def _stem_dtype(self):
+        return torch.float32 if self._full_precision() else torch.float16
+
+    def _resize_launch(self, *args, **kwargs):
+        """engine.resize_launch into the stem buffer of the current precision."""
+        return (engine.resize_launch_f32 if self._full_precision() else engine.resize_launch)(*args, **kwargs)
 
     # ---- JPEG streams (the Image.open(path).convert("RGB") of odtk/data.py:50, then the raw-image path) ------------------
     def forward_jpeg(self, datas, resize=800, max_size=1333, canvas=None):
@@ -1167,7 +1335,7 @@ class Model:
         """Decode into the packed pixel buffer at the resize plan's offsets, then resize it into the stem buffer; the
         resize kernel reads the size table staged with the batch."""
         engine.jpeg_launch(batch, bufs["buf"], plan.table, bufs["workspace"], bufs["pixels"], bufs["status"])
-        return engine.resize_launch(bufs["pixels"], bufs["pixels"].numel(), plan, bufs["buf"][batch.resize_off:], out=xp)
+        return self._resize_launch(bufs["pixels"], bufs["pixels"].numel(), plan, bufs["buf"][batch.resize_off:], out=xp)
 
     def _capture_jpeg(self, batch, plan, capacity):
         """CUDA graph of decode + resize + network over static buffers of `capacity` (staging, workspace, pixel bytes)
@@ -1175,7 +1343,7 @@ class Model:
         canvas and the buffers replays it."""
         bufs = self._jpeg_buffers(plan.n, capacity)
         hs, ws = plan.canvas
-        xp = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=torch.float16, device=bufs["buf"].device)
+        xp = torch.empty((plan.n, hs + 6, ws + 8, 4), dtype=self._stem_dtype(), device=bufs["buf"].device)
 
         def run():
             self._jpeg_decode_resize(batch, plan, bufs, xp)

@@ -7,7 +7,9 @@ mbarrier rings: conv modes 0 / 1 / 2 / 3 with N tiles 64 and 128, ragged M and N
 fp32 / sigmoid / candidate epilogues, the fused stem + pool (stem.cu: halo rows at the image edges), the fused bottleneck
 tail (bottleneck.cu: C1 64 / 128, projected identity, GEMM3 with 64 / 128 outputs -- shared-memory A operands written
 by the epilogues), the s8 instantiation of the conv kernel (stride 2 in modes 3 and 1, residual / upsample addends, level-view
-input and output) and the INT8 heads and network scope of the model, decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
+input and output) and the INT8 heads and network scope of the model, the split-TF32 fp32 instantiation (`fp32`: modes 0 / 1 / 2 /
+3, N tiles 64 / 128, several tiles per CTA so the A_lo side buffers and the named barrier cycle, tile table and level views,
+fp32 addends, NCHW / sigmoid / candidate epilogues, the fp32 small kernels, the fp32 model), decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
 iou, target assignment, the cooperative loss kernel."""
 import os
 import sys
@@ -36,6 +38,75 @@ def conv(n, h, w, cin, cout, ks, **kw):
     torch.cuda.synchronize()
     print("conv %s -> plan %s" % ((n, h, w, cin, cout, ks), {k: v for k, v in engine.last_plan().items() if v}), flush=True)
     return y
+
+
+def conv32(n, h, w, cin, cout, ks, x=None, **kw):
+    """One odtk_conv2d_f32 launch on random fp32 operands (addends requested by residual=True / upsample=True)."""
+    x = (torch.randn((n, h, w, cin), generator=g).to(DEV)) if x is None else x
+    hi, lo = [t.to(DEV) for t in engine.pack_weight_tf32x2(torch.randn((cout, cin, ks, ks), generator=g) * 0.05)]
+    stride = kw.get("stride", 1)
+    oh, ow = ((h - 1) // 2 + 1, (w - 1) // 2 + 1) if stride == 2 else (h, w)
+    if kw.pop("residual", False):
+        kw["residual"] = torch.randn((n, oh, ow, cout), generator=g).to(DEV)
+    if kw.pop("upsample", False):
+        kw["upsample"] = torch.randn((n, h // 2, w // 2, cout), generator=g).to(DEV)
+    y = engine.conv2d_f32(x, hi, lo, torch.randn(cout, generator=g).to(DEV), cout, ks, **kw)
+    torch.cuda.synchronize()
+    print("conv_f32 %s -> plan %s" % ((n, h, w, cin, cout, ks, stride), {k: v for k, v in engine.last_plan().items() if v}), flush=True)
+    return y
+
+
+def fp32_cases():
+    """Every variant of the split-TF32 instance (conv.cu, kOpTF32x3) and the fp32 twins of layers.cu."""
+    conv32(2, 16, 16, 64, 64, 1, relu=True)                                # mode 0, N tile 64
+    conv32(2, 16, 16, 256, 256, 1, relu=True, residual=True)               # residual epilogue
+    conv32(1, 16, 32, 256, 256, 1, upsample=True)                          # upsample-add epilogue
+    conv32(1, 18, 20, 256, 256, 1, upsample=True)                          # ragged last M tile
+    conv32(40, 100, 160, 64, 256, 1, relu=True)                            # mode 0, N tile 128, several tiles per CTA
+    conv32(1, 16, 24, 64, 64, 3, relu=True)                                # mode 1, N tile 64
+    conv32(1, 7, 10, 96, 256, 3, relu=True)                                # mode 1, 70-pixel patch, 3 K blocks per tap
+    conv32(10, 48, 64, 256, 256, 3, relu=True, residual=True)              # mode 1, N tile 128, several tiles per CTA
+    conv32(2, 26, 40, 128, 128, 3, relu=True, stride=2)                    # mode 3 (parity split)
+    conv32(2, 28, 20, 256, 512, 1, stride=2)                               # mode 3, 1x1
+    conv32(2, 25, 39, 256, 256, 3, relu=True, stride=2)                    # mode 1, element-strided boxes
+    conv32(2, 100, 160, 256, 36, 3, out_mode=engine.OUT_NCHW_F32)          # narrow head output, ragged N tile
+    conv32(1, 24, 32, 256, 720, 3, out_mode=engine.OUT_NCHW_F32_SIGMOID)   # ragged 128-wide N tile
+    conv32(1, 5, 7, 256, 2160, 3, out_mode=engine.OUT_NCHW_F32)
+    # stem (mode 2) over the fp32 NHWC4 image: even and odd sides; max-pool
+    for h, w in ((64, 96), (37, 51)):
+        x = torch.randn((2, h, w, 3), generator=g).to(DEV)
+        hi, lo = [t.to(DEV) for t in engine.pack_stem_weight_tf32x2(torch.randn((64, 3, 7, 7), generator=g) * 0.1)]
+        engine.maxpool3x3s2_f32(engine.stem_conv_f32(engine.pad_input_f32(x), h, w, hi, lo, torch.randn(64, generator=g).to(DEV), 64))
+        torch.cuda.synchronize()
+        print("stem_f32 %dx%d ok" % (h, w), flush=True)
+    # atlas: one launch over every level (tile table), level view -> level view, stride 2 into a level view, ReLU copy
+    m = Model("ResNet18FPN", classes=2)
+    sizes = ((20, 32), (10, 16), (5, 8), (3, 4), (2, 2))
+    at = m._atlas_for(2, sizes, torch.device(DEV))
+    xa = torch.randn(at["buf"][0].shape, generator=g).to(DEV)
+    ya = torch.zeros(at["buf"][0].shape, dtype=torch.float32, device=DEV)
+    conv32(2, xa.shape[1], xa.shape[2], 256, 256, 3, x=xa, relu=True, out=ya, tile_tab=at["tab"])
+    conv32(2, *sizes[1], 256, 256, 3, x=engine.AtlasView(xa, at["rows"][1], *sizes[1]), out=engine.AtlasView(ya, at["rows"][1], *sizes[1]))
+    conv32(2, *sizes[2], 256, 256, 3, stride=2, out=engine.AtlasView(ya, at["rows"][3], *sizes[3]))
+    engine.relu_from_view_f32(engine.AtlasView(ya, at["rows"][3], *sizes[3]))
+    # input side
+    engine.preprocess_u8_f32(torch.randint(0, 256, (2, 100, 130, 3), dtype=torch.uint8, generator=g).to(DEV))
+    imgs = [torch.randint(0, 256, s, dtype=torch.uint8, generator=g) for s in ((30, 40, 3), (300, 170, 3), (900, 41, 3))]
+    engine.preprocess_resize_u8(imgs, 64, 100, f32=True)
+    torch.cuda.synchronize()
+    print("fp32 layers ok", flush=True)
+    # the fp32 model: candidate epilogue and dense route, axis-aligned and rotated
+    for rotated in (False, True):
+        classes, na = 4, 27 if rotated else 9
+        sd = make_state_dict("ResNet18FPN", classes, na, rotated, seed=1)
+        sd["cls_head.8.bias"] = torch.full_like(sd["cls_head.8.bias"], -2.5)
+        m = Model("ResNet18FPN", classes=classes, rotated_bbox=rotated).load_state_dict(sd).cuda(0).set_precision("fp32")
+        x = torch.randn((2, 3, 128, 256), generator=g).to(DEV)
+        for fused in (True, False):
+            m.fused_candidates = fused
+            out = m(x)
+            torch.cuda.synchronize()
+            print("model fp32 rotated=%s fused=%s detections=%d" % (rotated, fused, int((out[0] > 0).sum())), flush=True)
 
 
 def main():
@@ -131,6 +202,8 @@ def main():
             out = m(x)
             torch.cuda.synchronize()
             print("model int8 network rotated=%s detections=%d" % (rotated, int((out[0] > 0).sum())), flush=True)
+    if only in ("", "fp32"):
+        fp32_cases()
     if only in ("", "postproc"):
         cls, deltas = synth.head_outputs(1, seed=0)
         anchors = [box.generate_anchors(s, box.DEFAULT_RATIOS, box.DEFAULT_SCALES).reshape(-1).tolist() for s in synth.LEVEL_STRIDES]
