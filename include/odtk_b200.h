@@ -297,6 +297,51 @@ typedef struct {
   int tab_tiles;
 } odtk_conv_f32_t;
 int odtk_conv2d_f32(const odtk_conv_f32_t *desc, odtk_stream_t stream);
+
+/* ---- training: backward of the 3x3 stride-1 head convolutions (H100-native; the reference runs them through cuDNN's
+ * autograd, odtk/train.py:94-123).  All three calls work over the pyramid atlas of odtk_conv_t (or a dense NHWC tensor).
+ *
+ * Weight gradient: dw[co, ci, ky, kx] = sum over images and pixels p of g[p, co] * x[p + (ky - 1, kx - 1), ci] (zero
+ * padding), db[co] = sum_p g[p, co]; fp32 results in the reference's parameter layouts ([cout, cin, 3, 3], [cout]).
+ *   g   NHWC fp16 [n, h, width, cout_pad]: the gradient w.r.t. the convolution's output (before its ReLU), cout_pad a
+ *       multiple of 64, zero outside the pixels of the levels and in the channels >= cout
+ *   x   NHWC fp16 [n, h, width, cin]: the convolution's input, cin % 128 == 0
+ *   tile_tab / tab_tiles   the atlas tile table of odtk_conv_t, or NULL: the 8 x 16 tiles of a dense h x width image
+ * Deterministic: the K (pixel) dimension is split over the CTAs, fp32 partials are summed in a fixed order, so two calls
+ * on the same inputs return the same bits.  workspace == NULL or workspace_size == 0 returns the bytes needed.       */
+typedef struct {
+  const void *g;
+  const void *x;
+  float *dw;            /* fp32 [cout, cin, 3, 3]                                                            */
+  float *db;            /* fp32 [cout] or NULL                                                               */
+  int n, h, width, cin, cout, cout_pad;
+  const void *tile_tab;
+  int tab_tiles;
+} odtk_wgrad_t;
+long long odtk_conv_wgrad(const odtk_wgrad_t *desc, void *workspace, size_t workspace_size, odtk_stream_t stream);
+
+/* Loss gradients -> fp16 gradient atlas: level l's fp32 NCHW gradient [batch, channels, height, width] times *scale (a
+ * DEVICE fp32 scalar, NULL for 1: the upstream autograd factor, e.g. a GradScaler scale, read without a host sync) lands at rows [row0, row0 + height) x columns [0, width) of the NHWC
+ * fp16 atlas [batch, rows, atlas_width, cout_pad], channels >= `channels` as zeros.  Nothing else of the atlas is written:
+ * the caller zero-fills it once (gap rows and columns right of the narrow levels are the convolutions' padding).  fp16
+ * overflow gives +-inf (round to nearest), never a saturated value, so that a GradScaler sees it and skips the step.    */
+typedef struct {
+  const float *grad;    /* device fp32 [batch, channels, height, width] */
+  int height, width, row0;
+} odtk_grad_level_t;
+int odtk_grad_to_atlas(int batch, int num_levels, const odtk_grad_level_t *levels, int channels, const float *scale, void *atlas,
+                       int rows, int atlas_width, int cout_pad, odtk_stream_t stream);
+
+/* Input gradient of a 3x3 stride-1 convolution, masked by the ReLU derivative of its input: odtk_conv2d on `base` (x =
+ * the output gradient g, w = the weights rotated by 180 degrees with cin / cout swapped, out_mode ODTK_OUT_NHWC_F16, no
+ * bias, no ReLU; residual adds a second gradient, e.g. the other head tower's), then every output element whose `mask`
+ * element is not > 0 becomes 0.  mask: NHWC fp16 [n, h, width, cout] (the layer input saved by the forward pass; the
+ * tile table's geometry when base.tile_tab is set), or NULL for no mask.  fp16 overflow gives +-inf.                  */
+typedef struct {
+  odtk_conv_t base;
+  const void *mask;
+} odtk_conv_dgrad_t;
+int odtk_conv2d_dgrad(const odtk_conv_dgrad_t *desc, odtk_stream_t stream);
 /* fp32 twins of the small layers around the convolutions (full-precision mode), same geometry as the fp16 calls:
  *   odtk_pad_input_f32          NHWC fp32 RGB [n, h, w, 3] -> zero-bordered NHWC4 fp32 [n, h+6, w+8, 4]
  *   odtk_preprocess_u8_f32      as odtk_preprocess_u8, the normalised fp32 values without the fp16 rounding

@@ -56,6 +56,10 @@ SIGNATURES = {
     "odtk_relu_copy_rows_s8": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int] +
                                [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     "odtk_conv2d_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_conv_wgrad": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "odtk_grad_to_atlas": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
+                                          ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
+    "odtk_conv2d_dgrad": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     "odtk_pad_input_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "odtk_preprocess_u8_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 5 + [_c_f32p, _c_f32p, ctypes.c_void_p]),
     "odtk_preprocess_resize_u8_f32": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p] +

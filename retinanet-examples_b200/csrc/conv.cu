@@ -61,8 +61,8 @@ constexpr int kSplitBytes = 2 * 2 * kLoBytes;
 constexpr int kSmemBytesF32 = kPipeBytes + kSplitBytes + 1024 + 256;
 static_assert(kSmemBytesF32 <= 227 * 1024, "fp32 instance exceeds the opt-in shared memory");
 
-// operand types of conv_gemm_kernel
-enum ConvOp { kOpF16 = 0, kOpS8 = 1, kOpTF32x3 = 2 };
+// operand types of conv_gemm_kernel; kOpF16Mask: fp16 with the ReLU-derivative mask of the input gradient (odtk_conv2d_dgrad)
+enum ConvOp { kOpF16 = 0, kOpS8 = 1, kOpTF32x3 = 2, kOpF16Mask = 3 };
 
 // round to the nearest tf32 value, ties away from zero (low 13 bits cleared)
 __device__ __forceinline__ float tf32_rna(float x) {
@@ -317,12 +317,14 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           continue;
         }
       }
-      if (OP == kOpF16 && p.out_mode == ODTK_OUT_NHWC_F16) {
+      if ((OP == kOpF16 || OP == kOpF16Mask) && p.out_mode == ODTK_OUT_NHWC_F16) {
         if (!valid) continue;
         const long long opix = p.mode != 0 ? ((long long)img * p.oH + p.oR + h) * p.oW + w : m;
         __half *o = reinterpret_cast<__half *>(p.out) + opix * p.ldy;
         const __half *res = p.residual ? p.residual + m * p.ldr : nullptr;
         const __half *up = p.upsample ? p.upsample + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
+        const __half *msk = nullptr;
+        if constexpr (OP == kOpF16Mask) msk = p.mask ? p.mask + m * p.Cout : nullptr;
 #pragma unroll
         for (int j = 0; j < BN / 8; j++) {
           const int col = n0 + 8 * j + 2 * q;
@@ -331,6 +333,13 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           if (p.bias) { v0 += __ldg(p.bias + col); v1 += __ldg(p.bias + col + 1); }
           if (res) { const float2 r = __half22float2(*reinterpret_cast<const __half2 *>(res + col)); v0 += r.x; v1 += r.y; }
           if (up) { const float2 u = __half22float2(*reinterpret_cast<const __half2 *>(up + col)); v0 += u.x; v1 += u.y; }
+          if constexpr (OP == kOpF16Mask) {
+            if (msk) {   // a select, not a product: an inf gradient where the input was <= 0 still becomes 0
+              const __half2 mm = *reinterpret_cast<const __half2 *>(msk + col);
+              if (!(__low2float(mm) > 0.0f)) v0 = 0.0f;
+              if (!(__high2float(mm) > 0.0f)) v1 = 0.0f;
+            }
+          }
           __half2 y = __floats2half2_rn(v0, v1);
           if (p.relu) {   // on the packed halves: max(round(x), 0) == round(max(x, 0))
             y = __hmax2(y, __float2half2_rn(0.0f));
@@ -516,7 +525,9 @@ bool device_ready() {
       cudaFuncSetAttribute(conv_gemm_kernel<64, kOpS8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
       cudaFuncSetAttribute(conv_gemm_kernel<128, kOpS8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
       cudaFuncSetAttribute(conv_gemm_kernel<64, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess)
+      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<64, kOpF16Mask>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpF16Mask>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
     return false;
   g_dev_ready[dev] = true;
   return true;
@@ -543,6 +554,9 @@ int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMa
     } else if (op == kOpTF32x3) {
       if (BN == 64) launch_bn<64, kOpTF32x3>(grid, stream, tmA, tmB, tmA2, tmB2, p);
       else          launch_bn<128, kOpTF32x3>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+    } else if (op == kOpF16Mask) {
+      if (BN == 64) launch_bn<64, kOpF16Mask>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      else          launch_bn<128, kOpF16Mask>(grid, stream, tmA, tmB, tmA2, tmB2, p);
     } else {
       if (BN == 64) launch_bn<64, kOpF16>(grid, stream, tmA, tmB, tmA2, tmB2, p);
       else          launch_bn<128, kOpF16>(grid, stream, tmA, tmB, tmA2, tmB2, p);
@@ -637,9 +651,15 @@ int a_operand(ConvParams &p, CUtensorMap &tmA, const void *x, int n, int h, int 
 }
 
 // odtk_conv2d, plus (mode 0 only) a second operand pair added to the same accumulator: y = x * w^T + x2 * w2^T with
-// x2 [M, c2in], w2 [cout, c2in] (the projected identity of a bottleneck block)
-int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cudaStream_t stream) {
+// x2 [M, c2in], w2 [cout, c2in] (the projected identity of a bottleneck block).  dgrad: odtk_conv2d_dgrad (the masked
+// instance; a tile-table launch may then take a residual, a whole atlas like y).
+int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cudaStream_t stream, bool dgrad = false,
+             const void *mask = nullptr) {
   if (!d || !d->x || !d->w) return ODTK_E_INVALID;
+  if (dgrad && (d->ksize != 3 || d->stride > 1 || d->out_mode != ODTK_OUT_NHWC_F16 || d->relu || d->groups > 1 || d->upsample ||
+                d->x_rows > 0 || d->x_width > 0 || d->y_rows > 0 || d->y_width > 0 || d->y_row_off > 0))
+    return ODTK_E_UNSUPPORTED;
+  if (mask && ((uintptr_t)mask & 3)) return ODTK_E_INVALID;
   if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
   if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
   if (d->ksize != 1 && d->ksize != 3) return ODTK_E_UNSUPPORTED;
@@ -690,10 +710,12 @@ int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cud
   const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
   const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
   const bool y_view = d->y_rows > 0 || d->y_width > 0 || d->y_row_off > 0;
-  if ((x_view || y_view || d->tile_tab) && (d->ksize != 3 || d->residual || d->upsample)) return ODTK_E_UNSUPPORTED;
+  if ((x_view || y_view || (d->tile_tab && !dgrad)) && (d->ksize != 3 || d->residual || d->upsample)) return ODTK_E_UNSUPPORTED;
   if (y_view && d->out_mode != ODTK_OUT_NHWC_F16) return ODTK_E_UNSUPPORTED;
   if (d->tile_tab && (d->tab_tiles <= 0 || stride != 1 || x_view || y_view)) return ODTK_E_INVALID;
   if (x2 && (d->ksize != 1 || stride != 1 || c2in <= 0 || c2in % 64 || !w2 || (((uintptr_t)x2 | (uintptr_t)w2) & 15))) return ODTK_E_INVALID;
+  if (dgrad && p.ldy != d->cout) return ODTK_E_UNSUPPORTED;   // the mask is read with the output's row stride
+  p.mask = (const __half *)mask;
 
   CUtensorMap tmA;
   const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
@@ -726,7 +748,7 @@ int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cud
     uint32_t boxW[2] = {64, (uint32_t)BN};
     if (!encode_map(&tmA2, x2, 2, dims, str, box) || !encode_map(&tmB2, w2, 2, dimsW, strW, boxW)) return ODTK_E_CUDA;
   }
-  return launch(p, BN, tmA, tmB, tmA2, tmB2, stream);
+  return launch(p, BN, tmA, tmB, tmA2, tmB2, stream, dgrad ? kOpF16Mask : kOpF16);
 }
 
 // odtk_conv2d_s8_ex: the same kernel on s8 operands, with the geometry of odtk_conv2d: 1x1 as GEMM rows (mode 0), 3x3 as
@@ -924,6 +946,11 @@ __global__ void pack_bias_kernel(const float *bias, __half *out, int cout) {
 
 extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
   return conv_run(d, nullptr, nullptr, 0, (cudaStream_t)stream_);
+}
+
+extern "C" int odtk_conv2d_dgrad(const odtk_conv_dgrad_t *d, odtk_stream_t stream_) {
+  if (!d) return ODTK_E_INVALID;
+  return conv_run(&d->base, nullptr, nullptr, 0, (cudaStream_t)stream_, true, d->mask);
 }
 
 extern "C" int odtk_conv2d_s8(const odtk_conv_s8_t *d, odtk_stream_t stream_) {

@@ -54,4 +54,7 @@ struct ConvParams {
   // fp32 addends of ODTK_OUT_NHWC_F32 (odtk_conv2d_f32): residual [M, ldr] at the output pixel, upsample
   // [N, up_h, up_w, Cout] at (h >> 1, w >> 1); NULL when absent
   const float *res32, *up32;
+  // input-gradient instance (odtk_conv2d_dgrad): NHWC fp16 [M, Cout] at the output pixel; an output element whose mask
+  // element is not > 0 becomes 0 (the ReLU derivative of the forward layer's input), or NULL
+  const __half *mask;
 };

@@ -834,3 +834,131 @@ def relu_from_view_f32(view):
     STATS["launches"] += 1
     _trace("relu_f32", 0, out.numel() * 8, n=n, h=h, w=w, cin=c)
     return out
+
+
+# ---- training: backward of the 3x3 stride-1 head convolutions -----------------------------------------------------------
+class WgradDesc(ctypes.Structure):
+    """odtk_wgrad_t (include/odtk_b200.h)."""
+    _fields_ = [("g", ctypes.c_void_p), ("x", ctypes.c_void_p), ("dw", ctypes.c_void_p), ("db", ctypes.c_void_p)] + \
+               [(f, ctypes.c_int) for f in ("n", "h", "width", "cin", "cout", "cout_pad")] + \
+               [("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int)]
+
+
+class GradLevel(ctypes.Structure):
+    """odtk_grad_level_t (include/odtk_b200.h)."""
+    _fields_ = [("grad", ctypes.c_void_p), ("height", ctypes.c_int), ("width", ctypes.c_int), ("row0", ctypes.c_int)]
+
+
+class ConvDgradDesc(ctypes.Structure):
+    """odtk_conv_dgrad_t (include/odtk_b200.h)."""
+    _fields_ = [("base", ConvDesc), ("mask", ctypes.c_void_p)]
+
+
+def pad64(c):
+    return (c + 63) // 64 * 64
+
+
+def _tab_px(n, h, w, tile_tab):
+    """Pixels a launch covers: n * h * w dense, or the pixels of the levels a tile table lists."""
+    if tile_tab is None:
+        return n * h * w
+    return n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
+
+
+def pack_weight_dgrad(weight, cout_pad=None):
+    """Weights of the input gradient of a 3x3 stride-1 convolution: [Cout, Cin, 3, 3] -> the forward convolution with Cin
+    outputs over Cout_pad inputs (pad_out zero-padded to a multiple of 64), rotated by 180 degrees:
+    w'[ci, co, ky, kx] = w[co, ci, 2 - ky, 2 - kx], packed like pack_weight ([Cin, 9 * Cout_pad] fp16)."""
+    cout, cin, kh, kw = weight.shape
+    assert kh == 3 and kw == 3
+    cout_pad = pad64(cout) if cout_pad is None else cout_pad
+    w = weight.detach().float()
+    if cout_pad > cout:
+        w = torch.cat([w, w.new_zeros((cout_pad - cout, cin, kh, kw))], dim=0)
+    out = pack_weight(w.transpose(0, 1).flip(2, 3))
+    _trace("pack_weight_dgrad", 0, weight.numel() * 4 + out.numel() * 2, cin=cin, cout=cout)
+    return out
+
+
+def conv_wgrad(g, x, cout, tile_tab=None, bias=True):
+    """Weight (and bias) gradient of a 3x3 stride-1 pad-1 convolution (odtk_conv_wgrad): g NHWC fp16 [N, H, W, Cout_pad]
+    (the gradient w.r.t. its output before the ReLU, zero outside the levels and in the channels >= cout), x NHWC fp16
+    [N, H, W, Cin] (its input).  tile_tab: both are whole atlases and only the listed tiles count.  Returns fp32
+    (dw [cout, Cin, 3, 3], db [cout] or None), bit-identical run to run."""
+    assert g.is_cuda and g.dtype == torch.float16 and g.is_contiguous()
+    assert x.is_cuda and x.dtype == torch.float16 and x.is_contiguous()
+    n, h, wd, cpad = g.shape
+    cin = x.shape[3]
+    assert tuple(x.shape[:3]) == (n, h, wd)
+    dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=g.device)
+    db = torch.empty((cout,), dtype=torch.float32, device=g.device) if bias else None
+    d = WgradDesc()
+    d.g, d.x, d.dw, d.db = g.data_ptr(), x.data_ptr(), dw.data_ptr(), (db.data_ptr() if db is not None else None)
+    d.n, d.h, d.width, d.cin, d.cout, d.cout_pad = n, h, wd, cin, cout, cpad
+    if tile_tab is not None:
+        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    L = _lib.lib()
+    size = _lib.check(L.odtk_conv_wgrad(ctypes.byref(d), None, 0, None), "conv_wgrad (workspace query)")
+    ws = torch.empty(int(size), dtype=torch.uint8, device=g.device)
+    _lib.check(L.odtk_conv_wgrad(ctypes.byref(d), ctypes.c_void_p(ws.data_ptr()), size, _stream()), "conv_wgrad")
+    STATS["launches"] += 1
+    if STATS["trace"] is not None:
+        px = _tab_px(n, h, wd, tile_tab)
+        # G once per output-channel tile row, X once per tap; the fp32 partials and the result
+        _trace("wgrad3x3", 2 * px * cout * 9 * cin, px * (cpad + cin) * 2 + int(size) * 2 + dw.numel() * 4,
+               n=n, h=h, w=wd, cin=cin, cout=cout)
+    return dw, db
+
+
+def grad_to_atlas(grads, rows0, scale, atlas):
+    """Per-level fp32 NCHW loss gradients [B, C, H_l, W_l] * scale (a number, or a one-element fp32 tensor on the atlas's
+    device, read there without a host sync) -> the fp16 NHWC gradient atlas [B, rows, width, C_pad]
+    (odtk_grad_to_atlas): level l at rows [rows0[l], + H_l), columns [0, W_l); channels >= C are written as 0; nothing
+    else is written (the caller's atlas is zero there).  fp16 overflow is +-inf."""
+    assert atlas.is_cuda and atlas.dtype == torch.float16 and atlas.is_contiguous()
+    b, rows, aw, cpad = atlas.shape
+    ch = grads[0].shape[1]
+    gs = [t.float().contiguous() for t in grads]
+    assert all(t.device == atlas.device for t in gs)
+    sc = (scale if torch.is_tensor(scale) else torch.tensor(float(scale))).to(atlas.device, torch.float32).reshape(1).contiguous()
+    levels = (GradLevel * len(gs))()
+    for l, (t, r0) in enumerate(zip(gs, rows0)):
+        assert t.shape[0] == b and t.shape[1] == ch
+        levels[l].grad, levels[l].height, levels[l].width, levels[l].row0 = t.data_ptr(), t.shape[2], t.shape[3], int(r0)
+    _lib.check(_lib.lib().odtk_grad_to_atlas(b, len(gs), ctypes.cast(levels, ctypes.c_void_p), ch, ctypes.c_void_p(sc.data_ptr()),
+                                             ctypes.c_void_p(atlas.data_ptr()), rows, aw, cpad, _stream()), "grad_to_atlas")
+    STATS["launches"] += 1
+    px = sum(t.shape[0] * t.shape[2] * t.shape[3] for t in gs)
+    _trace("grad_to_atlas", 0, px * ch * 4 + px * cpad * 2, n=b, h=rows, w=aw, cin=ch, cout=cpad)
+    return atlas
+
+
+def conv2d_dgrad(g, w, cout, mask=None, residual=None, tile_tab=None, out=None):
+    """Input gradient of a 3x3 stride-1 convolution (odtk_conv2d_dgrad): g NHWC fp16 [N, H, W, Cout_pad] convolved with
+    w = pack_weight_dgrad(weight) into NHWC fp16 [N, H, W, cout] (cout = the forward layer's Cin), + residual (same shape),
+    then zero wherever mask (NHWC fp16, same shape: the forward layer's input) is not > 0.  tile_tab: whole atlases, only
+    the listed tiles are written (`out` must then be zero outside them)."""
+    assert g.is_cuda and g.dtype == torch.float16 and g.is_contiguous()
+    assert w.device == g.device and w.dtype == torch.float16 and w.is_contiguous() and w.shape[1] == 9 * g.shape[3]
+    n, h, wd, cpad = g.shape
+    if out is None:
+        out = (torch.zeros if tile_tab is not None else torch.empty)((n, h, wd, cout), dtype=torch.float16, device=g.device)
+    for t in (mask, residual, out):
+        assert t is None or (t.device == g.device and t.dtype == torch.float16 and t.is_contiguous() and tuple(t.shape) == (n, h, wd, cout))
+    e = ConvDgradDesc()
+    d = e.base
+    d.x, d.w, d.y = g.data_ptr(), w.data_ptr(), out.data_ptr()
+    d.residual = residual.data_ptr() if residual is not None else None
+    if tile_tab is not None:
+        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cpad, cout, 3
+    d.out_mode = OUT_NHWC_F16
+    e.mask = mask.data_ptr() if mask is not None else None
+    _lib.check(_lib.lib().odtk_conv2d_dgrad(ctypes.byref(e), _stream()), "conv2d_dgrad")
+    STATS["launches"] += 1
+    if STATS["trace"] is not None:
+        px = _tab_px(n, h, wd, tile_tab)
+        _trace("dgrad3x3", 2 * px * cout * 9 * cpad,
+               px * cpad * 2 + w.numel() * 2 + px * cout * 2 * (1 + (mask is not None) + (residual is not None)),
+               n=n, h=h, w=wd, cin=cpad, cout=cout, residual=residual is not None, mask=mask is not None)
+    return out

@@ -189,6 +189,23 @@ class _Conv:
         return engine.conv2d(low, self.w, self.b, self.cout, 1, relu, residual, upsample, out_mode)
 
 
+class _HeadsTrain(torch.autograd.Function):
+    """(cls_loss, box_loss) of the training forward as a function of the head parameters (Model._train_forward /
+    Model._train_backward)."""
+
+    @staticmethod
+    def forward(ctx, model, x, targets, *params):
+        cls_loss, box_loss, state = model._train_forward(x, targets)
+        ctx.model, ctx.state = model, state
+        ctx.set_materialize_grads(False)       # a loss outside the graph gives None: its head gets no gradient
+        return cls_loss, box_loss
+
+    @staticmethod
+    def backward(ctx, g_cls, g_box):
+        grads = ctx.model._train_backward(ctx.state, g_cls, g_box, ctx.needs_input_grad[3:])
+        return (None, None, None) + tuple(grads)
+
+
 class Model:
     'RetinaNet - https://arxiv.org/abs/1708.02002 (reference: odtk/model.py:15-72)'
 
@@ -242,6 +259,17 @@ class Model:
         self._calib_hook = None
         self._calib_net = False       # calibration also records the network scope's tensors
         self._f32 = None              # full precision: split-TF32 weights of every layer (packed on first use)
+        self._params = None           # trainable head parameters (created by named_parameters / parameters)
+        self._param_versions = {}     # (head, layer index) -> the parameters' _version when their fp16 weights were packed
+        self._sd_versions = {}        # parameter name -> its _version when it was last copied into the state dict
+        self._dgrad_w = {}            # (head, layer index) -> (weight _version, input-gradient weights of pack_weight_dgrad)
+        self._fwd_gen = 0             # counts forward passes: a backward must follow its own forward
+        # test hooks, both only while want_atlas_grad is set: the training backward also computes d(loss)/d(atlas) into
+        # last_atlas_grad, which ALIASES a gradient buffer of the atlas geometry (the next backward overwrites it), and
+        # last_train keeps the last training forward's atlas views, head outputs and loss gradients
+        self.want_atlas_grad = False
+        self.last_train = None
+        self.last_atlas_grad = None
 
     def __repr__(self):
         return '\n'.join(['     model: {}'.format(self.name), '  backbone: {}'.format(self.backbone),
@@ -290,6 +318,8 @@ class Model:
         return model, state
 
     def state_dict(self):
+        """The reference's state_dict (CPU fp32 tensors); trained head parameters are copied in first."""
+        self._params_to_sd()
         return self._sd
 
     def load_state_dict(self, sd):
@@ -300,10 +330,84 @@ class Model:
         self._sd = {k: v.detach().float().cpu() for k, v in sd.items() if torch.is_tensor(v)}
         self._packed = None
         self._f32 = None
+        if self._params is not None:       # as nn.Module: the existing parameter tensors take the new values in place
+            with torch.no_grad():
+                for n, p in self._params.items():
+                    p.copy_(self._sd[n])
+            self._param_versions = {}
+            self._sd_versions = {n: p._version for n, p in self._params.items()}
         return self
+
+    # ---- trainable head parameters ----------------------------------------------------------------------------------
+    def _head_param_names(self):
+        return ["%s.%d.%s" % (head, i, k) for head in ("cls_head", "box_head") for i in (0, 2, 4, 6, 8) for k in ("weight", "bias")]
+
+    def named_parameters(self, prefix="", recurse=True):
+        """(name, parameter) of the class and box heads, with the reference's names, shapes and order
+        (cls_head.{0,2,4,6,8}.{weight,bias}, then box_head.*): fp32 CUDA leaf tensors, created from the state dict on the
+        first call (after .cuda()).  The backbone and the FPN are frozen: they have no backward kernels here and are not
+        listed.  Once the parameters exist, the training-mode forward returns losses connected to them (the head
+        backward runs on the sm_90a kernels: odtk_conv_wgrad, odtk_conv2d_dgrad), and every forward uses their current
+        values (the fp16 weights are repacked when a parameter changed, e.g. after optimizer.step())."""
+        if self._params is None:
+            if self._packed is None or self.device is None:
+                raise RuntimeError("call .cuda() before asking for parameters: they are CUDA tensors")
+            self._params = {n: torch.nn.Parameter(self._sd[n].to(self.device, torch.float32).clone())
+                            for n in self._head_param_names()}
+            self._param_versions = {(head, i): (self._params["%s.%d.weight" % (head, i)]._version,
+                                                self._params["%s.%d.bias" % (head, i)]._version)
+                                    for head in ("cls_head", "box_head") for i in (0, 2, 4, 6, 8)}
+            self._sd_versions = {n: p._version for n, p in self._params.items()}
+        for n, p in self._params.items():
+            yield prefix + n, p
+
+    def parameters(self, recurse=True):
+        for _, p in self.named_parameters():
+            yield p
+
+    def zero_grad(self, set_to_none=True):
+        for p in self.parameters():
+            if set_to_none:
+                p.grad = None
+            elif p.grad is not None:
+                p.grad.zero_()
+
+    def _params_to_sd(self):
+        """Copy every head parameter that changed since its last copy into the state dict (read by state_dict(), save()
+        and the fp32 / INT8 weight packing)."""
+        if self._params is not None:
+            for n, p in self._params.items():
+                if self._sd_versions.get(n) != p._version:
+                    self._sd[n] = p.detach().float().cpu().clone()
+                    self._sd_versions[n] = p._version
+
+    def _sync_params(self):
+        """Repack the fp16 weights of every head layer whose parameters changed since they were packed; counts the
+        forward pass."""
+        self._fwd_gen += 1
+        if self._params is None or self._packed is None:
+            return
+        P, changed = self._packed, False
+        for head in ("cls_head", "box_head"):
+            for k, i in enumerate((0, 2, 4, 6, 8)):
+                w, b = self._params["%s.%d.weight" % (head, i)], self._params["%s.%d.bias" % (head, i)]
+                v = (w._version, b._version)
+                if self._param_versions.get((head, i)) != v:
+                    with torch.no_grad():
+                        P[head][k] = _Conv(w.detach(), b.detach().clone(), 1, self.device)
+                    self._param_versions[(head, i)] = v
+                    changed = True
+        if changed:
+            self._f32 = None
+            if self._int8 is not None:
+                self._params_to_sd()
+                self._pack_int8()
+            if getattr(self, "_graphs", None):
+                self._graphs = {}
 
     def cuda(self, device=None):
         self.device = torch.device("cuda", torch.cuda.current_device() if device is None else device)
+        self._params_to_sd()
         self._pack()
         return self
 
@@ -318,10 +422,11 @@ class Model:
         return self
 
     def train(self, mode=True):
-        """Training-mode forward (odtk/model.py:130-138): `model([images, targets])` returns (cls_loss, box_loss).  The
-        convolutions have no backward kernels here (the training loop is outside the hot path): the
-        losses and -- `_compute_loss(..., with_grad=True)` -- their gradients w.r.t. the head outputs are what this
-        provides."""
+        """Training-mode forward (odtk/model.py:130-138): `model([images, targets])` returns (cls_loss, box_loss).  Once
+        the head parameters exist (named_parameters / parameters), the losses are connected to them and .backward()
+        fills their .grad on the sm_90a backward kernels; the backbone and the FPN are frozen (no backward kernels).
+        Without them, the losses and -- `_compute_loss(..., with_grad=True)` -- their gradients w.r.t. the head outputs
+        are what this provides.  The training forward runs in fp16 over the pyramid atlas whatever set_precision chose."""
         self.training = bool(mode)
         return self
 
@@ -497,6 +602,7 @@ class Model:
 
     def _f32_layers(self):
         if self._f32 is None:
+            self._params_to_sd()          # trained head parameters
             self._f32 = self._pack_f32()
         return self._f32
 
@@ -1082,6 +1188,7 @@ class Model:
         (sigmoid) class maps [B, A*C, H, W] and box maps [B, A*4|6, H, W], fp32 NCHW."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
+        self._sync_params()
         if self._full_precision():
             return self._heads(self._features_f32(*self._input_f32(x)), sigmoid)
         return self._heads(self._features(self._stem(self._to_nhwc_half(x))), sigmoid)
@@ -1193,9 +1300,96 @@ class Model:
             box_tgt.append(bt)
         return loss_mod.retina_loss(cls_heads, box_heads, cls_idx, box_tgt, self.classes, with_grad=with_grad)
 
+    # ---- training the heads: forward with saved tower outputs, backward on odtk_conv_wgrad / odtk_conv2d_dgrad ----------
+    def _train_forward(self, x, targets):
+        """Training forward of the heads over the pyramid atlas with every tower output kept (the inference path
+        ping-pongs two buffers) and the loss gradients from the same odtk_retina_loss launch.  Returns the two losses
+        and the state the backward needs."""
+        if self._packed is None:
+            raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
+        views = self._features(self._stem(self._to_nhwc_half(x)))
+        if not isinstance(views[0], engine.AtlasView):
+            raise ValueError("training the heads runs over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0) or the "
+                             "backbone does not use it")
+        P = self._packed
+        atlas0 = views[0].atlas
+        at = self._atlas_for(atlas0.shape[0], tuple((v.h, v.w) for v in views), atlas0.device)
+        if "train" not in at:        # zero-initialised once: gap rows / columns are never written
+            at["train"] = {h: [torch.zeros_like(atlas0) for _ in range(4)] for h in ("cls_head", "box_head")}
+        outs = {}
+        for head in ("cls_head", "box_head"):
+            t = atlas0
+            for i, conv in enumerate(P[head][:-1]):
+                conv(t, relu=True, out=at["train"][head][i], tile_tab=at["tab"], valid_px=at["px"])
+                t = at["train"][head][i]
+            outs[head] = [P[head][-1](engine.AtlasView(t, at["rows"][l], v.h, v.w), out_mode=engine.OUT_NCHW_F32)
+                          for l, v in enumerate(views)]
+        cls_loss, box_loss, cls_grads, box_grads = self._compute_loss(x, outs["cls_head"], outs["box_head"], targets,
+                                                                      with_grad=True)
+        state = {"gen": self._fwd_gen, "at": at, "views": views, "heads": outs,
+                 "grads": {"cls_head": cls_grads, "box_head": box_grads}}
+        self.last_train = state if self.want_atlas_grad else None
+        return cls_loss.clone(), box_loss.clone(), state
+
+    def _train_backward(self, state, g_cls, g_box, needs):
+        """Gradients of the head parameters (None where `needs` is False) for upstream gradients g_cls / g_box of the two
+        losses.  Per head, from the last layer down: the loss gradients times the upstream factor into the fp16 gradient
+        atlas, then per layer the weight / bias gradient (odtk_conv_wgrad) and the input gradient masked by the ReLU of
+        the layer's input (odtk_conv2d_dgrad).  The first tower layer's input gradient, d(atlas), is only computed when
+        want_atlas_grad is set (the box tower's with the class tower's as its residual addend)."""
+        if state["gen"] != self._fwd_gen:
+            raise RuntimeError("the model ran another forward pass after this training forward: its saved activations "
+                               "are gone; call backward() before the next forward")
+        at, tab = state["at"], state["at"]["tab"]
+        P, params = self._packed, self._params
+        names = list(params)
+        need = dict(zip(names, needs))
+        got = {}
+        atlas0 = state["views"][0].atlas
+        if "gbuf" not in at:
+            at["gbuf"] = [torch.zeros_like(atlas0) for _ in range(4)]    # tower gradient ping-pong + d(atlas) (cls, sum)
+        gbuf, d_atlas = at["gbuf"], None
+        want_atlas = self.want_atlas_grad
+        for head, g in (("cls_head", g_cls), ("box_head", g_box)):
+            lname = ["%s.%d" % (head, i) for i in (0, 2, 4, 6, 8)]
+            needed = [need[n + ".weight"] or need[n + ".bias"] for n in lname]
+            if g is None or not (any(needed) or want_atlas):
+                continue
+            cpad = engine.pad64(P[head][-1].cout)
+            key = "grad%d" % cpad
+            if key not in at:
+                at[key] = torch.zeros(atlas0.shape[:3] + (cpad,), dtype=torch.float16, device=atlas0.device)
+            G = engine.grad_to_atlas(state["grads"][head], at["rows"], g, at[key])   # g stays on the device: no sync
+            inputs = [atlas0] + at["train"][head]
+            for k in range(4, -1, -1):
+                wn, bn = lname[k] + ".weight", lname[k] + ".bias"
+                if need[wn] or need[bn]:
+                    dw, db = engine.conv_wgrad(G, inputs[k], P[head][k].cout, tile_tab=tab, bias=need[bn])
+                    if need[wn]:
+                        got[wn] = dw
+                    if need[bn]:
+                        got[bn] = db
+                if not (want_atlas or any(needed[:k])):
+                    break
+                cached = self._dgrad_w.get((head, k))
+                if cached is None or cached[0] != (params[wn]._version, id(params[wn])):
+                    cached = self._dgrad_w[(head, k)] = ((params[wn]._version, id(params[wn])),
+                                                         engine.pack_weight_dgrad(params[wn], cpad if k == 4 else 256))
+                wpk = cached[1]
+                if k > 0:
+                    G = engine.conv2d_dgrad(G, wpk, 256, mask=inputs[k], tile_tab=tab, out=gbuf[k & 1])
+                else:
+                    d_atlas = engine.conv2d_dgrad(G, wpk, 256, residual=d_atlas, tile_tab=tab,
+                                                  out=gbuf[2] if d_atlas is None else gbuf[3])
+        self.last_atlas_grad = d_atlas if want_atlas else None
+        return [got.get(n) for n in names]
+
     def forward(self, x, rotated_bbox=None):
+        self._sync_params()
         if self.training:
             x, targets = x
+            if self._params is not None and torch.is_grad_enabled() and any(p.requires_grad for p in self._params.values()):
+                return _HeadsTrain.apply(self, x, targets.float().to(x.device), *self._params.values())
             cls_heads, box_heads = self.forward_heads(x, sigmoid=False)
             return self._compute_loss(x, cls_heads, box_heads, targets.float().to(cls_heads[0].device))
         if self.fused_candidates and not self.exporting:
@@ -1240,6 +1434,7 @@ class Model:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
         if self.training or self.exporting:
             raise RuntimeError("forward_images runs inference: call .eval() and leave exporting off")
+        self._sync_params()
         plan = engine.ResizePlan(engine.image_shapes(images), resize, max_size, self.stride, canvas)
         hs, ws = plan.canvas
         if getattr(self, "_graphs", None) is None:
@@ -1300,6 +1495,7 @@ class Model:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
         if self.training or self.exporting:
             raise RuntimeError("forward_jpeg runs inference: call .eval() and leave exporting off")
+        self._sync_params()
         batch = jpeg.JpegBatch(datas)
         plan = engine.ResizePlan(batch.shapes, resize, max_size, self.stride, canvas)
         hs, ws = plan.canvas
@@ -1391,5 +1587,6 @@ class Model:
 
     def __call__(self, x, rotated_bbox=None, static_input=False):
         if getattr(self, "_graphs", None) is not None and not self.exporting and not self.training:
+            self._sync_params()
             return self._forward_graphed(x, rotated_bbox, static_input)
         return self.forward(x, rotated_bbox)

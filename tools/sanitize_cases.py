@@ -10,7 +10,8 @@ by the epilogues), the s8 instantiation of the conv kernel (stride 2 in modes 3 
 input and output) and the INT8 heads and network scope of the model, the split-TF32 fp32 instantiation (`fp32`: modes 0 / 1 / 2 /
 3, N tiles 64 / 128, several tiles per CTA so the A_lo side buffers and the named barrier cycle, tile table and level views,
 fp32 addends, NCHW / sigmoid / candidate epilogues, the fp32 small kernels, the fp32 model), decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
-iou, target assignment, the cooperative loss kernel."""
+iou, target assignment, the cooperative loss kernel, and head training (`train`: the weight-gradient kernel, the bias-gradient
+and reduce kernels, the gradient atlas, the masked input-gradient conv instance, one SGD step of the model)."""
 import os
 import sys
 
@@ -109,8 +110,42 @@ def fp32_cases():
             print("model fp32 rotated=%s fused=%s detections=%d" % (rotated, fused, int((out[0] > 0).sum())), flush=True)
 
 
+def train_cases():
+    """Head training: wgrad_kernel (TMA / mbarrier ring, split-K partial writes, an output tile with no second 64-channel
+    G box, a dense image without tile table), bgrad_partial / wgrad_reduce, grad_to_atlas_kernel, the kOpF16Mask conv
+    instance with its mask and residual reads in tile-table mode, and one SGD step of the model."""
+    from retinanet_examples_b200.model import Model as M
+    at = M("ResNet18FPN", classes=1)._atlas_for(2, ((16, 24), (8, 12), (4, 6), (2, 3), (1, 2)), torch.device(DEV))
+    n, ha, wa = at["buf"][0].shape[:3]
+    for cout in (256, 36):
+        cpad = engine.pad64(cout)
+        gg, xx = rnd(n, ha, wa, cpad, scale=0.1), rnd(n, ha, wa, 256)
+        engine.conv_wgrad(gg, xx, cout, tile_tab=at["tab"])
+        engine.conv_wgrad(gg, xx, cout)
+        wd = engine.pack_weight_dgrad(torch.randn((cout, 256, 3, 3), generator=g).to(DEV) * 0.02, cpad)
+        a = engine.conv2d_dgrad(gg, wd, 256, mask=xx, tile_tab=at["tab"])
+        engine.conv2d_dgrad(gg, wd, 256, residual=a, tile_tab=at["tab"])
+        torch.cuda.synchronize()
+        print("wgrad / dgrad cout=%d ok" % cout, flush=True)
+    grads = [torch.randn((2, 54, h, w), generator=g).to(DEV) for h, w in ((16, 24), (8, 12), (4, 6), (2, 3), (1, 2))]
+    engine.grad_to_atlas(grads, at["rows"], 3.0, torch.zeros((n, ha, wa, 64), dtype=torch.float16, device=DEV))
+    sd = make_state_dict("ResNet18FPN", 3, 9, False, seed=1)
+    m = Model("ResNet18FPN", classes=3).load_state_dict(sd).cuda(0)
+    opt = torch.optim.SGD(m.parameters(), lr=0.01, momentum=0.9)
+    m.train()
+    x = torch.randn((2, 3, 128, 256), generator=g).to(DEV)
+    t = torch.tensor([[[20., 30., 60., 40., 1.], [100., 10., 50., 90., 2.]], [[5., 5., 100., 100., 0.], [-1.] * 5]]).to(DEV)
+    cls_loss, box_loss = m([x, t])
+    ((cls_loss + box_loss) * 1024.0).backward()
+    opt.step()
+    torch.cuda.synchronize()
+    print("train step ok", flush=True)
+
+
 def main():
     only = sys.argv[1] if len(sys.argv) > 1 else ""
+    if only in ("", "train"):
+        train_cases()
     if only in ("", "conv"):
         conv(2, 16, 16, 64, 64, 1, relu=True)                              # mode 0
         conv(2, 16, 16, 256, 256, 1, relu=True, residual=True)             # residual epilogue
