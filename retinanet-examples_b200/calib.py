@@ -30,18 +30,15 @@ def network_tensors(backbone):
     block of layer3 / layer4 its convolutions' ReLU outputs except the last, its downsample output (first block) and the
     block output, then P5, P4 and P3 (lateral5, and lateral4 / lateral3 after the top-down add).  ValueError for a backbone
     the scope does not cover (ResNeXt's grouped 3x3, MobileNetV2)."""
-    from .model import RESNET_LAYERS, RESNEXT
+    from .model import RESNET_LAYERS, RESNEXT, network_walk
     if backbone not in RESNET_LAYERS or backbone in RESNEXT:
         raise ValueError("INT8 network scope covers the ResNet18/34/50/101/152 FPN backbones, not %r" % (backbone,))
-    block, layers = RESNET_LAYERS[backbone]
-    f = "backbones.%s.features." % backbone
-    names = [f + "layer2"]
-    convs = ("conv1", "conv2") if block == "bottleneck" else ("conv1",)
-    for li in (3, 4):
-        for b in range(layers[li - 1]):
-            p = f + "layer%d.%d" % (li, b)
-            names += [p + "." + c for c in convs] + ([p + ".downsample"] if b == 0 else []) + [p]
-    return names + ["backbones.%s.lateral%d" % (backbone, k) for k in (5, 4, 3)]
+    walk = network_walk(backbone)
+    names = ["backbones.%s.features.layer2" % backbone]
+    for blk in walk["blocks"]:
+        if blk["level"] >= 4:
+            names += [c["y"] for c in blk["convs"][:-1]] + ([blk["down"]["y"]] if blk["down"] else []) + [blk["convs"][-1]["y"]]
+    return names + [walk["lateral%d" % k]["y"] for k in (5, 4, 3)]
 
 
 def max_threshold(absmax):

@@ -509,6 +509,22 @@ void launch_bn(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUte
   cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, OP>, tmA, tmB, tmA2, tmB2, p);
 }
 
+// Every compile-time instance of conv_gemm_kernel: N tile, operand type, launcher and dynamic shared memory.
+struct Instance {
+  int bn, op;
+  const void *fn;
+  void (*launch)(int, cudaStream_t, const CUtensorMap &, const CUtensorMap &, const CUtensorMap &, const CUtensorMap &,
+                 const ConvParams &);
+  int smem;
+};
+template <int BN, int OP>
+constexpr Instance instance() {
+  return {BN, OP, (const void *)conv_gemm_kernel<BN, OP>, launch_bn<BN, OP>, OP == kOpTF32x3 ? kSmemBytesF32 : kSmemBytes};
+}
+const Instance kInstances[] = {instance<64, kOpF16>(),     instance<128, kOpF16>(),     instance<64, kOpS8>(),
+                               instance<128, kOpS8>(),     instance<64, kOpTF32x3>(),   instance<128, kOpTF32x3>(),
+                               instance<64, kOpF16Mask>(), instance<128, kOpF16Mask>()};
+
 // Per-device state (one process may drive several GPUs): the > 48 KB dynamic-shared-memory opt-in of every kernel
 // instance is a per-device function attribute.
 constexpr int kMaxDevices = 64;
@@ -520,49 +536,32 @@ bool device_ready() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return false;
   std::lock_guard<std::mutex> lk(g_dev_mu);
   if (g_dev_ready[dev]) return true;
-  if (cudaFuncSetAttribute(conv_gemm_kernel<64, kOpF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<64, kOpS8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpS8>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<64, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpTF32x3>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytesF32) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<64, kOpF16Mask>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess ||
-      cudaFuncSetAttribute(conv_gemm_kernel<128, kOpF16Mask>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes) != cudaSuccess)
-    return false;
+  for (const Instance &k : kInstances)
+    if (cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem) != cudaSuccess) return false;
   g_dev_ready[dev] = true;
   return true;
 }
 
 thread_local odtk_conv_plan_t g_last_plan;
 
-void set_stages(ConvParams &p, int BN, int op = kOpF16) {
+void set_stages(ConvParams &p, int BN, int op) {
   p.nstages = kPipeBytes / ((128 + (op == kOpTF32x3 ? 2 * BN : BN)) * p.row_bytes);
   if (p.nstages > kMaxStages) p.nstages = kMaxStages;
 }
 
 int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
-           const CUtensorMap &tmB2, cudaStream_t stream, int op = kOpF16) {
+           const CUtensorMap &tmB2, cudaStream_t stream, int op) {
   const int total = p.num_m_tiles * p.num_n_tiles;
   const int sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
   const int grid = total < sms ? total : sms;
   g_last_plan = odtk_conv_plan_t{p.mode, 0, BN, p.num_m_tiles, p.num_n_tiles, p.nstages, 0, 0, 0, 0, 0, 0, p.TH, p.TW, grid, 0};
-  {
-    OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    if (op == kOpS8) {
-      if (BN == 64) launch_bn<64, kOpS8>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-      else          launch_bn<128, kOpS8>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-    } else if (op == kOpTF32x3) {
-      if (BN == 64) launch_bn<64, kOpTF32x3>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-      else          launch_bn<128, kOpTF32x3>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-    } else if (op == kOpF16Mask) {
-      if (BN == 64) launch_bn<64, kOpF16Mask>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-      else          launch_bn<128, kOpF16Mask>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-    } else {
-      if (BN == 64) launch_bn<64, kOpF16>(grid, stream, tmA, tmB, tmA2, tmB2, p);
-      else          launch_bn<128, kOpF16>(grid, stream, tmA, tmB, tmA2, tmB2, p);
+  for (const Instance &k : kInstances)
+    if (k.bn == BN && k.op == op) {
+      OdtkProfScope prof(ODTK_PROF_CONV, stream);
+      k.launch(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
     }
-  }
-  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+  return ODTK_E_UNSUPPORTED;
 }
 
 // out_mode ODTK_OUT_CANDIDATES: the decode workspace of the level the launch covers
@@ -577,13 +576,16 @@ int set_sink(ConvParams &p, const odtk_cand_sink_t *k, int cout, int h, int widt
   return ODTK_OK;
 }
 
+CUtensorMapDataType map_type(int es) {
+  return es == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+}
+
 // A operand of a 1x1 / 3x3, stride 1 / 2 launch: the mode, the output patch and tile grid, and the tensor map of x (the
 // top-left h x width rectangle of images xH x xW pixels apart).  es: bytes per element, 2 (fp16), 1 (s8) or 4 (fp32); a K
-// block is one 128-byte swizzle row of channels either way.  Shared by odtk_conv2d, odtk_conv2d_s8_ex and odtk_conv2d_f32.
+// block is one 128-byte swizzle row of channels either way.
 int a_operand(ConvParams &p, CUtensorMap &tmA, const void *x, int n, int h, int width, int cin, int ksize, int stride,
-              uint64_t xH, uint64_t xW, bool x_view, const void *tile_tab, int tab_tiles, bool upsample, int es) {
-  const CUtensorMapDataType dt = es == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
-                                : es == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+              uint64_t xH, uint64_t xW, bool x_view, const void *tile_tab, int tab_tiles, int es) {
+  const CUtensorMapDataType dt = map_type(es);
   const uint32_t kc = 128 / es;   // channels per K block
   const uint64_t C = (uint64_t)cin, W = (uint64_t)width, H = (uint64_t)h;
   if (stride == 2 && ((h & 1) || (width & 1) || x_view)) {
@@ -610,7 +612,6 @@ int a_operand(ConvParams &p, CUtensorMap &tmA, const void *x, int n, int h, int 
     // stride-2 1x1 / 3x3 (pad ksize/2) on even-sized inputs: 5-D parity-split view of the NHWC tensor
     // {2C (column parity x channel), W/2, 2 (row parity), H/2, N}; out-of-range half-rows/columns
     // (the -1 of the top/left taps) are zero-filled by the TMA unit == padding.
-    if (upsample) return ODTK_E_UNSUPPORTED;
     const int OH = h / 2, OW = width / 2;
     p.mode = 3;
     p.H = OH; p.W = OW;
@@ -650,282 +651,194 @@ int a_operand(ConvParams &p, CUtensorMap &tmA, const void *x, int n, int h, int 
   return ODTK_OK;
 }
 
-// odtk_conv2d, plus (mode 0 only) a second operand pair added to the same accumulator: y = x * w^T + x2 * w2^T with
-// x2 [M, c2in], w2 [cout, c2in] (the projected identity of a bottleneck block).  dgrad: odtk_conv2d_dgrad (the masked
-// instance; a tile-table launch may then take a residual, a whole atlas like y).
-int conv_run(const odtk_conv_t *d, const void *x2, const void *w2, int c2in, cudaStream_t stream, bool dgrad = false,
-             const void *mask = nullptr) {
-  if (!d || !d->x || !d->w) return ODTK_E_INVALID;
-  if (dgrad && (d->ksize != 3 || d->stride > 1 || d->out_mode != ODTK_OUT_NHWC_F16 || d->relu || d->groups > 1 || d->upsample ||
-                d->x_rows > 0 || d->x_width > 0 || d->y_rows > 0 || d->y_width > 0 || d->y_row_off > 0))
+// A operand of the ResNet stem (mode 2): 7x7 stride-2 pad-3 over the image zero-padded to NHWC4 [n, h+6, width+8, 4], im2col-
+// free.  For filter row r the A operand of output pixels (oh, ow..) is the 8-pixel x 4-channel window starting at padded
+// pixel (2*oh + r, 2*ow): 32 elements, consecutive output pixels 8 elements apart -- an OVERLAPPING-window 5-D tensor map
+// {32 elements, OW, 7 rows (one padded row), OH (two padded rows), N}.  One window row is one swizzle row: 64 bytes in
+// fp16, 128 in fp32; K = 7 blocks of 32.
+int stem_operand(ConvParams &p, CUtensorMap &tmA, const void *xp, int n, int h, int width, int es) {
+  const int OH = (h - 1) / 2 + 1, OW = (width - 1) / 2 + 1;
+  const uint64_t HP = (uint64_t)h + 6, WP = (uint64_t)width + 8;
+  p.mode = 2;
+  p.H = OH; p.W = OW; p.Cin = 4;
+  p.kw = 1; p.taps = 7; p.pad = 0; p.kblocks_per_tap = 1;
+  p.row_bytes = 32 * es;
+  p.M = (long long)n * OH * OW;
+  choose_patch(OH, OW, p.TH, p.TW);
+  p.tiles_h = (OH + p.TH - 1) / p.TH;
+  p.tiles_w = (OW + p.TW - 1) / p.TW;
+  p.num_m_tiles = n * p.tiles_h * p.tiles_w;
+  uint64_t dims[5] = {32, (uint64_t)OW, 7, (uint64_t)OH, (uint64_t)n};
+  uint64_t str[4] = {8 * (uint64_t)es, WP * 4 * es, WP * 8 * es, HP * WP * 4 * es};
+  uint32_t box[5] = {32, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
+  if (!encode_map(&tmA, xp, 5, dims, str, box, es == 4 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B, nullptr,
+                  map_type(es)))
     return ODTK_E_UNSUPPORTED;
-  if (mask && ((uintptr_t)mask & 3)) return ODTK_E_INVALID;
-  if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
-  if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
-  if (d->ksize != 1 && d->ksize != 3) return ODTK_E_UNSUPPORTED;
-  if (d->cin % 64 != 0) return ODTK_E_UNSUPPORTED;  // 64-channel K blocks (128-byte swizzle rows)
-  const int groups = d->groups > 1 ? d->groups : 1;
+  return ODTK_OK;
+}
+
+// B operand: weights [cout, K] in boxes of one swizzle row (p.row_bytes) x BN output channels
+bool b_operand(CUtensorMap &tmB, const void *w, uint64_t K, int cout, int BN, int row_bytes, int es) {
+  uint64_t dims[2] = {K, (uint64_t)cout};
+  uint64_t str[1] = {K * es};
+  uint32_t box[2] = {(uint32_t)(row_bytes / es), (uint32_t)BN};
+  return encode_map(&tmB, w, 2, dims, str, box, row_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_128B,
+                    nullptr, map_type(es));
+}
+
+// What differs between the operand types of the convolution entry points; a K block is one 128-byte row of 128 / es
+// channels, so Cin must be a multiple of that.
+struct OpSpec {
+  int op;           // conv_gemm_kernel instance
+  int es;           // bytes per activation / weight element
+  int nhwc_mode;    // the NHWC output mode; the others are ODTK_OUT_NCHW_F32[_SIGMOID] and ODTK_OUT_CANDIDATES
+  int nhwc_cout;    // Cout multiple of NHWC outputs
+  int ldy_mult;     // output row stride multiple of NHWC outputs
+  int addend_align; // byte alignment of the residual / upsample addends
+  bool relu6;       // relu 2 (ReLU6, NHWC output only) allowed; otherwise relu is 0 or 1
+};
+constexpr OpSpec kSpecF16 = {kOpF16, 2, ODTK_OUT_NHWC_F16, 16, 8, 4, true};
+constexpr OpSpec kSpecS8 = {kOpS8, 1, ODTK_OUT_NHWC_S8, 16, 1, 2, false};
+constexpr OpSpec kSpecF32 = {kOpTF32x3, 4, ODTK_OUT_NHWC_F32, 2, 2, 8, false};
+
+// The fields of odtk_conv_t, odtk_conv_s8_ex_t and odtk_conv_f32_t in one place, plus the fp16-only extras: a second
+// operand pair (mode 0) added to the same accumulator, y = x * w^T + x2 * w2^T with x2 [M, c2in], w2 [cout, c2in] (the
+// projected identity of a bottleneck block), and the input-gradient launch (odtk_conv2d_dgrad: the masked instance; a
+// tile-table launch may then take a residual, a whole atlas like y).
+struct ConvArgs {
+  const void *x, *w, *w_lo, *residual, *upsample, *x2, *w2, *mask, *tile_tab;
+  const float *bias, *alpha;
+  void *y;
+  const odtk_cand_sink_t *sink;
+  int n, h, width, cin, cout, ksize, stride, relu, out_mode, ldy, ldr, groups, c2in, tab_tiles;
+  int x_rows, x_width, y_rows, y_row_off, y_width;
+  float inv_out_scale, res_scale, up_scale;
+  bool dgrad;
+};
+
+// One convolution on conv_gemm_kernel: 1x1 as GEMM rows (mode 0), 3x3 as shifted boxes (mode 1) over a dense tensor, a
+// level view of the atlas or the whole atlas with its tile table, stride 2 on the parity-split view (mode 3, even sizes) or
+// element-strided boxes (odd sizes, level views), and in fp32 the 7x7 stem (mode 2).  NHWC outputs may add a residual and /
+// or a nearest-upsampled addend, and may land in a level view of an atlas.  Every argument is checked before any CUDA call.
+int conv_run(const ConvArgs &a, const OpSpec &s, cudaStream_t stream) {
+  if (!a.x || !a.w || (s.op == kOpS8 && !a.alpha) || (s.op == kOpTF32x3 && !a.w_lo)) return ODTK_E_INVALID;
+  if (a.dgrad && (a.ksize != 3 || a.stride > 1 || a.out_mode != ODTK_OUT_NHWC_F16 || a.relu || a.groups > 1 || a.upsample ||
+                  a.x_rows > 0 || a.x_width > 0 || a.y_rows > 0 || a.y_width > 0 || a.y_row_off > 0))
+    return ODTK_E_UNSUPPORTED;
+  if (a.mask && ((uintptr_t)a.mask & 3)) return ODTK_E_INVALID;
+  if (a.out_mode == ODTK_OUT_CANDIDATES ? !a.sink : !a.y) return ODTK_E_INVALID;
+  if (a.n <= 0 || a.h <= 0 || a.width <= 0 || a.cin <= 0 || a.cout <= 0) return ODTK_E_INVALID;
+  if (a.out_mode != s.nhwc_mode && a.out_mode != ODTK_OUT_NCHW_F32 && a.out_mode != ODTK_OUT_NCHW_F32_SIGMOID &&
+      a.out_mode != ODTK_OUT_CANDIDATES)
+    return ODTK_E_INVALID;
+  const int stride = a.stride > 1 ? a.stride : 1;
+  const bool stem = s.op == kOpTF32x3 && a.ksize == 7;   // the fp32 ResNet stem over the NHWC4 image
+  const int kc = 128 / s.es;                              // channels per K block
+  if (stem ? (a.cin != 3 || stride != 2) : ((a.ksize != 1 && a.ksize != 3) || a.cin % kc)) return ODTK_E_UNSUPPORTED;
+  const int groups = a.groups > 1 ? a.groups : 1;
   if (groups > 1) {
     // grouped convolution (ResNeXt conv2): output block j of 64 channels depends only on input chunk j, as long as a
     // group never straddles a 64-channel chunk; `w` is then [cout, ksize*ksize*64], block-diagonal inside the chunk
-    if (d->cin != d->cout || d->cin % groups || 64 % (d->cin / groups) || d->residual || d->upsample || d->ksize != 3 ||
-        d->out_mode != ODTK_OUT_NHWC_F16)
+    if (a.cin != a.cout || a.cin % groups || 64 % (a.cin / groups) || a.residual || a.upsample || a.ksize != 3 ||
+        a.out_mode != ODTK_OUT_NHWC_F16)
       return ODTK_E_UNSUPPORTED;
   }
-  if (d->out_mode < 0 || d->out_mode > 3) return ODTK_E_INVALID;
-  if (d->relu == 2 && d->out_mode != ODTK_OUT_NHWC_F16) return ODTK_E_UNSUPPORTED;   // ReLU6 only on fp16 activations
-  if (d->out_mode == ODTK_OUT_NHWC_F16 && (d->cout % 16)) return ODTK_E_UNSUPPORTED;
-  if (d->out_mode != ODTK_OUT_NHWC_F16 && (d->residual || d->upsample)) return ODTK_E_UNSUPPORTED;
-  if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  if (((uintptr_t)d->x | (uintptr_t)d->w | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15) return ODTK_E_INVALID;
-  if ((d->residual && ((uintptr_t)d->residual & 3)) || (d->upsample && ((uintptr_t)d->upsample & 3))) return ODTK_E_INVALID;
+  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
+  if (s.relu6 ? (a.relu == 2 && a.out_mode != s.nhwc_mode) : (a.relu != 0 && a.relu != 1)) return ODTK_E_UNSUPPORTED;
+  const bool nhwc = a.out_mode == s.nhwc_mode;
+  if (nhwc && (a.cout % s.nhwc_cout)) return ODTK_E_UNSUPPORTED;
+  if ((long long)a.n * a.h * a.width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  if (((uintptr_t)a.x | (uintptr_t)a.w | (uintptr_t)a.w_lo | (a.out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)a.y)) & 15)
+    return ODTK_E_INVALID;
+  // strided views: the input / output may be a rectangle of a larger NHWC buffer (a level of the pyramid atlas)
+  const uint64_t xH = a.x_rows > 0 ? (uint64_t)a.x_rows : (uint64_t)a.h, xW = a.x_width > 0 ? (uint64_t)a.x_width : (uint64_t)a.width;
+  const bool x_view = xH != (uint64_t)a.h || xW != (uint64_t)a.width;
+  const bool y_view = a.y_rows > 0 || a.y_width > 0 || a.y_row_off > 0;
+  const bool addend = a.residual || a.upsample;
+  // addends and output views need the NHWC output; views and tile tables are 3x3 without addends
+  if ((addend || y_view) && !nhwc) return ODTK_E_UNSUPPORTED;
+  if ((x_view || y_view || (a.tile_tab && !a.dgrad)) && (a.ksize != 3 || addend)) return ODTK_E_UNSUPPORTED;
+  if ((stem && addend) || (a.upsample && stride != 1)) return ODTK_E_UNSUPPORTED;
+  if (a.tile_tab && (a.tab_tiles <= 0 || x_view || y_view || stride != 1)) return ODTK_E_INVALID;
+  if ((((uintptr_t)a.residual | (uintptr_t)a.upsample) & (s.addend_align - 1)) || (a.upsample && ((a.h & 1) || (a.width & 1))))
+    return ODTK_E_INVALID;
+  const int ldy = a.ldy > 0 ? a.ldy : a.cout, ldr = a.ldr > 0 ? a.ldr : a.cout;
+  if ((nhwc && ldy % s.ldy_mult) || (a.residual && (ldr & 1))) return ODTK_E_INVALID;
+  if (a.x2 && (a.ksize != 1 || stride != 1 || a.c2in <= 0 || a.c2in % 64 || !a.w2 || (((uintptr_t)a.x2 | (uintptr_t)a.w2) & 15)))
+    return ODTK_E_INVALID;
+  if (a.dgrad && ldy != a.cout) return ODTK_E_UNSUPPORTED;   // the mask is read with the output's row stride
   if (!device_ready()) return ODTK_E_CUDA;
-  const int sms = odtk_sm_count();
+  const int op = a.dgrad ? kOpF16Mask : s.op;
   ConvParams p;
   memset(&p, 0, sizeof p);
-  p.N = d->n; p.H = d->h; p.W = d->width; p.Cin = d->cin; p.Cout = d->cout;
-  p.kw = d->ksize; p.taps = d->ksize * d->ksize; p.pad = d->ksize / 2;
-  p.kblocks_per_tap = groups > 1 ? 1 : d->cin / 64;
+  p.N = a.n; p.H = a.h; p.W = a.width; p.Cin = a.cin; p.Cout = a.cout;
+  p.kw = a.ksize; p.taps = a.ksize * a.ksize; p.pad = a.ksize / 2;
+  p.kblocks_per_tap = groups > 1 ? 1 : a.cin / kc;
   p.grouped = groups > 1;
   p.row_bytes = 128;
-  p.M = (long long)d->n * d->h * d->width;
-  p.bias = d->bias;
-  p.residual = (const __half *)d->residual;
-  p.upsample = (const __half *)d->upsample;
-  p.out = d->y;
-  p.relu = d->relu;
-  p.out_mode = d->out_mode;
-  p.ldy = d->ldy > 0 ? d->ldy : d->cout;
-  p.ldr = d->ldr > 0 ? d->ldr : d->cout;
-  p.up_h = d->h / 2; p.up_w = d->width / 2;
+  p.M = (long long)a.n * a.h * a.width;
+  p.bias = a.bias;
+  p.out = a.y;
+  p.relu = a.relu;
+  p.out_mode = a.out_mode;
+  p.ldy = ldy;
+  p.ldr = ldr;
+  p.up_h = a.h / 2; p.up_w = a.width / 2;
+  if (s.op == kOpS8) {
+    p.alpha = a.alpha;
+    p.inv_out_scale = a.inv_out_scale;
+    p.res8 = (const int8_t *)a.residual; p.res_scale = a.res_scale;
+    p.up8 = (const int8_t *)a.upsample; p.up_scale = a.up_scale;
+  } else if (s.op == kOpTF32x3) {
+    p.res32 = (const float *)a.residual;
+    p.up32 = (const float *)a.upsample;
+  } else {
+    p.residual = (const __half *)a.residual;
+    p.upsample = (const __half *)a.upsample;
+    p.mask = (const __half *)a.mask;
+  }
   if (p.out_mode == ODTK_OUT_CANDIDATES) {
-    const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
+    const int rc = set_sink(p, a.sink, a.cout, a.h, a.width);
     if (rc != ODTK_OK) return rc;
   }
-  if (p.out_mode == ODTK_OUT_NHWC_F16 && (p.ldy % 8)) return ODTK_E_INVALID;
-  if ((p.residual && (p.ldr & 1)) || (d->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
-  const int stride = d->stride > 1 ? d->stride : 1;
-  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
-  // strided views: the input / output may be a rectangle of a larger NHWC buffer (a level of the pyramid atlas)
-  const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
-  const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
-  const bool y_view = d->y_rows > 0 || d->y_width > 0 || d->y_row_off > 0;
-  if ((x_view || y_view || (d->tile_tab && !dgrad)) && (d->ksize != 3 || d->residual || d->upsample)) return ODTK_E_UNSUPPORTED;
-  if (y_view && d->out_mode != ODTK_OUT_NHWC_F16) return ODTK_E_UNSUPPORTED;
-  if (d->tile_tab && (d->tab_tiles <= 0 || stride != 1 || x_view || y_view)) return ODTK_E_INVALID;
-  if (x2 && (d->ksize != 1 || stride != 1 || c2in <= 0 || c2in % 64 || !w2 || (((uintptr_t)x2 | (uintptr_t)w2) & 15))) return ODTK_E_INVALID;
-  if (dgrad && p.ldy != d->cout) return ODTK_E_UNSUPPORTED;   // the mask is read with the output's row stride
-  p.mask = (const __half *)mask;
-
   CUtensorMap tmA;
-  const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
-                           d->tab_tiles, d->upsample != nullptr, 2);
+  const int rc = stem ? stem_operand(p, tmA, a.x, a.n, a.h, a.width, s.es)
+                      : a_operand(p, tmA, a.x, a.n, a.h, a.width, a.cin, a.ksize, stride, xH, xW, x_view, a.tile_tab,
+                                  a.tab_tiles, s.es);
   if (rc != ODTK_OK) return rc;
-  p.oH = d->y_rows > 0 ? d->y_rows : p.H;
-  p.oR = d->y_row_off > 0 ? d->y_row_off : 0;
-  p.oW = d->y_width > 0 ? d->y_width : p.W;
-  if ((long long)d->n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
+  p.oH = a.y_rows > 0 ? a.y_rows : p.H;
+  p.oR = a.y_row_off > 0 ? a.y_row_off : 0;
+  p.oW = a.y_width > 0 ? a.y_width : p.W;
+  if ((long long)a.n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
   // N tile: 64 or 128 output channels.  128 halves the A-operand traffic; 64 when Cout is narrow, for grouped convs (one
   // 64-channel chunk per tile), or when 128-wide tiles would leave SMs idle.
-  int BN = (groups > 1 || d->cout <= 64) ? 64 : 128;
-  if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
-  p.num_n_tiles = (d->cout + BN - 1) / BN;
-  set_stages(p, BN);
-  CUtensorMap tmB, tmA2, tmB2;
-  const uint64_t K = (uint64_t)p.taps * (groups > 1 ? 64 : d->cin);
-  {
-    uint64_t dims[2] = {K, (uint64_t)d->cout};
-    uint64_t str[1] = {K * 2};
-    uint32_t box[2] = {64, (uint32_t)BN};
-    if (!encode_map(&tmB, d->w, 2, dims, str, box)) return ODTK_E_CUDA;
-  }
-  tmA2 = tmA; tmB2 = tmB;
-  if (x2) {
-    p.kblocks2 = c2in / 64;
-    uint64_t dims[2] = {(uint64_t)c2in, (uint64_t)p.M}, str[1] = {(uint64_t)c2in * 2};
+  int BN = (groups > 1 || a.cout <= 64) ? 64 : 128;
+  if (BN == 128 && (long long)p.num_m_tiles * ((a.cout + 127) / 128) < odtk_sm_count()) BN = 64;
+  p.num_n_tiles = (a.cout + BN - 1) / BN;
+  set_stages(p, BN, op);
+  CUtensorMap tmB, tmA2 = tmA, tmB2;
+  const uint64_t K = stem ? 224 : (uint64_t)p.taps * (groups > 1 ? 64 : a.cin);
+  if (!b_operand(tmB, a.w, K, a.cout, BN, p.row_bytes, s.es)) return ODTK_E_CUDA;
+  tmB2 = tmB;
+  if (a.w_lo && !b_operand(tmB2, a.w_lo, K, a.cout, BN, p.row_bytes, s.es)) return ODTK_E_CUDA;   // fp32: the low weight half
+  if (a.x2) {
+    p.kblocks2 = a.c2in / 64;
+    uint64_t dims[2] = {(uint64_t)a.c2in, (uint64_t)p.M}, str[1] = {(uint64_t)a.c2in * 2};
     uint32_t box[2] = {64, 128};
-    uint64_t dimsW[2] = {(uint64_t)c2in, (uint64_t)d->cout}, strW[1] = {(uint64_t)c2in * 2};
-    uint32_t boxW[2] = {64, (uint32_t)BN};
-    if (!encode_map(&tmA2, x2, 2, dims, str, box) || !encode_map(&tmB2, w2, 2, dimsW, strW, boxW)) return ODTK_E_CUDA;
+    if (!encode_map(&tmA2, a.x2, 2, dims, str, box) || !b_operand(tmB2, a.w2, a.c2in, a.cout, BN, 128, 2)) return ODTK_E_CUDA;
   }
-  return launch(p, BN, tmA, tmB, tmA2, tmB2, stream, dgrad ? kOpF16Mask : kOpF16);
+  return launch(p, BN, tmA, tmB, tmA2, tmB2, stream, op);
 }
 
-// odtk_conv2d_s8_ex: the same kernel on s8 operands, with the geometry of odtk_conv2d: 1x1 as GEMM rows (mode 0), 3x3 as
-// shifted boxes (mode 1) over a dense tensor, a level view of the atlas or the whole atlas with its tile table, stride 2 on
-// the parity-split view (mode 3, even sizes) or element-strided boxes (odd sizes, level views).  NHWC s8 outputs may add a
-// residual and / or a nearest-upsampled addend, and may land in a level view of an atlas.
-int conv_run_s8(const odtk_conv_s8_ex_t *e, cudaStream_t stream) {
-  if (!e) return ODTK_E_INVALID;
-  const odtk_conv_s8_t *d = &e->base;
-  if (!d->x || !d->w || !d->alpha) return ODTK_E_INVALID;
-  if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
-  if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
-  if (d->out_mode != ODTK_OUT_NHWC_S8 && d->out_mode != ODTK_OUT_NCHW_F32 && d->out_mode != ODTK_OUT_NCHW_F32_SIGMOID &&
-      d->out_mode != ODTK_OUT_CANDIDATES)
-    return ODTK_E_INVALID;
-  if ((d->ksize != 1 && d->ksize != 3) || d->cin % 128) return ODTK_E_UNSUPPORTED;   // 128-channel K blocks
-  if (d->relu != 0 && d->relu != 1) return ODTK_E_UNSUPPORTED;
-  if (d->out_mode == ODTK_OUT_NHWC_S8 && (d->cout % 16)) return ODTK_E_UNSUPPORTED;
-  if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  if (((uintptr_t)d->x | (uintptr_t)d->w | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15) return ODTK_E_INVALID;
-  const int stride = e->stride > 1 ? e->stride : 1;
-  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
-  const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
-  const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
-  const bool y_view = e->y_rows > 0 || e->y_width > 0 || e->y_row_off > 0;
-  const bool addend = e->residual || e->upsample;
-  // addends and output views: NHWC s8 only; views and tile tables: 3x3 without addends (as odtk_conv2d)
-  if ((addend || y_view) && d->out_mode != ODTK_OUT_NHWC_S8) return ODTK_E_UNSUPPORTED;
-  if ((x_view || y_view || d->tile_tab) && (d->ksize != 3 || addend)) return ODTK_E_UNSUPPORTED;
-  if (e->upsample && stride != 1) return ODTK_E_UNSUPPORTED;
-  if (d->tile_tab && (d->tab_tiles <= 0 || x_view || y_view || stride != 1)) return ODTK_E_INVALID;
-  if ((((uintptr_t)e->residual | (uintptr_t)e->upsample) & 1) || (e->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
-  if (!device_ready()) return ODTK_E_CUDA;
-  const int sms = odtk_sm_count();
-  ConvParams p;
-  memset(&p, 0, sizeof p);
-  p.N = d->n; p.H = d->h; p.W = d->width; p.Cin = d->cin; p.Cout = d->cout;
-  p.kw = d->ksize; p.taps = d->ksize * d->ksize; p.pad = d->ksize / 2;
-  p.kblocks_per_tap = d->cin / 128;
-  p.row_bytes = 128;
-  p.M = (long long)d->n * d->h * d->width;
-  p.alpha = d->alpha;
-  p.bias = d->bias;
-  p.out = d->y;
-  p.relu = d->relu;
-  p.out_mode = d->out_mode;
-  p.ldy = d->cout;
-  p.ldr = d->cout;
-  p.inv_out_scale = d->inv_out_scale;
-  p.res8 = (const int8_t *)e->residual; p.res_scale = e->res_scale;
-  p.up8 = (const int8_t *)e->upsample; p.up_scale = e->up_scale;
-  p.up_h = d->h / 2; p.up_w = d->width / 2;
-  if (p.out_mode == ODTK_OUT_CANDIDATES) {
-    const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
-    if (rc != ODTK_OK) return rc;
-  }
-  CUtensorMap tmA, tmB;
-  const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
-                           d->tab_tiles, e->upsample != nullptr, 1);
-  if (rc != ODTK_OK) return rc;
-  p.oH = e->y_rows > 0 ? e->y_rows : p.H;
-  p.oR = e->y_row_off > 0 ? e->y_row_off : 0;
-  p.oW = e->y_width > 0 ? e->y_width : p.W;
-  if ((long long)d->n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
-  // N tile as for odtk_conv2d
-  int BN = d->cout <= 64 ? 64 : 128;
-  if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
-  p.num_n_tiles = (d->cout + BN - 1) / BN;
-  set_stages(p, BN);
-  {
-    const uint64_t K = (uint64_t)p.taps * d->cin;
-    uint64_t dims[2] = {K, (uint64_t)d->cout};
-    uint64_t str[1] = {K};
-    uint32_t box[2] = {128, (uint32_t)BN};
-    if (!encode_map(&tmB, d->w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_UINT8)) return ODTK_E_CUDA;
-  }
-  return launch(p, BN, tmA, tmB, tmA, tmB, stream, kOpS8);
-}
-
-// odtk_conv2d_f32: the kernel on fp32 operands (split TF32).  1x1 / 3x3 with the geometry of odtk_conv2d (dense, atlas views,
-// tile tables, stride 2 on either view), plus ksize 7 / stride 2 / cin 3: the ResNet stem over the NHWC4 fp32 image
-// [n, h+6, width+8, 4] (mode 2, any h and width).  NHWC fp32 outputs may add an fp32 residual and / or upsample addend and
-// may land in a level view of an fp32 atlas.
-int conv_run_f32(const odtk_conv_f32_t *d, cudaStream_t stream) {
-  if (!d || !d->x || !d->w_hi || !d->w_lo) return ODTK_E_INVALID;
-  if (d->out_mode == ODTK_OUT_CANDIDATES ? !d->sink : !d->y) return ODTK_E_INVALID;
-  if (d->n <= 0 || d->h <= 0 || d->width <= 0 || d->cin <= 0 || d->cout <= 0) return ODTK_E_INVALID;
-  if (d->out_mode != ODTK_OUT_NHWC_F32 && d->out_mode != ODTK_OUT_NCHW_F32 && d->out_mode != ODTK_OUT_NCHW_F32_SIGMOID &&
-      d->out_mode != ODTK_OUT_CANDIDATES)
-    return ODTK_E_INVALID;
-  const int stride = d->stride > 1 ? d->stride : 1;
-  const bool stem = d->ksize == 7;
-  if (stem ? (d->cin != 3 || stride != 2) : ((d->ksize != 1 && d->ksize != 3) || d->cin % 32)) return ODTK_E_UNSUPPORTED;
-  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
-  if (d->relu != 0 && d->relu != 1) return ODTK_E_UNSUPPORTED;
-  if (d->out_mode == ODTK_OUT_NHWC_F32 && (d->cout % 2)) return ODTK_E_UNSUPPORTED;   // float2 stores
-  if ((long long)d->n * d->h * d->width >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  if (((uintptr_t)d->x | (uintptr_t)d->w_hi | (uintptr_t)d->w_lo | (d->out_mode == ODTK_OUT_CANDIDATES ? 0 : (uintptr_t)d->y)) & 15)
-    return ODTK_E_INVALID;
-  const uint64_t xH = d->x_rows > 0 ? (uint64_t)d->x_rows : (uint64_t)d->h, xW = d->x_width > 0 ? (uint64_t)d->x_width : (uint64_t)d->width;
-  const bool x_view = xH != (uint64_t)d->h || xW != (uint64_t)d->width;
-  const bool y_view = d->y_rows > 0 || d->y_width > 0 || d->y_row_off > 0;
-  const bool addend = d->residual || d->upsample;
-  // as odtk_conv2d_s8_ex: addends and output views need NHWC fp32, views and tile tables are 3x3 without addends
-  if ((addend || y_view) && d->out_mode != ODTK_OUT_NHWC_F32) return ODTK_E_UNSUPPORTED;
-  if ((x_view || y_view || d->tile_tab) && (d->ksize != 3 || addend)) return ODTK_E_UNSUPPORTED;
-  if (stem && addend) return ODTK_E_UNSUPPORTED;
-  if (d->upsample && stride != 1) return ODTK_E_UNSUPPORTED;
-  if (d->tile_tab && (d->tab_tiles <= 0 || x_view || y_view || stride != 1)) return ODTK_E_INVALID;
-  if ((((uintptr_t)d->residual | (uintptr_t)d->upsample) & 7) || (d->upsample && ((d->h & 1) || (d->width & 1)))) return ODTK_E_INVALID;
-  if (!device_ready()) return ODTK_E_CUDA;
-  const int sms = odtk_sm_count();
-  ConvParams p;
-  memset(&p, 0, sizeof p);
-  p.N = d->n; p.H = d->h; p.W = d->width; p.Cin = d->cin; p.Cout = d->cout;
-  p.row_bytes = 128;
-  p.M = (long long)d->n * d->h * d->width;
-  p.bias = d->bias;
-  p.out = d->y;
-  p.relu = d->relu;
-  p.out_mode = d->out_mode;
-  p.ldy = d->ldy > 0 ? d->ldy : d->cout;
-  p.ldr = d->ldr > 0 ? d->ldr : d->cout;
-  p.res32 = (const float *)d->residual;
-  p.up32 = (const float *)d->upsample;
-  p.up_h = d->h / 2; p.up_w = d->width / 2;
-  if ((p.out_mode == ODTK_OUT_NHWC_F32 && (p.ldy & 1)) || (p.res32 && (p.ldr & 1))) return ODTK_E_INVALID;   // float2 accesses
-  if (p.out_mode == ODTK_OUT_CANDIDATES) {
-    const int rc = set_sink(p, d->sink, d->cout, d->h, d->width);
-    if (rc != ODTK_OK) return rc;
-  }
-  CUtensorMap tmA, tmB, tmB2;
-  uint64_t K;
-  if (stem) {
-    // NHWC4 window rows as in odtk_stem_conv, in fp32: 8 pixels x 4 channels = 32 floats = one 128-byte swizzle row
-    const int OH = (d->h - 1) / 2 + 1, OW = (d->width - 1) / 2 + 1;
-    const uint64_t HP = (uint64_t)d->h + 6, WP = (uint64_t)d->width + 8;
-    p.mode = 2;
-    p.H = OH; p.W = OW; p.Cin = 4;
-    p.kw = 1; p.taps = 7; p.pad = 0; p.kblocks_per_tap = 1;
-    p.M = (long long)d->n * OH * OW;
-    choose_patch(OH, OW, p.TH, p.TW);
-    p.tiles_h = (OH + p.TH - 1) / p.TH;
-    p.tiles_w = (OW + p.TW - 1) / p.TW;
-    p.num_m_tiles = d->n * p.tiles_h * p.tiles_w;
-    uint64_t dims[5] = {32, (uint64_t)OW, 7, (uint64_t)OH, (uint64_t)d->n};
-    uint64_t str[4] = {32, WP * 16, WP * 32, HP * WP * 16};
-    uint32_t box[5] = {32, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
-    if (!encode_map(&tmA, d->x, 5, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32))
-      return ODTK_E_UNSUPPORTED;
-    K = 224;
-  } else {
-    p.kw = d->ksize; p.taps = d->ksize * d->ksize; p.pad = d->ksize / 2;
-    p.kblocks_per_tap = d->cin / 32;
-    const int rc = a_operand(p, tmA, d->x, d->n, d->h, d->width, d->cin, d->ksize, stride, xH, xW, x_view, d->tile_tab,
-                             d->tab_tiles, d->upsample != nullptr, 4);
-    if (rc != ODTK_OK) return rc;
-    K = (uint64_t)p.taps * d->cin;
-  }
-  p.oH = d->y_rows > 0 ? d->y_rows : p.H;
-  p.oR = d->y_row_off > 0 ? d->y_row_off : 0;
-  p.oW = d->y_width > 0 ? d->y_width : p.W;
-  if ((long long)d->n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
-  // N tile as for odtk_conv2d
-  int BN = d->cout <= 64 ? 64 : 128;
-  if (BN == 128 && (long long)p.num_m_tiles * ((d->cout + 127) / 128) < sms) BN = 64;
-  p.num_n_tiles = (d->cout + BN - 1) / BN;
-  set_stages(p, BN, kOpTF32x3);
-  {
-    uint64_t dims[2] = {K, (uint64_t)d->cout};
-    uint64_t str[1] = {K * 4};
-    uint32_t box[2] = {32, (uint32_t)BN};
-    if (!encode_map(&tmB, d->w_hi, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32) ||
-        !encode_map(&tmB2, d->w_lo, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, nullptr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32))
-      return ODTK_E_CUDA;
-  }
-  return launch(p, BN, tmA, tmB, tmA, tmB2, stream, kOpTF32x3);
+ConvArgs f16_args(const odtk_conv_t *d) {
+  ConvArgs a;
+  memset(&a, 0, sizeof a);
+  a.x = d->x; a.w = d->w; a.bias = d->bias; a.residual = d->residual; a.upsample = d->upsample; a.y = d->y;
+  a.n = d->n; a.h = d->h; a.width = d->width; a.cin = d->cin; a.cout = d->cout; a.ksize = d->ksize; a.relu = d->relu;
+  a.out_mode = d->out_mode; a.ldy = d->ldy; a.ldr = d->ldr; a.stride = d->stride; a.sink = d->sink; a.groups = d->groups;
+  a.x_rows = d->x_rows; a.x_width = d->x_width; a.y_rows = d->y_rows; a.y_row_off = d->y_row_off; a.y_width = d->y_width;
+  a.tile_tab = d->tile_tab; a.tab_tiles = d->tab_tiles;
+  return a;
 }
 
 // bias operand: [cout, 64] fp16 with (hi, lo, 0, ...): hi + lo == bias to 2^-22 relative
@@ -945,12 +858,30 @@ __global__ void pack_bias_kernel(const float *bias, __half *out, int cout) {
 }  // namespace
 
 extern "C" int odtk_conv2d(const odtk_conv_t *d, odtk_stream_t stream_) {
-  return conv_run(d, nullptr, nullptr, 0, (cudaStream_t)stream_);
+  if (!d) return ODTK_E_INVALID;
+  return conv_run(f16_args(d), kSpecF16, (cudaStream_t)stream_);
 }
 
 extern "C" int odtk_conv2d_dgrad(const odtk_conv_dgrad_t *d, odtk_stream_t stream_) {
   if (!d) return ODTK_E_INVALID;
-  return conv_run(&d->base, nullptr, nullptr, 0, (cudaStream_t)stream_, true, d->mask);
+  ConvArgs a = f16_args(&d->base);
+  a.dgrad = true;
+  a.mask = d->mask;
+  return conv_run(a, kSpecF16, (cudaStream_t)stream_);
+}
+
+extern "C" int odtk_conv2d_s8_ex(const odtk_conv_s8_ex_t *e, odtk_stream_t stream_) {
+  if (!e) return ODTK_E_INVALID;
+  const odtk_conv_s8_t *d = &e->base;
+  ConvArgs a;
+  memset(&a, 0, sizeof a);
+  a.x = d->x; a.w = d->w; a.alpha = d->alpha; a.bias = d->bias; a.y = d->y;
+  a.n = d->n; a.h = d->h; a.width = d->width; a.cin = d->cin; a.cout = d->cout; a.ksize = d->ksize; a.relu = d->relu;
+  a.out_mode = d->out_mode; a.inv_out_scale = d->inv_out_scale; a.sink = d->sink;
+  a.x_rows = d->x_rows; a.x_width = d->x_width; a.tile_tab = d->tile_tab; a.tab_tiles = d->tab_tiles;
+  a.stride = e->stride; a.residual = e->residual; a.res_scale = e->res_scale; a.upsample = e->upsample; a.up_scale = e->up_scale;
+  a.y_rows = e->y_rows; a.y_row_off = e->y_row_off; a.y_width = e->y_width;
+  return conv_run(a, kSpecS8, (cudaStream_t)stream_);
 }
 
 extern "C" int odtk_conv2d_s8(const odtk_conv_s8_t *d, odtk_stream_t stream_) {
@@ -958,62 +889,44 @@ extern "C" int odtk_conv2d_s8(const odtk_conv_s8_t *d, odtk_stream_t stream_) {
   odtk_conv_s8_ex_t e;
   memset(&e, 0, sizeof e);
   e.base = *d;
-  return conv_run_s8(&e, (cudaStream_t)stream_);
-}
-
-extern "C" int odtk_conv2d_s8_ex(const odtk_conv_s8_ex_t *e, odtk_stream_t stream_) {
-  return conv_run_s8(e, (cudaStream_t)stream_);
+  return odtk_conv2d_s8_ex(&e, stream_);
 }
 
 extern "C" int odtk_conv2d_f32(const odtk_conv_f32_t *d, odtk_stream_t stream_) {
-  return conv_run_f32(d, (cudaStream_t)stream_);
+  if (!d) return ODTK_E_INVALID;
+  ConvArgs a;
+  memset(&a, 0, sizeof a);
+  a.x = d->x; a.w = d->w_hi; a.w_lo = d->w_lo; a.bias = d->bias; a.residual = d->residual; a.upsample = d->upsample; a.y = d->y;
+  a.n = d->n; a.h = d->h; a.width = d->width; a.cin = d->cin; a.cout = d->cout; a.ksize = d->ksize; a.stride = d->stride;
+  a.relu = d->relu; a.out_mode = d->out_mode; a.ldy = d->ldy; a.ldr = d->ldr; a.sink = d->sink;
+  a.x_rows = d->x_rows; a.x_width = d->x_width; a.y_rows = d->y_rows; a.y_row_off = d->y_row_off; a.y_width = d->y_width;
+  a.tile_tab = d->tile_tab; a.tab_tiles = d->tab_tiles;
+  return conv_run(a, kSpecF32, (cudaStream_t)stream_);
 }
 
-// ResNet stem: 7x7 stride-2 pad-3 convolution of the RGB image, im2col-free.  `xp` is the image
-// zero-padded to NHWC4 [n, h+6, w+8, 4] fp16 by odtk_pad_input.  For filter row r the A operand of
-// output pixels (oh, ow..) is the 8-pixel x 4-channel window starting at padded pixel (2*oh + r, 2*ow):
-// 64 contiguous bytes, consecutive output pixels 16 bytes apart -- an OVERLAPPING-window 5-D tensor map
-// {32 elements, OW (16 B), 7 rows (one padded row), OH (two padded rows), N}.  K = 7 blocks of 32
-// (SWIZZLE_64B), weights packed [cout, 7*32] with k = r*32 + s*4 + c (zero for s = 7 or c = 3).
+// ResNet stem in fp16: 7x7 stride-2 pad-3 convolution of the RGB image zero-padded to NHWC4 [n, h+6, w+8, 4] fp16 by
+// odtk_pad_input (stem_operand), weights packed [cout, 7*32] with k = r*32 + s*4 + c (zero for s = 7 or c = 3).  Even h and
+// width; one N tile (cout <= 128).
 extern "C" int odtk_stem_conv(const void *xp, const void *w, const float *bias, void *y, int n, int h, int width,
                               int cout, int relu, odtk_stream_t stream_) {
   if (!xp || !w || !y || n <= 0 || h <= 0 || width <= 0) return ODTK_E_INVALID;
   if ((h & 1) || (width & 1) || cout % 16 || cout > 128) return ODTK_E_UNSUPPORTED;
   if (((uintptr_t)xp | (uintptr_t)w | (uintptr_t)y) & 15) return ODTK_E_INVALID;
-  cudaStream_t stream = (cudaStream_t)stream_;
   if (!device_ready()) return ODTK_E_CUDA;
-  const int OH = h / 2, OW = width / 2, HP = h + 6, WP = width + 8;
-  if ((long long)n * OH * OW >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  if ((long long)n * (h / 2) * (width / 2) >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
   ConvParams p;
   memset(&p, 0, sizeof p);
-  p.mode = 2;
-  p.N = n; p.H = OH; p.W = OW; p.Cin = 4; p.Cout = cout;
-  p.kw = 1; p.taps = 7; p.pad = 0; p.kblocks_per_tap = 1;
-  p.row_bytes = 64;
-  p.M = (long long)n * OH * OW;
+  p.N = n; p.Cout = cout;
+  CUtensorMap tmA, tmB;
+  const int rc = stem_operand(p, tmA, xp, n, h, width, 2);
+  if (rc != ODTK_OK) return rc;
   const int BN = cout <= 64 ? 64 : 128;
   p.num_n_tiles = 1;
-  set_stages(p, BN);
+  set_stages(p, BN, kOpF16);
   p.bias = bias; p.out = y; p.relu = relu; p.out_mode = ODTK_OUT_NHWC_F16; p.ldy = cout; p.ldr = cout;
-  p.oH = OH; p.oR = 0; p.oW = OW;
-  choose_patch(OH, OW, p.TH, p.TW);
-  p.tiles_h = (OH + p.TH - 1) / p.TH;
-  p.tiles_w = (OW + p.TW - 1) / p.TW;
-  p.num_m_tiles = n * p.tiles_h * p.tiles_w;
-  CUtensorMap tmA, tmB;
-  {
-    uint64_t dims[5] = {32, (uint64_t)OW, 7, (uint64_t)OH, (uint64_t)n};
-    uint64_t str[4] = {16, (uint64_t)WP * 8, (uint64_t)WP * 16, (uint64_t)HP * WP * 8};
-    uint32_t box[5] = {32, (uint32_t)p.TW, 1, (uint32_t)p.TH, 1};
-    if (!encode_map(&tmA, xp, 5, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B)) return ODTK_E_UNSUPPORTED;
-  }
-  {
-    uint64_t dims[2] = {224, (uint64_t)cout};
-    uint64_t str[1] = {224 * 2};
-    uint32_t box[2] = {32, (uint32_t)BN};
-    if (!encode_map(&tmB, w, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B)) return ODTK_E_CUDA;
-  }
-  return launch(p, BN, tmA, tmB, tmA, tmB, stream);
+  p.oH = p.H; p.oR = 0; p.oW = p.W;
+  if (!b_operand(tmB, w, 224, cout, BN, p.row_bytes, 2)) return ODTK_E_CUDA;
+  return launch(p, BN, tmA, tmB, tmA, tmB, (cudaStream_t)stream_, kOpF16);
 }
 
 // Pack a fp32 bias vector into the [cout, 64] fp16 (hi, lo) layout (see odtk_conv_t.bias_op).

@@ -146,50 +146,67 @@ class AtlasView:
         return self.atlas.data_ptr() + self.row_off * self.atlas.shape[2] * self.atlas.shape[3] * self.elem
 
 
+def _conv_setup(d, yd, x, cout, ksize, stride, out_mode, out, sink, tile_tab, nhwc_mode, nhwc_dtype):
+    """The fields odtk_conv_t, odtk_conv_s8_t and odtk_conv_f32_t share: x, y (allocated unless given: NHWC of the
+    precision's dtype or NCHW fp32), the atlas views of x and y (yd: the struct with the y_* fields), the tile table, the
+    sink and the sizes.  Returns the output."""
+    n, h, wd, cin = x.shape
+    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
+    if out_mode == OUT_CANDIDATES:
+        assert sink is not None
+    elif out is None:
+        if out_mode == nhwc_mode:
+            out = torch.empty((n, oh, ow, cout), dtype=nhwc_dtype, device=x.device)
+        else:
+            out = torch.empty((n, cout, oh, ow), dtype=torch.float32, device=x.device)
+    d.x, d.y = x.data_ptr(), (out.data_ptr() if out is not None else None)
+    if isinstance(x, AtlasView):
+        d.x_rows, d.x_width = x.atlas.shape[1], x.atlas.shape[2]
+    if isinstance(out, AtlasView):
+        yd.y_rows, yd.y_row_off, yd.y_width = out.atlas.shape[1], 0, out.atlas.shape[2]   # data_ptr() already points at the level
+    if tile_tab is not None:
+        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    d.sink = ctypes.addressof(sink) if sink is not None else None
+    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cin, cout, ksize
+    return out
+
+
+def _conv_launched(suffix, es, x, cout, ksize, stride, out_mode, nhwc_mode, tile_tab, wbytes, residual, upsample, groups=1):
+    """Trace entry of a convolution with es-byte activations: activations read once (atlas launches: the pixels of the
+    levels; 1x1 stride 2: the pixels it samples), the weights, the output, the addends."""
+    STATS["launches"] += 1
+    if STATS["trace"] is None:
+        return
+    n, h, wd, cin = x.shape
+    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
+    px = n * oh * ow if tile_tab is None else _tab_px(n, h, wd, tile_tab)
+    obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * (es if out_mode == nhwc_mode else 4)
+    xbytes = px * cin * es if (tile_tab is not None or (ksize == 1 and stride == 2)) else n * h * wd * cin * es
+    _trace("conv%dx%d%s" % (ksize, ksize, suffix), 2 * px * cout * ksize * ksize * cin // groups,
+           xbytes + wbytes + obytes + (px * cout * es if residual is not None else 0)
+           + (px * cout * es // 4 if upsample is not None else 0),
+           n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
+           upsample=upsample is not None, out_mode=out_mode)
+
+
 def conv2d(x, w, bias, cout, ksize, relu=False, residual=None, upsample=None, out_mode=OUT_NHWC_F16, out=None,
            stride=1, bias_op=None, sink=None, groups=1, tile_tab=None):
     """x: NHWC fp16 [N,H,W,Cin] (or an AtlasView); w: packed fp16 [Cout, ksize*ksize*Cin]; bias fp32 [Cout] or None.
     Stride 1 / 2, pad ksize//2.  Returns NHWC fp16 [N,H,W,Cout] or NCHW fp32 [N,Cout,H,W]; `out` may be an AtlasView
     (the result lands in that rectangle).  tile_tab (device int32 [T, 4]): x and out are whole atlases, one launch
     covers all the levels the table lists."""
-    xv = x if isinstance(x, AtlasView) else None
-    assert xv is not None or (x.is_cuda and x.dtype == torch.float16 and x.is_contiguous())
-    n, h, wd, cin = x.shape
-    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
-    if out_mode == OUT_CANDIDATES:
-        assert sink is not None
-    elif out is None:
-        if out_mode == OUT_NHWC_F16:
-            out = torch.empty((n, oh, ow, cout), dtype=torch.float16, device=x.device)
-        else:
-            out = torch.empty((n, cout, oh, ow), dtype=torch.float32, device=x.device)
+    assert isinstance(x, AtlasView) or (x.is_cuda and x.dtype == torch.float16 and x.is_contiguous())
     d = ConvDesc()
-    d.x, d.w, d.y = x.data_ptr(), w.data_ptr(), (out.data_ptr() if out is not None else None)
-    if xv is not None:
-        d.x_rows, d.x_width = xv.atlas.shape[1], xv.atlas.shape[2]
-    if isinstance(out, AtlasView):
-        d.y_rows, d.y_row_off, d.y_width = out.atlas.shape[1], 0, out.atlas.shape[2]      # data_ptr() already points at the level
-        d.y_row_off = 0
-    if tile_tab is not None:
-        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
-    d.sink = ctypes.addressof(sink) if sink is not None else None
+    out = _conv_setup(d, d, x, cout, ksize, stride, out_mode, out, sink, tile_tab, OUT_NHWC_F16, torch.float16)
+    d.w = w.data_ptr()
     d.bias = bias.data_ptr() if bias is not None else None
     d.residual = residual.data_ptr() if residual is not None else None
     d.upsample = upsample.data_ptr() if upsample is not None else None
-    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cin, cout, ksize
     d.relu, d.out_mode, d.ldy, d.ldr, d.stride = int(relu), out_mode, 0, 0, int(stride)
     d.bias_op = bias_op.data_ptr() if bias_op is not None else None
     d.groups = int(groups)
     _lib.check(_lib.lib().odtk_conv2d(ctypes.byref(d), _stream()), "conv2d")
-    STATS["launches"] += 1
-    if STATS["trace"] is not None:
-        px = n * oh * ow if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
-        obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * (2 if out_mode == OUT_NHWC_F16 else 4)
-        _trace("conv%dx%d" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin // groups,
-               (px * cin * 2 if ((ksize == 1 and stride == 2) or tile_tab is not None) else n * h * wd * cin * 2) + w.numel() * 2 + obytes + (px * cout * 2 if residual is not None else 0)
-               + (px * cout // 2 if upsample is not None else 0),
-               n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
-               upsample=upsample is not None, out_mode=out_mode)
+    _conv_launched("", 2, x, cout, ksize, stride, out_mode, OUT_NHWC_F16, tile_tab, w.numel() * 2, residual, upsample, groups)
     return out
 
 
@@ -205,48 +222,22 @@ def conv2d_s8(x, w, alpha, bias, cout, ksize, relu=False, out_mode=OUT_NHWC_S8, 
     xv = x if isinstance(x, AtlasView) else None
     assert xv is not None or (x.is_cuda and x.dtype == torch.int8 and x.is_contiguous())
     assert (xv.atlas if xv is not None else x).dtype == torch.int8 and w.dtype == torch.int8
-    n, h, wd, cin = x.shape
-    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
-    if out_mode == OUT_CANDIDATES:
-        assert sink is not None
-    elif out is None:
-        if out_mode == OUT_NHWC_S8:
-            out = torch.empty((n, oh, ow, cout), dtype=torch.int8, device=x.device)
-        else:
-            out = torch.empty((n, cout, oh, ow), dtype=torch.float32, device=x.device)
     for t in (residual, upsample):
         assert t is None or (t.is_cuda and t.dtype == torch.int8 and t.is_contiguous())
     e = ConvS8ExDesc()
     d = e.base
-    d.x, d.w, d.alpha, d.y = x.data_ptr(), w.data_ptr(), alpha.data_ptr(), (out.data_ptr() if out is not None else None)
+    out = _conv_setup(d, e, x, cout, ksize, stride, out_mode, out, sink, tile_tab, OUT_NHWC_S8, torch.int8)
+    d.w, d.alpha = w.data_ptr(), alpha.data_ptr()
     d.bias = bias.data_ptr() if bias is not None else None
-    if xv is not None:
-        d.x_rows, d.x_width = xv.atlas.shape[1], xv.atlas.shape[2]
-    if tile_tab is not None:
-        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
-    d.sink = ctypes.addressof(sink) if sink is not None else None
-    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cin, cout, ksize
     d.relu, d.out_mode, d.inv_out_scale = int(relu), out_mode, float(inv_out_scale)
     e.stride = int(stride)
     e.residual, e.res_scale = (residual.data_ptr() if residual is not None else None), float(res_scale)
     e.upsample, e.up_scale = (upsample.data_ptr() if upsample is not None else None), float(up_scale)
-    if isinstance(out, AtlasView):
-        e.y_rows, e.y_row_off, e.y_width = out.atlas.shape[1], 0, out.atlas.shape[2]     # data_ptr() already points at the level
     if stride == 1 and residual is None and upsample is None and not isinstance(out, AtlasView):
         _lib.check(_lib.lib().odtk_conv2d_s8(ctypes.byref(d), _stream()), "conv2d_s8")
     else:
         _lib.check(_lib.lib().odtk_conv2d_s8_ex(ctypes.byref(e), _stream()), "conv2d_s8_ex")
-    STATS["launches"] += 1
-    if STATS["trace"] is not None:
-        # 1-byte operands: activations read once (atlas launches: the pixels of the levels; 1x1 stride 2: the pixels it
-        # samples), int8 weights, the output, the addends
-        px = n * oh * ow if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
-        obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * (1 if out_mode == OUT_NHWC_S8 else 4)
-        xbytes = px * cin if (tile_tab is not None or (ksize == 1 and stride == 2)) else n * h * wd * cin
-        _trace("conv%dx%d_s8" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin,
-               xbytes + w.numel() + obytes + (px * cout if residual is not None else 0) + (px * cout // 4 if upsample is not None else 0),
-               n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
-               upsample=upsample is not None, out_mode=out_mode)
+    _conv_launched("_s8", 1, x, cout, ksize, stride, out_mode, OUT_NHWC_S8, tile_tab, w.numel(), residual, upsample)
     return out
 
 
@@ -287,30 +278,26 @@ def relu(x):
 
 
 def relu_from_view(view):
-    """ReLU of a pyramid level that lives inside the atlas, into a new dense tensor [N, h, w, C]."""
+    """ReLU of a pyramid level that lives inside the atlas (fp16, int8 or fp32) into a new dense tensor [N, h, w, C] of its
+    dtype: the input of FPN pyramid7, ReLU(P6)."""
     n, h, w, c = view.shape
     a = view.atlas
-    out = torch.empty((n, h, w, c), dtype=torch.float16, device=a.device)
-    _lib.check(_lib.lib().odtk_copy_rows_f16(ctypes.c_void_p(view.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w * c,
-                                             a.shape[1] * a.shape[2] * c, a.shape[2] * c, h * w * c, w * c, 1, _stream()), "copy_rows_f16")
+    out = torch.empty((n, h, w, c), dtype=a.dtype, device=a.device)
+    args = (ctypes.c_void_p(view.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w * c, a.shape[1] * a.shape[2] * c,
+            a.shape[2] * c, h * w * c, w * c)
+    L = _lib.lib()
+    if a.dtype == torch.float16:
+        _lib.check(L.odtk_copy_rows_f16(*args, 1, _stream()), "copy_rows_f16")
+    else:
+        name = {torch.int8: "relu_copy_rows_s8", torch.float32: "relu_copy_rows_f32"}[a.dtype]
+        _lib.check(getattr(L, "odtk_" + name)(*args, _stream()), name)
     STATS["launches"] += 1
-    _trace("relu", 0, out.numel() * 4, n=n, h=h, w=w, cin=c)
+    _trace({torch.float16: "relu", torch.int8: "relu_s8", torch.float32: "relu_f32"}[a.dtype], 0,
+           out.numel() * 2 * a.element_size(), n=n, h=h, w=w, cin=c)
     return out
 
 
-def relu_from_view_s8(view):
-    """ReLU of a level of the int8 atlas into a new dense int8 tensor [N, h, w, C] (odtk_relu_copy_rows_s8): pyramid7's
-    input ReLU(P6) in the INT8 network."""
-    n, h, w, c = view.shape
-    a = view.atlas
-    assert a.dtype == torch.int8
-    out = torch.empty((n, h, w, c), dtype=torch.int8, device=a.device)
-    _lib.check(_lib.lib().odtk_relu_copy_rows_s8(ctypes.c_void_p(view.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w * c,
-                                                 a.shape[1] * a.shape[2] * c, a.shape[2] * c, h * w * c, w * c, _stream()),
-               "relu_copy_rows_s8")
-    STATS["launches"] += 1
-    _trace("relu_s8", 0, out.numel() * 2, n=n, h=h, w=w, cin=c)
-    return out
+relu_from_view_s8 = relu_from_view_f32 = relu_from_view   # the names of the INT8 and fp32 atlas ReLU before they merged
 
 
 def maxpool3x3s2(x):
@@ -703,44 +690,18 @@ def conv2d_f32(x, w_hi, w_lo, bias, cout, ksize, relu=False, residual=None, upsa
     assert (xv.atlas if xv is not None else x).dtype == torch.float32
     assert xv is not None or (x.is_cuda and x.is_contiguous())
     assert w_hi.dtype == torch.float32 and w_lo.dtype == torch.float32
-    n, h, wd, cin = x.shape
-    oh, ow = ((h - 1) // 2 + 1, (wd - 1) // 2 + 1) if stride == 2 else (h, wd)
-    if out_mode == OUT_CANDIDATES:
-        assert sink is not None
-    elif out is None:
-        if out_mode == OUT_NHWC_F32:
-            out = torch.empty((n, oh, ow, cout), dtype=torch.float32, device=x.device)
-        else:
-            out = torch.empty((n, cout, oh, ow), dtype=torch.float32, device=x.device)
     for t in (residual, upsample):
         assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
     d = ConvF32Desc()
-    d.x, d.w_hi, d.w_lo, d.y = x.data_ptr(), w_hi.data_ptr(), w_lo.data_ptr(), (out.data_ptr() if out is not None else None)
+    out = _conv_setup(d, d, x, cout, ksize, stride, out_mode, out, sink, tile_tab, OUT_NHWC_F32, torch.float32)
+    d.w_hi, d.w_lo = w_hi.data_ptr(), w_lo.data_ptr()
     d.bias = bias.data_ptr() if bias is not None else None
     d.residual = residual.data_ptr() if residual is not None else None
     d.upsample = upsample.data_ptr() if upsample is not None else None
-    if xv is not None:
-        d.x_rows, d.x_width = xv.atlas.shape[1], xv.atlas.shape[2]
-    if isinstance(out, AtlasView):
-        d.y_rows, d.y_row_off, d.y_width = out.atlas.shape[1], 0, out.atlas.shape[2]     # data_ptr() already points at the level
-    if tile_tab is not None:
-        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
-    d.sink = ctypes.addressof(sink) if sink is not None else None
-    d.n, d.h, d.width, d.cin, d.cout, d.ksize, d.stride = n, h, wd, cin, cout, ksize, int(stride)
-    d.relu, d.out_mode = int(relu), out_mode
+    d.stride, d.relu, d.out_mode = int(stride), int(relu), out_mode
     _lib.check(_lib.lib().odtk_conv2d_f32(ctypes.byref(d), _stream()), "conv2d_f32")
-    STATS["launches"] += 1
-    if STATS["trace"] is not None:
-        # 4-byte operands: activations read once (atlas launches: the pixels of the levels; 1x1 stride 2: the pixels it
-        # samples), both weight halves, the output, the addends
-        px = n * oh * ow if tile_tab is None else n * int(((tile_tab[:, 2] - tile_tab[:, 0]).clamp(max=8) * (tile_tab[:, 3] - tile_tab[:, 1]).clamp(max=16)).sum())
-        obytes = 0 if out_mode == OUT_CANDIDATES else px * cout * 4
-        xbytes = px * cin * 4 if (tile_tab is not None or (ksize == 1 and stride == 2)) else n * h * wd * cin * 4
-        _trace("conv%dx%d_f32" % (ksize, ksize), 2 * px * cout * ksize * ksize * cin,
-               xbytes + (w_hi.numel() + w_lo.numel()) * 4 + obytes + (px * cout * 4 if residual is not None else 0)
-               + (px * cout if upsample is not None else 0),
-               n=n, h=h, w=wd, cin=cin, cout=cout, stride=int(stride), residual=residual is not None,
-               upsample=upsample is not None, out_mode=out_mode)
+    _conv_launched("_f32", 4, x, cout, ksize, stride, out_mode, OUT_NHWC_F32, tile_tab, (w_hi.numel() + w_lo.numel()) * 4,
+                residual, upsample)
     return out
 
 
@@ -818,21 +779,6 @@ def maxpool3x3s2_f32(x):
                                                 _stream()), "maxpool3x3s2_f32")
     STATS["launches"] += 1
     _trace("maxpool_f32", 0, x.numel() * 4 + out.numel() * 4, n=n, h=h, w=w, cin=c)
-    return out
-
-
-def relu_from_view_f32(view):
-    """ReLU of a level of the fp32 atlas into a new dense fp32 tensor [N, h, w, C] (odtk_relu_copy_rows_f32): pyramid7's
-    input ReLU(P6) in full precision."""
-    n, h, w, c = view.shape
-    a = view.atlas
-    assert a.dtype == torch.float32
-    out = torch.empty((n, h, w, c), dtype=torch.float32, device=a.device)
-    _lib.check(_lib.lib().odtk_relu_copy_rows_f32(ctypes.c_void_p(view.data_ptr()), ctypes.c_void_p(out.data_ptr()), n, h, w * c,
-                                                  a.shape[1] * a.shape[2] * c, a.shape[2] * c, h * w * c, w * c, _stream()),
-               "relu_copy_rows_f32")
-    STATS["launches"] += 1
-    _trace("relu_f32", 0, out.numel() * 8, n=n, h=h, w=w, cin=c)
     return out
 
 

@@ -144,8 +144,85 @@ def make_state_dict(backbone="ResNet50FPN", classes=80, num_anchors=9, rotated=F
     return sd
 
 
+def network_walk(backbone):
+    """Every convolution of the model once, in the shape of a packed layer set: "stem", "blocks" [{convs, down, level,
+    last, name}], "lateral3-5", "smooth3-5", "pyramid6-7", "cls_head", "box_head" (MobileNetV2FPN: the heads only, its
+    backbone is packed by Model._pack_mobilenet).  A convolution is a dict: conv / bn (state-dict prefixes; bn None for a
+    convolution with its own bias), stride, groups, x / y (the names of its input and output tensors, those of
+    calib.network_tensors and the calibration tables) and, for the convolutions that add one, res / up (the name of the
+    residual / upsample addend)."""
+    def conv(c, bn=None, stride=1, groups=1, x=None, y=None, **addend):
+        return dict(conv=c, bn=bn, stride=stride, groups=groups, x=x, y=y, **addend)
+
+    walk = {}
+    for head in calib.HEADS:
+        names = ["heads.input"] + ["%s.%d" % (head, i) for i in (0, 2, 4, 6, 8)]
+        walk[head] = [conv(names[k + 1], x=names[k], y=names[k + 1]) for k in range(5)]
+    if backbone in MOBILENET:
+        return walk
+    block, layers = RESNET_LAYERS[backbone]
+    f, n = "backbones.%s.features." % backbone, "backbones.%s." % backbone
+    groups = RESNEXT.get(backbone, (1, 64))[0]
+    exp = 4 if block == "bottleneck" else 1
+    walk["stem"] = conv(f + "conv1", f + "bn1", 2, x="input", y=f + "conv1")
+    blocks, taps, x, inplanes = [], {}, f + "maxpool", 64
+    for li, (planes, nblocks) in enumerate(zip((64, 128, 256, 512), layers)):
+        for b in range(nblocks):
+            stride = 2 if (b == 0 and li > 0) else 1
+            p = f + "layer%d.%d" % (li + 1, b)
+            y = f + "layer2" if (li == 1 and b == nblocks - 1) else p      # C3 is named after its layer
+            down = None
+            if b == 0 and (stride != 1 or inplanes != planes * exp):
+                down = conv(p + ".downsample.0", p + ".downsample.1", stride, x=x, y=p + ".downsample")
+            if block == "bottleneck":       # torchvision v1.5: the 3x3 carries the stride
+                ins, strides, gs = [x, p + ".conv1", p + ".conv2"], [1, stride, 1], [1, groups, 1]
+            else:
+                ins, strides, gs = [x, p + ".conv1"], [stride, 1], [1, 1]
+            outs = ins[1:] + [y]
+            convs = [conv(p + ".conv%d" % (k + 1), p + ".bn%d" % (k + 1), strides[k], gs[k], x=ins[k], y=outs[k])
+                     for k in range(len(ins))]
+            convs[-1]["res"] = down["y"] if down else x
+            blocks.append({"convs": convs, "down": down, "level": li + 2, "last": b == nblocks - 1, "name": p})
+            x, inplanes = y, planes * exp
+        taps[li + 2] = x
+    walk["blocks"] = blocks
+    walk["lateral5"] = conv(n + "lateral5", x=taps[5], y=n + "lateral5")
+    walk["lateral4"] = conv(n + "lateral4", x=taps[4], y=n + "lateral4", up=n + "lateral5")
+    walk["lateral3"] = conv(n + "lateral3", x=taps[3], y=n + "lateral3", up=n + "lateral4")
+    for k in (3, 4, 5):       # smooth and pyramid write the atlas the heads read
+        walk["smooth%d" % k] = conv(n + "smooth%d" % k, x=n + "lateral%d" % k, y="heads.input")
+    walk["pyramid6"] = conv(n + "pyramid6", stride=2, x=taps[5], y="heads.input")
+    walk["pyramid7"] = conv(n + "pyramid7", stride=2, x="heads.input", y="heads.input")
+    return walk
+
+
+def pack_walk(walk, make):
+    """The packed layer set of `walk` with every convolution replaced by make(convolution) (None: not in this set)."""
+    P = {}
+    for k, v in walk.items():
+        if k == "blocks":
+            P[k] = [dict(b, convs=[make(c) for c in b["convs"]], down=make(b["down"]) if b["down"] else None) for b in v]
+        else:
+            P[k] = [make(c) for c in v] if isinstance(v, list) else make(v)
+    return P
+
+
+def walk_weights(sd, c):
+    """(weight, bias) of a convolution of network_walk, BatchNorm folded (fp32)."""
+    if c["bn"] is None:
+        return sd[c["conv"] + ".weight"], sd.get(c["conv"] + ".bias")
+    bn = c["bn"]
+    return engine.fold_bn(sd[c["conv"] + ".weight"], sd[bn + ".weight"], sd[bn + ".bias"], sd[bn + ".running_mean"],
+                          sd[bn + ".running_var"])
+
+
+def _out_size(x, stride):
+    return (x.shape[1] - 1) // stride + 1, (x.shape[2] - 1) // stride + 1
+
+
 class _Conv:
-    """One packed convolution: fp16 weights in the kernel's K order, fp32 bias, geometry."""
+    """One packed convolution: fp16 weights in the kernel's K order, fp32 bias, geometry.  Packed layers of every precision
+    take (x, relu, residual, upsample, out, out_mode, sink, tile_tab, valid_px) and count their FLOPs."""
 
     def __init__(self, weight, bias, stride=1, device="cuda", groups=1):
         cout, cin, kh, kw = weight.shape
@@ -166,27 +243,70 @@ class _Conv:
         self.w = engine.pack_weight(weight, self.kpad).to(device)
         self.b = bias.float().contiguous().to(device) if bias is not None else None
 
-    def __call__(self, x, relu=False, residual=None, upsample=None, out_mode=engine.OUT_NHWC_F16, in_relu=False,
-                 sink=None, out=None, tile_tab=None, valid_px=None):
-        oh, ow = (x.shape[1] - 1) // self.stride + 1, (x.shape[2] - 1) // self.stride + 1
+    def __call__(self, x, relu=False, residual=None, upsample=None, out=None, out_mode=engine.OUT_NHWC_F16, sink=None,
+                 tile_tab=None, valid_px=None):
+        oh, ow = _out_size(x, self.stride)
         px = x.shape[0] * oh * ow if valid_px is None else valid_px          # atlas launches: only the pixels of the levels count
         engine.STATS["conv_flops"] += 2 * px * self.cout * self.ks * self.ks * self.cin // self.groups
         if self.stem and x.shape[1] % 2 == 0 and x.shape[2] % 2 == 0 and residual is None and upsample is None:
             return engine.stem_conv(x, self.w_stem, self.b, self.cout, relu)
         if self.direct:
-            assert not in_relu
             return engine.conv2d(x, self.w, self.b, self.cout, self.ks, relu, residual, upsample, out_mode,
                                  sink=sink, groups=self.groups, out=out, tile_tab=tile_tab)
         assert sink is None
         if self.stride == 2 and self.ks in (1, 3) and self.cin % 64 == 0 and upsample is None:
             # stride-2 convolution, any size: strided TMA view (even sizes: parity split, odd sizes: element-strided
-            # boxes), no gather pre-pass; ReLU on the input (FPN pyramid7) is one tiny elementwise launch
-            if in_relu:
-                x = engine.relu_from_view(x) if isinstance(x, engine.AtlasView) else engine.relu(x)
+            # boxes), no gather pre-pass
             return engine.conv2d(x, self.w, self.b, self.cout, self.ks, relu, residual, None, out_mode, stride=2,
                                  groups=self.groups, out=out)
-        low = engine.lower_conv(x, self.ks, self.stride, self.ks // 2, self.kpad if self.cin % 8 else None, in_relu)
+        low = engine.lower_conv(x, self.ks, self.stride, self.ks // 2, self.kpad if self.cin % 8 else None)
         return engine.conv2d(low, self.w, self.b, self.cout, 1, relu, residual, upsample, out_mode)
+
+
+class _ConvS8:
+    """One packed INT8 convolution: symmetric per-channel s8 weights and its epilogue constants from the calibration scales
+    of its tensors -- alpha[c] = s_in * s_w[c] (fp32), the fp32 bias, inv_out = 1 / s_out (None: an fp32 output), and the
+    scales of its residual / upsample addends."""
+
+    def __init__(self, weight, bias, s_in, s_out, stride=1, device="cuda", res_scale=None, up_scale=None):
+        q, s_w = engine.pack_weight_s8(weight)
+        self.w = q.to(device)
+        self.alpha = (s_w * torch.tensor(s_in, dtype=torch.float32)).contiguous().to(device)
+        self.b = bias.float().contiguous().to(device) if bias is not None else None
+        self.cout, self.ks, self.stride = weight.shape[0], weight.shape[2], stride
+        self.inv_out = float(np.float32(1.0) / s_out) if s_out is not None else None
+        self.res_scale, self.up_scale = res_scale, up_scale
+
+    def __call__(self, x, relu=False, residual=None, upsample=None, out=None, out_mode=engine.OUT_NHWC_S8, sink=None,
+                 tile_tab=None, valid_px=None):
+        oh, ow = _out_size(x, self.stride)
+        px = x.shape[0] * oh * ow if valid_px is None else valid_px
+        engine.STATS["conv_flops"] += 2 * px * self.cout * self.ks * self.ks * x.shape[3]
+        return engine.conv2d_s8(x, self.w, self.alpha, self.b, self.cout, self.ks, relu=relu, out_mode=out_mode, out=out,
+                                inv_out_scale=self.inv_out if self.inv_out is not None else 1.0, sink=sink,
+                                tile_tab=tile_tab, stride=self.stride, residual=residual,
+                                res_scale=self.res_scale if residual is not None else 0.0, upsample=upsample,
+                                up_scale=self.up_scale if upsample is not None else 0.0)
+
+
+class _ConvF32:
+    """One packed full-precision convolution: the fp32 weights split into two tf32-valued halves
+    (engine.pack_weight_tf32x2; the stem in its window K order), the fp32 bias, geometry."""
+
+    def __init__(self, weight, bias, stride=1, device="cuda", stem=False):
+        hi, lo = engine.pack_stem_weight_tf32x2(weight) if stem else engine.pack_weight_tf32x2(weight)
+        self.hi, self.lo = hi.to(device), lo.to(device)
+        self.b = bias.float().contiguous().to(device) if bias is not None else None
+        self.cout, self.ks, self.stride = weight.shape[0], weight.shape[2], stride
+
+    def __call__(self, x, relu=False, residual=None, upsample=None, out=None, out_mode=engine.OUT_NHWC_F32, sink=None,
+                 tile_tab=None, valid_px=None):
+        oh, ow = _out_size(x, self.stride)
+        px = x.shape[0] * oh * ow if valid_px is None else valid_px
+        engine.STATS["conv_flops"] += 2 * px * self.cout * self.ks * self.ks * x.shape[3]
+        return engine.conv2d_f32(x, self.hi, self.lo, self.b, self.cout, self.ks, relu=relu, residual=residual,
+                                 upsample=upsample, out_mode=out_mode, out=out, stride=self.stride, sink=sink,
+                                 tile_tab=tile_tab)
 
 
 class _HeadsTrain(torch.autograd.Function):
@@ -243,10 +363,6 @@ class Model:
         self.device = None
         self.parallel_heads = True
         self.fused_candidates = os.environ.get("ODTK_FUSED_CANDIDATES", "1") != "0"
-        self.fused_stem = os.environ.get("ODTK_FUSED_STEM", "1") != "0"
-        self.merged_heads = os.environ.get("ODTK_MERGED_HEADS", "1") != "0"
-        self.fused_bneck = os.environ.get("ODTK_FUSED_BNECK", "1") != "0"
-        self.fused_conv1 = os.environ.get("ODTK_FUSED_CONV1", "1") != "0"
         self._atlas = {}
         self._fused = {}
         self._head_streams = None
@@ -254,7 +370,7 @@ class Model:
         self._packed_out = {}
         self.precision = "fp16"
         self._int8_table = None       # calibration table of the INT8 heads (set_precision)
-        self._int8 = None             # their packed s8 weights, alpha, bias, requantisation scales
+        self._int8 = None             # the INT8 network: fp16 layers with the s8 ones of int8_scope in their place
         self.int8_scope = "heads"     # "heads" or "network" (layer3, layer4 and the FPN in INT8 as well)
         self._calib_hook = None
         self._calib_net = False       # calibration also records the network scope's tensors
@@ -434,190 +550,89 @@ class Model:
         return self
 
     def _pack(self):
-        sd, dev = self._sd, self.device
-        P = {}
         self._f32 = None
-
-        def conv_bn(prefix_conv, prefix_bn, stride=1, groups=1):
-            w, b = engine.fold_bn(sd[prefix_conv + ".weight"], sd[prefix_bn + ".weight"], sd[prefix_bn + ".bias"],
-                                  sd[prefix_bn + ".running_mean"], sd[prefix_bn + ".running_var"])
-            return _Conv(w, b, stride, dev, groups)
-
-        def conv_b(prefix, stride=1):
-            return _Conv(sd[prefix + ".weight"], sd.get(prefix + ".bias"), stride, dev)
-
+        sd, dev = self._sd, self.device
         if self.backbone in MOBILENET:
+            P = {}
             self._pack_mobilenet(P)
-            self._packed = P
-            self._pack_int8()
-            return
-        block, layers = RESNET_LAYERS[self.backbone]
-        f = "backbones.%s.features." % self.backbone
-        P["stem"] = conv_bn(f + "conv1", f + "bn1", 2)
-        blocks = []
-        for li, nblocks in enumerate(layers):
-            for b in range(nblocks):
-                stride = 2 if (b == 0 and li > 0) else 1
-                p = f + "layer%d.%d." % (li + 1, b)
-                blk = {"level": li + 2, "last": b == nblocks - 1, "name": p[:-1]}
-                if block == "bottleneck":
-                    blk["convs"] = [conv_bn(p + "conv1", p + "bn1"),
-                                    conv_bn(p + "conv2", p + "bn2", stride, RESNEXT.get(self.backbone, (1, 64))[0]),
-                                    conv_bn(p + "conv3", p + "bn3")]
-                else:
-                    blk["convs"] = [conv_bn(p + "conv1", p + "bn1", stride), conv_bn(p + "conv2", p + "bn2")]
-                blk["down"] = conv_bn(p + "downsample.0", p + "downsample.1", stride) if (p + "downsample.0.weight") in sd else None
-                blocks.append(blk)
-        P["blocks"] = blocks
-        n = "backbones.%s." % self.backbone
-        for k in ("lateral3", "lateral4", "lateral5", "smooth3", "smooth4", "smooth5"):
-            P[k] = conv_b(n + k)
-        P["pyramid6"] = conv_b(n + "pyramid6", 2)
-        P["pyramid7"] = conv_b(n + "pyramid7", 2)
-        for head in ("cls_head", "box_head"):
-            P[head] = [conv_b("%s.%d" % (head, i)) for i in (0, 2, 4, 6, 8)]
+        else:
+            P = pack_walk(network_walk(self.backbone),
+                          lambda c: _Conv(*walk_weights(sd, c), c["stride"], dev, c["groups"]))
         self._packed = P
         self._pack_int8()
 
     def _pack_int8(self):
-        """s8 weights of the 10 head layers (symmetric, per output channel) and their epilogue constants from the
-        calibration table: alpha[c] = s_in * s_w[c] (fp32), the fp32 bias, inv_out = 1 / s_out for the tower layers."""
+        """The INT8 network (set_precision("int8")): the fp16 layers with s8 ones in place of the layers `int8_scope` runs on
+        the s8 tensor cores -- the 10 head layers, and in scope "network" layer3, layer4 and the FPN too.  Every s8
+        convolution reads a tensor quantised with the scale of its table entry and requantises its output with the scale of
+        its own (calib.network_tensors); residual / upsample addends are dequantised with the scale of the tensor they are;
+        the smooth and pyramid convolutions write the s8 atlas with the "heads.input" scale.  Also the inverse scales of
+        the two fp16 -> s8 quantisations: C3 (network scope) and the atlas (heads scope)."""
         self._int8 = None
         if self._int8_table is None or self.device is None:
             return
-        scales, sd, dev = self._int8_table["scales"], self._sd, self.device
-        P = {"inv_in": float(np.float32(1.0) / np.float32(scales["heads.input"]))}
-        for head in calib.HEADS:
-            layers = []
-            for (s_in, inv), i in zip(calib.layer_scales(scales, head), (0, 2, 4, 6, 8)):
-                w = sd["%s.%d.weight" % (head, i)]
-                b = sd.get("%s.%d.bias" % (head, i))
-                q, s_w = engine.pack_weight_s8(w)
-                alpha = s_w * torch.tensor(s_in, dtype=torch.float32)
-                layers.append({"w": q.to(dev), "alpha": alpha.contiguous().to(dev), "cout": w.shape[0],
-                               "b": b.float().contiguous().to(dev) if b is not None else None,
-                               "inv_out": float(inv) if inv is not None else None})
-            P[head] = layers
-        if self.int8_scope == "network":
-            P["net"] = self._pack_int8_net()
-        self._int8 = P
-
-    def _pack_int8_net(self):
-        """Network scope: s8 weights (BatchNorm folded first) and epilogue constants of layer3, layer4 and the FPN.  Every
-        convolution reads a tensor quantised with the scale of its table entry (calib.network_tensors) and requantises its
-        output with the scale of its own; residual / upsample addends are dequantised with the scale of the tensor they
-        are; the smooth and pyramid convolutions write the s8 atlas with the "heads.input" scale."""
         S, sd, dev = self._int8_table["scales"], self._sd, self.device
-        block, layers = RESNET_LAYERS[self.backbone]
-        f, n = "backbones.%s.features." % self.backbone, "backbones.%s." % self.backbone
+        names = calib.table_tensors(self.backbone, self.int8_scope)
+        walk = network_walk(self.backbone)
+        if self.int8_scope == "heads":
+            walk = {h: walk[h] for h in calib.HEADS}
 
         def s32(name):
-            return np.float32(S[name])
+            return np.float32(S[name]) if name is not None and name in S else None
 
-        def layer(w, b, s_in, out, stride=1):
-            q, s_w = engine.pack_weight_s8(w)
-            return {"w": q.to(dev), "alpha": (s_w * torch.tensor(s_in, dtype=torch.float32)).contiguous().to(dev),
-                    "b": b.float().contiguous().to(dev) if b is not None else None, "cout": w.shape[0], "ks": w.shape[2],
-                    "stride": stride, "inv_out": float(np.float32(1.0) / s32(out))}
+        def make(c):
+            if c["x"] not in names:
+                return None
+            res, up = s32(c.get("res")), s32(c.get("up"))
+            return _ConvS8(*walk_weights(sd, c), s32(c["x"]), s32(c["y"]), c["stride"], dev,
+                           float(res) if res is not None else None, float(up) if up is not None else None)
 
-        def folded(pc, pb, s_in, out, stride=1):
-            w, b = engine.fold_bn(sd[pc + ".weight"], sd[pb + ".weight"], sd[pb + ".bias"], sd[pb + ".running_mean"],
-                                  sd[pb + ".running_var"])
-            return layer(w, b, s_in, out, stride)
-
-        def plain(name, s_in, out, stride=1):
-            return layer(sd[n + name + ".weight"], sd.get(n + name + ".bias"), s_in, out, stride)
-
-        x_name = f + "layer2"
-        c3 = x_name
-        blocks, c = [], {}
-        for li in (3, 4):
-            for b in range(layers[li - 1]):
-                p = f + "layer%d.%d" % (li, b)
-                stride = 2 if b == 0 else 1
-                mids = [p + ".conv1", p + ".conv2"] if block == "bottleneck" else [p + ".conv1"]
-                ins, outs = [x_name] + mids, mids + [p]
-                strided = 1 if block == "bottleneck" else 0          # torchvision v1.5: the 3x3 carries the stride
-                convs = [folded(p + ".conv%d" % (k + 1), p + ".bn%d" % (k + 1), s32(ins[k]), outs[k], stride if k == strided else 1)
-                         for k in range(len(ins))]
-                down = None
-                if (p + ".downsample.0.weight") in sd:
-                    down = folded(p + ".downsample.0", p + ".downsample.1", s32(x_name), p + ".downsample", stride)
-                blocks.append({"convs": convs, "down": down, "res_scale": float(s32(p + ".downsample" if down else x_name))})
-                x_name = p
-            c[li + 1] = x_name
-        N = {"inv_c3": float(np.float32(1.0) / s32(c3)), "blocks": blocks}
-        N["lateral5"] = plain("lateral5", s32(c[5]), n + "lateral5")
-        N["lateral4"] = dict(plain("lateral4", s32(c[4]), n + "lateral4"), up_scale=float(s32(n + "lateral5")))
-        N["lateral3"] = dict(plain("lateral3", s32(c3), n + "lateral3"), up_scale=float(s32(n + "lateral4")))
-        for k in (3, 4, 5):
-            N["smooth%d" % k] = plain("smooth%d" % k, s32(n + "lateral%d" % k), "heads.input")
-        N["pyramid6"] = plain("pyramid6", s32(c[5]), "heads.input", 2)
-        N["pyramid7"] = plain("pyramid7", s32("heads.input"), "heads.input", 2)
-        return N
-
-    def _pack_f32(self):
-        """Full precision: every convolution of the ResNet backbone, the FPN and the heads with BatchNorm folded in fp32 (as
-        _pack does), its weights split into two tf32-valued halves (engine.pack_weight_tf32x2), the fp32 bias and the
-        geometry."""
-        sd, dev = self._sd, self.device
-        block, layers = RESNET_LAYERS[self.backbone]
-        f, n = "backbones.%s.features." % self.backbone, "backbones.%s." % self.backbone
-
-        def layer(w, b, stride=1, stem=False):
-            hi, lo = engine.pack_stem_weight_tf32x2(w) if stem else engine.pack_weight_tf32x2(w)
-            return {"hi": hi.to(dev), "lo": lo.to(dev), "b": b.float().contiguous().to(dev) if b is not None else None,
-                    "cout": w.shape[0], "ks": w.shape[2], "stride": stride}
-
-        def folded(pc, pb, stride=1, stem=False):
-            w, b = engine.fold_bn(sd[pc + ".weight"], sd[pb + ".weight"], sd[pb + ".bias"], sd[pb + ".running_mean"],
-                                  sd[pb + ".running_var"])
-            return layer(w, b, stride, stem)
-
-        def plain(name, stride=1):
-            return layer(sd[n + name + ".weight"], sd.get(n + name + ".bias"), stride)
-
-        F = {"stem": folded(f + "conv1", f + "bn1", 2, stem=True), "blocks": []}
-        for li, nblocks in enumerate(layers):
-            for b in range(nblocks):
-                stride = 2 if (b == 0 and li > 0) else 1
-                p = f + "layer%d.%d." % (li + 1, b)
-                if block == "bottleneck":       # torchvision v1.5: the 3x3 carries the stride
-                    convs = [folded(p + "conv1", p + "bn1"), folded(p + "conv2", p + "bn2", stride), folded(p + "conv3", p + "bn3")]
-                else:
-                    convs = [folded(p + "conv1", p + "bn1", stride), folded(p + "conv2", p + "bn2")]
-                down = folded(p + "downsample.0", p + "downsample.1", stride) if (p + "downsample.0.weight") in sd else None
-                F["blocks"].append({"convs": convs, "down": down, "level": li + 2, "last": b == nblocks - 1})
-        for k in ("lateral3", "lateral4", "lateral5", "smooth3", "smooth4", "smooth5"):
-            F[k] = plain(k)
-        F["pyramid6"] = plain("pyramid6", 2)
-        F["pyramid7"] = plain("pyramid7", 2)
-        for head in ("cls_head", "box_head"):
-            F[head] = [layer(sd["%s.%d.weight" % (head, i)], sd.get("%s.%d.bias" % (head, i))) for i in (0, 2, 4, 6, 8)]
-        return F
-
-    def _full_precision(self):
-        """True when the inference forward runs in fp32 (set_precision("fp32")); the training-mode forward stays fp16."""
-        return self.precision == "fp32" and not self.training
+        N = dict(self._packed)
+        for k, v in pack_walk(walk, make).items():
+            if k == "blocks":
+                N[k] = [b8 if b8["convs"][0] is not None else b16 for b16, b8 in zip(N[k], v)]
+            elif v is not None:
+                N[k] = v
+        N["inv_in"] = float(np.float32(1.0) / np.float32(S["heads.input"]))
+        if self.int8_scope == "network":
+            N["inv_c3"] = float(np.float32(1.0) / s32("backbones.%s.features.layer2" % self.backbone))
+        self._int8 = N
 
     def _f32_layers(self):
+        """Full precision: every convolution of the ResNet backbone, the FPN and the heads with BatchNorm folded in fp32,
+        packed on first use."""
         if self._f32 is None:
             self._params_to_sd()          # trained head parameters
-            self._f32 = self._pack_f32()
+            sd, dev = self._sd, self.device
+            self._f32 = pack_walk(network_walk(self.backbone),
+                                  lambda c: _ConvF32(*walk_weights(sd, c), c["stride"], dev, stem=c["x"] == "input"))
         return self._f32
+
+    def _stem_dtype(self):
+        """The precision decision: fp32 activations from the stem input on (set_precision("fp32"), inference only), else
+        fp16 (the training-mode forward is always fp16)."""
+        return torch.float32 if self.precision == "fp32" and not self.training else torch.float16
+
+    def _net(self):
+        """The packed layers the forward runs: fp32, the INT8 network (inference only) or fp16."""
+        if self._stem_dtype() == torch.float32:
+            return self._f32_layers()
+        if self._int8 is not None and not self.training:
+            return self._int8
+        return self._packed
 
     def set_precision(self, precision, table=None, scope="heads"):
         """"fp16" (default), "fp32" or "int8".  "fp32" (full precision, the reference's --full-precision): fp32
         activations end to end and every convolution on split-TF32 tensor-core products (odtk_conv2d_f32); its head outputs
         are within 1e-4 - 2.3e-4 * max|ref| of fp32 PyTorch (measured on the H100) instead of fp16's 1.4e-3 - 2.1e-3 --
         ResNet18/34/50/101/152FPN (not ResNeXt or
-        MobileNetV2), over the pyramid atlas (ODTK_MERGED_HEADS=1); the fused stem-pool and bottleneck kernels are not
+        MobileNetV2); the fused stem-pool and bottleneck kernels are not
         used, and the split weights are packed on the first fp32 forward.  "int8": the head towers and the two final head layers run on the s8 tensor cores with the
         activation scales of `table` (a path or a dict, from `calibrate`).  scope "heads" (default): the backbone and the
         FPN stay fp16; "network" (a table from calibrate(..., scope="network")): ResNet layer3, layer4 and the FPN run in
         INT8 too, from layer2's output quantised once, and the FPN writes the s8 atlas the heads read -- the stem, layer1 and
         layer2 stay fp16 (ResNet18/34/50/101/152 backbones; ResNeXt and MobileNetV2 take "heads" only).  The training-mode
-        forward stays fp16.  INT8 needs the pyramid atlas (ODTK_MERGED_HEADS=1).  Captured CUDA graphs are dropped."""
+        forward stays fp16.  Captured CUDA graphs are dropped."""
         if precision == "fp16":
             self._int8_table = None
             self._int8 = None
@@ -625,16 +640,12 @@ class Model:
         elif precision == "fp32":
             if self.backbone not in FP32_BACKBONES:
                 raise ValueError("full precision covers %s, not %s" % (", ".join(FP32_BACKBONES), self.backbone))
-            if not self.merged_heads:
-                raise ValueError("full precision runs the heads over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
             self._int8_table = None
             self._int8 = None
             self.int8_scope = "heads"
         elif precision == "int8":
             if table is None:
                 raise ValueError("set_precision('int8') needs a calibration table (Model.calibrate)")
-            if not self.merged_heads:
-                raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
             if scope == "network":
                 calib.network_tensors(self.backbone)            # ValueError for the backbones the scope does not cover
             self._int8_table = calib.check_table(calib.load_table(table), self.backbone, self.classes, self.num_anchors, scope)
@@ -665,8 +676,6 @@ class Model:
         if scope not in calib.SCOPES:
             raise ValueError("INT8 scope must be 'heads' or 'network', got %r" % (scope,))
         names = calib.table_tensors(self.backbone, scope)
-        if not self.merged_heads:
-            raise ValueError("INT8 heads run over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
         batches = list(batches)
         col = calib.Collector()
         saved = (self._int8, self.parallel_heads, self.training, self.precision)
@@ -764,47 +773,67 @@ class Model:
 
     # ---- forward ---------------------------------------------------------------------------------
     def _stem(self, x=None, padded=None):
-        """conv1 + bn1 + relu + maxpool (odtk/backbones/resnet.py:25-28).  One fused kernel when the stem has the
-        standard 64 output channels and the image size is even; `padded` = (xp, h, w) from engine.preprocess_u8."""
+        """conv1 + bn1 + relu + maxpool (odtk/backbones/resnet.py:25-28).  fp16: one fused kernel when the stem has the
+        standard 64 output channels and the image size is even; `padded` = (xp, h, w) from engine.preprocess_u8 (fp32: the
+        NHWC4 fp32 stem buffer, stem convolution then max-pool)."""
         if self.backbone in MOBILENET:
             if padded is not None:
                 raise RuntimeError("the fused uint8 input path feeds the ResNet stem; pass a float / half image to MobileNetV2FPN")
             return x                                        # the 3x3 stem runs inside _features_mobilenet
-        stem = self._packed["stem"]
+        stem = self._net()["stem"]
         if padded is not None:
             xp, h, w = padded
             n = xp.shape[0]
         else:
             n, h, w = x.shape[0], x.shape[1], x.shape[2]
-        engine.STATS["conv_flops"] += 2 * n * (h // 2) * (w // 2) * stem.cout * 49 * 3
-        fused = self.fused_stem and stem.stem and stem.cout == 64 and h % 2 == 0 and w % 2 == 0
+        flops = 2 * n * ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1) * stem.cout * 49 * 3
+        engine.STATS["conv_flops"] += flops
+        if isinstance(stem, _ConvF32):
+            return engine.maxpool3x3s2_f32(engine.stem_conv_f32(xp, h, w, stem.hi, stem.lo, stem.b, stem.cout, relu=True))
+        fused = stem.stem and stem.cout == 64 and h % 2 == 0 and w % 2 == 0
         if padded is not None:
             if fused:
                 return engine.stem_pool_padded(xp, h, w, stem.w_stem, stem.b, stem.cout, relu=True)
             return engine.maxpool3x3s2(engine.stem_conv_padded(xp, h, w, stem.w_stem, stem.b, stem.cout, relu=True))
         if fused:
             return engine.stem_pool(x, stem.w_stem, stem.b, stem.cout, relu=True)
-        engine.STATS["conv_flops"] -= 2 * n * (h // 2) * (w // 2) * stem.cout * 49 * 3      # _Conv.__call__ counts it
+        engine.STATS["conv_flops"] -= flops      # _Conv.__call__ counts it
         return engine.maxpool3x3s2(stem(x, relu=True))
 
+    def _features_of(self, x):
+        """(pyramid level views, (h, w)) of an NCHW float batch, or of a uint8 HWC batch normalised and stride-padded on the
+        GPU (h, w: the padded size): the stem input of the current precision."""
+        f32 = self._stem_dtype() == torch.float32
+        if x.dtype == torch.uint8:
+            xp, hs, ws = (engine.preprocess_u8_f32 if f32 else engine.preprocess_u8)(x, self.stride)
+            return self._features(self._stem(padded=(xp, hs, ws))), (hs, ws)
+        if f32:
+            if x.dim() != 4:
+                raise ValueError("expected a [B, 3, H, W] batch")
+            xp = engine.pad_input_f32(x.permute(0, 2, 3, 1).contiguous().float())
+            return self._features(self._stem(padded=(xp, x.shape[2], x.shape[3]))), (x.shape[2], x.shape[3])
+        return self._features(self._stem(self._to_nhwc_half(x))), (x.shape[2], x.shape[3])
+
     def _features(self, x):
-        """`x`: the POOLED stem output [N, H/4, W/4, 64] (from _stem)."""
+        """`x`: the POOLED stem output [N, H/4, W/4, C] (from _stem).  The residual blocks, then the FPN.  fp16 blocks whose
+        shapes fit take the fused bottleneck kernels; every other block runs its downsample, then its convolutions with
+        the residual added in the last one's epilogue.  The INT8 network quantises C3 once, at its first s8 block."""
         if self.backbone in MOBILENET:
             return self._features_mobilenet(x)
-        P = self._packed
+        P = self._net()
         outs = {}
         blocks = P["blocks"]
-        net8 = self._int8.get("net") if (self._int8 is not None and not self.training) else None
         hook = self._calib_hook if self._calib_net else None     # network-scope calibration: layer3 / layer4 tensors
         z_next = None                 # conv1 of THIS block, already computed by the previous block's fused tail (GEMM3)
         for bi, blk in enumerate(blocks):
-            if net8 is not None and blk["level"] >= 4:
-                return self._features_s8(outs[3], net8)
-            tap = hook if blk["level"] >= 4 else None
             cs = blk["convs"]
             dn = blk["down"]
+            if isinstance(cs[0], _ConvS8) and x.dtype == torch.float16:
+                x = outs[3] = engine.quantize_f16_s8(x, P["inv_c3"])
+            fp16 = isinstance(cs[0], _Conv)
+            tap = hook if blk["level"] >= 4 else None
             z_in, z_next = z_next, None
-            if (self.fused_bneck and dn is not None and len(cs) == 3 and dn.ks == 1 and dn.stride == 1 and dn.cin == 64 and
+            if (fp16 and dn is not None and len(cs) == 3 and dn.ks == 1 and dn.stride == 1 and dn.cin == 64 and
                     dn.groups == 1 and cs[1].stride == 1 and cs[1].groups == 1 and cs[1].ks == 3 and cs[1].cin == 64 and
                     cs[1].cout == 64 and cs[2].cin == 64 and cs[2].cout == dn.cout and dn.cout % 128 == 0 and dn.cout <= 512):
                 # first block of layer1: conv2 + conv3 + the 1x1 PROJECTION of the block input (torchvision `downsample`)
@@ -822,7 +851,7 @@ class Model:
             identity = x if dn is None else dn(x)
             if tap is not None and dn is not None:
                 tap(blk["name"] + ".downsample", identity)
-            if (self.fused_bneck and tap is None and len(cs) == 3 and cs[1].stride == 1 and cs[1].groups == 1 and cs[1].ks == 3 and
+            if (fp16 and tap is None and len(cs) == 3 and cs[1].stride == 1 and cs[1].groups == 1 and cs[1].ks == 3 and
                     cs[1].cin in (64, 128) and cs[1].cout == cs[1].cin and cs[2].cin == cs[1].cin and cs[2].cout % 128 == 0 and
                     cs[2].cout <= 512):
                 # conv2 (3x3) + conv3 (1x1) + identity + ReLU in one kernel: the 3x3's output never leaves the SM
@@ -832,8 +861,9 @@ class Model:
                 # GEMM3: the NEXT block's conv1 (1x1, C2 -> 64 / 128, + ReLU) from this block's output while it is still in
                 # shared memory -- removes a full read of the widest tensor of the level
                 nxt = blocks[bi + 1]["convs"] if bi + 1 < len(blocks) else None
-                if (self.fused_conv1 and cs[1].cin == 64 and nxt is not None and len(nxt) == 3 and nxt[0].ks == 1 and nxt[0].stride == 1 and
-                        nxt[0].groups == 1 and nxt[0].cin == cs[2].cout and nxt[0].cout in (64, 128) and nxt[0].b is not None):
+                if (cs[1].cin == 64 and nxt is not None and len(nxt) == 3 and isinstance(nxt[0], _Conv) and nxt[0].ks == 1 and
+                        nxt[0].stride == 1 and nxt[0].groups == 1 and nxt[0].cin == cs[2].cout and nxt[0].cout in (64, 128) and
+                        nxt[0].b is not None):
                     engine.STATS["conv_flops"] += 2 * px * nxt[0].cin * nxt[0].cout
                     x, z_next = engine.bottleneck_tail(out, cs[1].w, cs[1].b, cs[2].w, cs[2].b, identity, relu=True,
                                                        w_next=nxt[0].w, b_next=nxt[0].b)
@@ -854,125 +884,29 @@ class Model:
             hook("backbones.%s.features.layer2" % self.backbone, outs[3])
         return self._fpn(outs[3], outs[4], outs[5])
 
-    def _conv8(self, L, x, relu=False, out=None, **addends):
-        """One network-scope s8 convolution (a layer of _pack_int8_net) of NHWC int8 x (or an int8 AtlasView)."""
-        n, h, w, cin = x.shape
-        oh, ow = ((h - 1) // 2 + 1, (w - 1) // 2 + 1) if L["stride"] == 2 else (h, w)
-        engine.STATS["conv_flops"] += 2 * n * oh * ow * L["cout"] * L["ks"] * L["ks"] * cin
-        return engine.conv2d_s8(x, L["w"], L["alpha"], L["b"], L["cout"], L["ks"], relu=relu, out=out,
-                                inv_out_scale=L["inv_out"], stride=L["stride"], **addends)
-
-    def _features_s8(self, c3, N):
-        """Network scope from layer2's fp16 output C3: one quantisation, then layer3, layer4 (residual added in the last
-        convolution's epilogue) and the FPN on s8."""
-        x = c3q = engine.quantize_f16_s8(c3, N["inv_c3"])
-        taps = []
-        for blk in N["blocks"]:
-            identity = x if blk["down"] is None else self._conv8(blk["down"], x)
-            t = x
-            for L in blk["convs"][:-1]:
-                t = self._conv8(L, t, relu=True)
-            x = self._conv8(blk["convs"][-1], t, relu=True, residual=identity, res_scale=blk["res_scale"])
-            taps.append(x)
-        nl3 = RESNET_LAYERS[self.backbone][1][2]
-        return self._fpn_s8(c3q, taps[nl3 - 1], taps[-1], N)
-
-    def _fpn_s8(self, c3, c4, c5, N):
-        """FPN on s8 taps: the laterals add the top-down path in their epilogue, smooth3/4/5 and pyramid6/7 write the s8
-        pyramid atlas the INT8 heads read."""
-        if not self.merged_heads:
-            raise ValueError("INT8 network scope writes the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0)")
-        p5 = self._conv8(N["lateral5"], c5)
-        p4 = self._conv8(N["lateral4"], c4, upsample=p5, up_scale=N["lateral4"]["up_scale"])
-        p3 = self._conv8(N["lateral3"], c3, upsample=p4, up_scale=N["lateral3"]["up_scale"])
-        n = c5.shape[0]
-        h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
-        sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
-                 ((h6 - 1) // 2 + 1, (w6 - 1) // 2 + 1))
-        at = self._atlas_for(n, sizes, c5.device)
-        v = [engine.AtlasView(self._atlas_s8(at)[0], r, h, w) for r, (h, w) in zip(at["rows"], sizes)]
-        self._conv8(N["smooth3"], p3, out=v[0])
-        self._conv8(N["smooth4"], p4, out=v[1])
-        self._conv8(N["smooth5"], p5, out=v[2])
-        self._conv8(N["pyramid6"], c5, out=v[3])
-        self._conv8(N["pyramid7"], engine.relu_from_view_s8(v[3]), out=v[4])
-        return v
-
-    def _conv32(self, L, x, relu=False, out=None, valid_px=None, **kw):
-        """One full-precision convolution (a layer of _pack_f32) of NHWC fp32 x (or an fp32 AtlasView)."""
-        n, h, w, cin = x.shape
-        oh, ow = ((h - 1) // 2 + 1, (w - 1) // 2 + 1) if L["stride"] == 2 else (h, w)
-        px = n * oh * ow if valid_px is None else valid_px
-        engine.STATS["conv_flops"] += 2 * px * L["cout"] * L["ks"] * L["ks"] * cin
-        return engine.conv2d_f32(x, L["hi"], L["lo"], L["b"], L["cout"], L["ks"], relu=relu, out=out, stride=L["stride"], **kw)
-
-    def _input_f32(self, x):
-        """NCHW float batch -> the fp32 NHWC4 stem buffer (xp, h, w)."""
-        if x.dim() != 4:
-            raise ValueError("expected a [B, 3, H, W] batch")
-        return engine.pad_input_f32(x.permute(0, 2, 3, 1).contiguous().float()), x.shape[2], x.shape[3]
-
-    def _features_f32(self, xp, h, w):
-        """Full precision from the fp32 NHWC4 stem buffer [N, h+6, w+8, 4]: stem convolution (+ ReLU) and max-pool, the
-        ResNet blocks as their 1x1 / 3x3 launches with the residual added in the last one's epilogue, then the FPN into
-        the fp32 atlas.  Returns the five level views."""
-        F = self._f32_layers()
-        st = F["stem"]
-        engine.STATS["conv_flops"] += 2 * xp.shape[0] * ((h - 1) // 2 + 1) * ((w - 1) // 2 + 1) * st["cout"] * 49 * 3
-        x = engine.maxpool3x3s2_f32(engine.stem_conv_f32(xp, h, w, st["hi"], st["lo"], st["b"], st["cout"], relu=True))
-        outs = {}
-        for blk in F["blocks"]:
-            identity = x if blk["down"] is None else self._conv32(blk["down"], x)
-            t = x
-            for L in blk["convs"][:-1]:
-                t = self._conv32(L, t, relu=True)
-            x = self._conv32(blk["convs"][-1], t, relu=True, residual=identity)
-            if blk["last"]:
-                outs[blk["level"]] = x
-        c3, c4, c5 = outs[3], outs[4], outs[5]
-        p5 = self._conv32(F["lateral5"], c5)
-        p4 = self._conv32(F["lateral4"], c4, upsample=p5)
-        p3 = self._conv32(F["lateral3"], c3, upsample=p4)
-        n = c5.shape[0]
-        h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
-        sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
-                 ((h6 - 1) // 2 + 1, (w6 - 1) // 2 + 1))
-        at = self._atlas_for(n, sizes, c5.device)
-        v = [engine.AtlasView(self._atlas_f32(at)[0], r, lh, lw) for r, (lh, lw) in zip(at["rows"], sizes)]
-        self._conv32(F["smooth3"], p3, out=v[0])
-        self._conv32(F["smooth4"], p4, out=v[1])
-        self._conv32(F["smooth5"], p5, out=v[2])
-        self._conv32(F["pyramid6"], c5, out=v[3])
-        self._conv32(F["pyramid7"], engine.relu_from_view_f32(v[3]), out=v[4])
-        return v
-
     def _fpn(self, c3, c4, c5):
-        """FPN (odtk/backbones/fpn.py:45-61) on the three backbone taps."""
-        P = self._packed
+        """FPN (odtk/backbones/fpn.py:45-61) on the three backbone taps, into the pyramid atlas: the five levels stacked in
+        ONE zero-separated NHWC buffer of the activation dtype, so that every head-tower layer is one launch over all
+        levels instead of five.  Returns the five level views."""
+        P = self._net()
         p5 = P["lateral5"](c5)
         p4 = P["lateral4"](c4, upsample=p5)
         p3 = P["lateral3"](c3, upsample=p4)
         if self._calib_net:
             for k, t in ((5, p5), (4, p4), (3, p3)):
                 self._calib_hook("backbones.%s.lateral%d" % (self.backbone, k), t)
-        if self.merged_heads and c5.shape[3] % 64 == 0:
-            # pyramid atlas: the five levels stacked in ONE zero-separated NHWC buffer, so that every head-tower layer is
-            # one launch over all levels instead of five
-            n = c5.shape[0]
-            h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
-            sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
-                     ((h6 - 1) // 2 + 1, (w6 - 1) // 2 + 1))
-            at = self._atlas_for(n, sizes, c5.device)
-            v = [engine.AtlasView(at["buf"][0], r, h, w) for r, (h, w) in zip(at["rows"], sizes)]
-            P["smooth3"](p3, out=v[0])
-            P["smooth4"](p4, out=v[1])
-            P["smooth5"](p5, out=v[2])
-            P["pyramid6"](c5, out=v[3])
-            P["pyramid7"](v[3], in_relu=True, out=v[4])
-            return v
-        p6 = P["pyramid6"](c5)
-        p7 = P["pyramid7"](p6, in_relu=True)
-        return [P["smooth3"](p3), P["smooth4"](p4), P["smooth5"](p5), p6, p7]
+        n = c5.shape[0]
+        h6, w6 = (c5.shape[1] - 1) // 2 + 1, (c5.shape[2] - 1) // 2 + 1
+        sizes = ((p3.shape[1], p3.shape[2]), (p4.shape[1], p4.shape[2]), (p5.shape[1], p5.shape[2]), (h6, w6),
+                 ((h6 - 1) // 2 + 1, (w6 - 1) // 2 + 1))
+        at = self._atlas_for(n, sizes, c5.device)
+        v = [engine.AtlasView(self._atlas_bufs(at, p3.dtype)[0], r, h, w) for r, (h, w) in zip(at["rows"], sizes)]
+        P["smooth3"](p3, out=v[0])
+        P["smooth4"](p4, out=v[1])
+        P["smooth5"](p5, out=v[2])
+        P["pyramid6"](c5, out=v[3])
+        P["pyramid7"](engine.relu_from_view(v[3]), out=v[4])
+        return v
 
     def _atlas_for(self, n, sizes, device):
         """Geometry + persistent, zero-initialised buffers of the pyramid atlas for one batch size / level geometry.
@@ -997,83 +931,31 @@ class Model:
         return at
 
     @staticmethod
-    def _atlas_s8(at):
-        """The five int8 buffers of an atlas geometry (INT8 heads), zero-initialised on first use."""
-        if "buf8" not in at:
+    def _atlas_bufs(at, dtype):
+        """The five buffers of an atlas geometry in `dtype`: at["buf"] for fp16, int8 (INT8) and fp32 (full precision) ones
+        zero-initialised on first use."""
+        if dtype == torch.float16:
+            return at["buf"]
+        key = "buf_" + str(dtype).split(".")[-1]
+        if key not in at:
             buf = at["buf"][0]
-            at["buf8"] = [torch.zeros(buf.shape, dtype=torch.int8, device=buf.device) for _ in range(5)]
-        return at["buf8"]
-
-    @staticmethod
-    def _atlas_f32(at):
-        """The five fp32 buffers of an atlas geometry (full precision), zero-initialised on first use."""
-        if "buf32" not in at:
-            buf = at["buf"][0]
-            at["buf32"] = [torch.zeros(buf.shape, dtype=torch.float32, device=buf.device) for _ in range(5)]
-        return at["buf32"]
+            at[key] = [torch.zeros(buf.shape, dtype=dtype, device=buf.device) for _ in range(5)]
+        return at[key]
 
     def _heads(self, features, sigmoid=True, sinks=None):
-        """Class / box heads on the five levels (odtk/model.py:134-135).  The ten conv chains are
-        independent, so each runs on its own CUDA stream (fork after the FPN, join before decode): the
-        small levels' launches (P5-P7 use 1-32 CTAs) overlap each other and the tail of the big
-        ones; inside a CUDA graph the chains become parallel branches."""
-        P = self._packed
-        nl = len(features)
-        cls_heads, box_heads = [None] * nl, [None] * nl
-        cls_mode = engine.OUT_NCHW_F32_SIGMOID if sigmoid else engine.OUT_NCHW_F32
-        if isinstance(features[0], engine.AtlasView):
-            return self._heads_atlas(features, cls_mode, sinks)
-        if self._int8 is not None and not self.training:
-            raise ValueError("INT8 heads run over the pyramid atlas, which this model does not use (ODTK_MERGED_HEADS=0 "
-                             "or a backbone whose C5 width is not a multiple of 64)")
-
-        def chain(head, t, final_mode, sink=None):
-            for conv in P[head][:-1]:
-                t = conv(t, relu=True)
-            if sink is not None:      # class scores go straight to the decode workspace (no dense map)
-                return P[head][-1](t, out_mode=engine.OUT_CANDIDATES, sink=sink)
-            return P[head][-1](t, out_mode=final_mode)
-
-        if not self.parallel_heads:
-            for i, t in enumerate(features):
-                cls_heads[i] = chain("cls_head", t, cls_mode, sinks[i] if sinks is not None else None)
-                box_heads[i] = chain("box_head", t, engine.OUT_NCHW_F32)
-            return cls_heads, box_heads
-        main = torch.cuda.current_stream()
-        if self._head_streams is None or len(self._head_streams) < 2 * nl:
-            self._head_streams = [torch.cuda.Stream(device=self.device) for _ in range(2 * nl)]
-        fork = torch.cuda.Event()
-        fork.record(main)
-        joins = []
-        for i, t in enumerate(features):
-            for j, (head, mode) in enumerate((("cls_head", cls_mode), ("box_head", engine.OUT_NCHW_F32))):
-                sink = sinks[i] if (sinks is not None and j == 0) else None
-                if i == 0 and j == 0:          # the biggest chain stays on the main stream
-                    cls_heads[0] = chain(head, t, mode, sink)
-                    continue
-                st = self._head_streams[2 * i + j]
-                st.wait_event(fork)
-                with torch.cuda.stream(st):
-                    out = chain(head, t, mode, sink)
-                    ev = torch.cuda.Event()
-                    ev.record(st)
-                joins.append(ev)
-                (cls_heads if j == 0 else box_heads)[i] = out
-        for ev in joins:
-            main.wait_event(ev)
-        return cls_heads, box_heads
+        """Class / box heads on the five levels of the pyramid atlas (odtk/model.py:134-135)."""
+        return self._heads_atlas(features, engine.OUT_NCHW_F32_SIGMOID if sigmoid else engine.OUT_NCHW_F32, sinks)
 
     def _heads_atlas(self, views, cls_mode, sinks):
         """Heads over the pyramid atlas: each of the 4 + 4 tower layers is ONE launch over all five levels (a tile table
         lists the 8 x 16 tiles of every level; weights are shared between levels anyway, odtk/model.py:134-135); the
         two final layers run per level on views of the last tower output (their outputs are per-level tensors).  The class
-        and the box tower are independent: two streams / two graph branches."""
-        P = self._packed
+        and the box tower are independent: two streams / two graph branches.  INT8 heads on an fp16 atlas quantise it
+        once, on the main stream before the fork."""
+        P = self._net()
         atlas0 = views[0].atlas
         sizes = tuple((v.h, v.w) for v in views)
         at = self._atlas_for(atlas0.shape[0], sizes, atlas0.device)
-        nl = len(views)
-        cls_heads, box_heads = [None] * nl, [None] * nl
         hook = self._calib_hook
         if hook is not None:              # calibration: the valid atlas pixels of the heads' input and of every tower output
             if "valid" not in at:
@@ -1082,6 +964,9 @@ class Model:
                     valid[r:r + h, :w] = True
                 at["valid"] = valid
             hook("heads.input", atlas0[:, at["valid"]])
+        if isinstance(P["cls_head"][0], _ConvS8) and atlas0.dtype == torch.float16:
+            atlas0 = engine.quantize_f16_s8(atlas0, P["inv_in"], out=self._atlas_bufs(at, torch.int8)[0])
+        bufs = self._atlas_bufs(at, atlas0.dtype)
 
         def tower(head, bufs, final_mode, use_sinks):
             t = atlas0
@@ -1100,57 +985,12 @@ class Model:
                     outs.append(P[head][-1](lv, out_mode=final_mode))
             return outs
 
-        i8 = self._int8 if not self.training else None
-        if i8 is not None:
-            # INT8: the fp16 atlas is quantised once (main stream, before the fork) -- in network scope the FPN wrote the s8
-            # atlas itself; towers and final layers run on s8
-            buf8 = self._atlas_s8(at)
-            q_in = atlas0 if atlas0.dtype == torch.int8 else engine.quantize_f16_s8(atlas0, i8["inv_in"], out=buf8[0])
-
-            def tower8(head, bufs, final_mode, use_sinks):
-                t = q_in
-                for i, layer in enumerate(i8[head][:-1]):
-                    nxt = bufs[i & 1]
-                    engine.STATS["conv_flops"] += 2 * at["px"] * 256 * 9 * 256
-                    engine.conv2d_s8(t, layer["w"], layer["alpha"], layer["b"], layer["cout"], 3, relu=True,
-                                     out_mode=engine.OUT_NHWC_S8, out=nxt, inv_out_scale=layer["inv_out"], tile_tab=at["tab"])
-                    t = nxt
-                last, outs = i8[head][-1], []
-                for l, v in enumerate(views):
-                    lv = engine.AtlasView(t, at["rows"][l], v.h, v.w)
-                    engine.STATS["conv_flops"] += 2 * lv.shape[0] * v.h * v.w * last["cout"] * 9 * 256
-                    mode, sink = (engine.OUT_CANDIDATES, use_sinks[l]) if use_sinks is not None else (final_mode, None)
-                    outs.append(engine.conv2d_s8(lv, last["w"], last["alpha"], last["b"], last["cout"], 3, out_mode=mode, sink=sink))
-                return outs
-
-            tower, bufs = tower8, buf8
-        elif self._full_precision():
-            # full precision: the FPN wrote the fp32 atlas; towers and final layers on split-TF32 products
-            f32 = self._f32_layers()
-
-            def tower32(head, bufs, final_mode, use_sinks):
-                t = atlas0
-                for i, L in enumerate(f32[head][:-1]):
-                    nxt = bufs[i & 1]
-                    self._conv32(L, t, relu=True, out=nxt, tile_tab=at["tab"], valid_px=at["px"])
-                    t = nxt
-                outs = []
-                for l, v in enumerate(views):
-                    lv = engine.AtlasView(t, at["rows"][l], v.h, v.w)
-                    mode, sink = (engine.OUT_CANDIDATES, use_sinks[l]) if use_sinks is not None else (final_mode, None)
-                    outs.append(self._conv32(f32[head][-1], lv, out_mode=mode, sink=sink))
-                return outs
-
-            tower, bufs = tower32, self._atlas_f32(at)
-        else:
-            bufs = at["buf"]
-
         if not self.parallel_heads:
             cls_heads = tower("cls_head", bufs[1:3], cls_mode, sinks)
             box_heads = tower("box_head", bufs[3:5], engine.OUT_NCHW_F32, None)
             return cls_heads, box_heads
         main = torch.cuda.current_stream()
-        if self._head_streams is None or len(self._head_streams) < 1:
+        if self._head_streams is None:
             self._head_streams = [torch.cuda.Stream(device=self.device)]
         side = self._head_streams[0]
         fork = torch.cuda.Event()
@@ -1176,12 +1016,8 @@ class Model:
         kernel that writes the stem's input buffer directly."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
-        P = self._packed
-        if self._full_precision():
-            xp, hs, ws = engine.preprocess_u8_f32(images, self.stride)
-            return self._heads(self._features_f32(xp, hs, ws), sigmoid), (hs, ws)
-        xp, hs, ws = engine.preprocess_u8(images, self.stride)
-        return self._heads(self._features(self._stem(padded=(xp, hs, ws))), sigmoid), (hs, ws)
+        features, size = self._features_of(images)
+        return self._heads(features, sigmoid), size
 
     def forward_heads(self, x, sigmoid=True):
         """The `exporting=True` view of the reference (odtk/model.py:142-144): per-level
@@ -1189,9 +1025,7 @@ class Model:
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
         self._sync_params()
-        if self._full_precision():
-            return self._heads(self._features_f32(*self._input_f32(x)), sigmoid)
-        return self._heads(self._features(self._stem(self._to_nhwc_half(x))), sigmoid)
+        return self._heads(self._features_of(x)[0], sigmoid)
 
     def _level_anchors(self, widths, width):
         strides, anchors = [], []
@@ -1211,19 +1045,7 @@ class Model:
         of odtk/model.py:140 are never written or re-read.  Same detections as the dense route."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
-        if self._full_precision():
-            if x.dtype == torch.uint8:
-                xp, hs, width = engine.preprocess_u8_f32(x, self.stride)
-                features = self._features_f32(xp, hs, width)
-            else:
-                width = x.shape[-1]
-                features = self._features_f32(*self._input_f32(x))
-        elif x.dtype == torch.uint8:
-            xp, hs, width = engine.preprocess_u8(x, self.stride)
-            features = self._features(self._stem(padded=(xp, hs, width)))
-        else:
-            width = x.shape[-1]
-            features = self._features(self._stem(self._to_nhwc_half(x)))
+        features, (_, width) = self._features_of(x)
         return self._detect_fused(features, width)
 
     def _detect_fused(self, features, width):
@@ -1308,9 +1130,6 @@ class Model:
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
         views = self._features(self._stem(self._to_nhwc_half(x)))
-        if not isinstance(views[0], engine.AtlasView):
-            raise ValueError("training the heads runs over the pyramid atlas; it is disabled (ODTK_MERGED_HEADS=0) or the "
-                             "backbone does not use it")
         P = self._packed
         atlas0 = views[0].atlas
         at = self._atlas_for(atlas0.shape[0], tuple((v.h, v.w) for v in views), atlas0.device)
@@ -1413,10 +1232,7 @@ class Model:
     def _forward_padded(self, xp, hs, width):
         """Detections from the stem's padded NHWC4 input buffer (fp32 in full precision): the fused-candidate or the dense
         route of forward()."""
-        if self._full_precision():
-            features = self._features_f32(xp, hs, width)
-        else:
-            features = self._features(self._stem(padded=(xp, hs, width)))
+        features = self._features(self._stem(padded=(xp, hs, width)))
         if self.fused_candidates:
             return self._detect_fused(features, width)
         return self._detect_dense(*self._heads(features), width)
@@ -1439,7 +1255,7 @@ class Model:
         hs, ws = plan.canvas
         if getattr(self, "_graphs", None) is None:
             xp, _, _, ratios = engine.preprocess_resize_u8(images, resize, max_size, self.stride, (hs, ws),
-                                                           f32=self._full_precision())
+                                                           f32=self._stem_dtype() == torch.float32)
             return self._forward_padded(xp, hs, ws), ratios
         key = ("images", plan.n, hs, ws)
         entry = self._graphs.get(key)
@@ -1473,12 +1289,9 @@ class Model:
             out = run()
         return {"graph": graph, "buf": buf, "xp": xp, "out": out, "capacity": capacity}
 
-    def _stem_dtype(self):
-        return torch.float32 if self._full_precision() else torch.float16
-
     def _resize_launch(self, *args, **kwargs):
         """engine.resize_launch into the stem buffer of the current precision."""
-        return (engine.resize_launch_f32 if self._full_precision() else engine.resize_launch)(*args, **kwargs)
+        return (engine.resize_launch_f32 if self._stem_dtype() == torch.float32 else engine.resize_launch)(*args, **kwargs)
 
     # ---- JPEG streams (the Image.open(path).convert("RGB") of odtk/data.py:50, then the raw-image path) ------------------
     def forward_jpeg(self, datas, resize=800, max_size=1333, canvas=None):

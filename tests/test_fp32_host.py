@@ -67,7 +67,7 @@ def test_conv_f32_rejects_bad_descriptors_without_a_gpu():
     assert L.odtk_conv2d_f32(ctypes.byref(d), None) == -1
 
 
-def test_set_precision_checks():
+def test_set_precision_argument_checks():
     assert set(FP32_BACKBONES) == {"ResNet18FPN", "ResNet34FPN", "ResNet50FPN", "ResNet101FPN", "ResNet152FPN"}
     for bb in ("ResNeXt50_32x4dFPN", "ResNeXt101_32x8dFPN", "MobileNetV2FPN"):
         with pytest.raises(ValueError, match="full precision"):
@@ -79,6 +79,3 @@ def test_set_precision_checks():
         m.set_precision("tf32")
     assert m.set_precision("fp32").precision == "fp32"
     assert m.set_precision("fp16").precision == "fp16"
-    m.merged_heads = False
-    with pytest.raises(ValueError, match="atlas"):
-        m.set_precision("fp32")

@@ -44,7 +44,7 @@ def gpu_info():
 
 
 def launch_names(backbone):
-    """Names of the fp32 convolution launches of one single-stream forward, in launch order (Model._features_f32 and
+    """Names of the fp32 convolution launches of one single-stream forward, in launch order (Model._stem, Model._features and
     the atlas heads: the class tower and its 5 final launches first, then the box tower)."""
     block, layers = RESNET_LAYERS[backbone]
     out = ["stem"]

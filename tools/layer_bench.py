@@ -3,8 +3,7 @@ launching stream, 2 warm-up + N timed launches each) and print / save a table:
     python tools/layer_bench.py [--batch 32] [--backbone ResNet50FPN] [--reps 5] [--tag name] [--rotated] [--out DIR]
 The calls are recorded by wrapping the engine's entry points while one eager forward runs, then replayed with the very
 same tensors (so shapes, strides, fused epilogues and the kernel variant chosen by the host code are the model's own).
-Environment toggles (ODTK_PDL, ODTK_FUSED_*) are read at first use: run once per setting and compare
-the JSON files.  Inputs of the small pyramid levels fit the L2, exactly as they do inside the real step."""
+The ODTK_PDL environment toggle is read at first use: run once per setting and compare the JSON files.  Inputs of the small pyramid levels fit the L2, exactly as they do inside the real step."""
 import argparse
 import collections
 import json

@@ -89,7 +89,7 @@ def fp32_cases():
     conv32(2, xa.shape[1], xa.shape[2], 256, 256, 3, x=xa, relu=True, out=ya, tile_tab=at["tab"])
     conv32(2, *sizes[1], 256, 256, 3, x=engine.AtlasView(xa, at["rows"][1], *sizes[1]), out=engine.AtlasView(ya, at["rows"][1], *sizes[1]))
     conv32(2, *sizes[2], 256, 256, 3, stride=2, out=engine.AtlasView(ya, at["rows"][3], *sizes[3]))
-    engine.relu_from_view_f32(engine.AtlasView(ya, at["rows"][3], *sizes[3]))
+    engine.relu_from_view(engine.AtlasView(ya, at["rows"][3], *sizes[3]))
     # input side
     engine.preprocess_u8_f32(torch.randint(0, 256, (2, 100, 130, 3), dtype=torch.uint8, generator=g).to(DEV))
     imgs = [torch.randint(0, 256, s, dtype=torch.uint8, generator=g) for s in ((30, 40, 3), (300, 170, 3), (900, 41, 3))]
@@ -216,7 +216,7 @@ def main():
         wq, s_w = engine.pack_weight_s8(torch.randn((256, 256, 3, 3), generator=g) * 0.05)
         engine.conv2d_s8(engine.AtlasView(at, 0, 32, 24), wq.to(DEV), (s_w * 0.05).to(DEV), None, 256, 3, relu=True, stride=2,
                          out=engine.AtlasView(at, 40, 16, 12), inv_out_scale=0.1)
-        engine.relu_from_view_s8(engine.AtlasView(at, 40, 16, 12))
+        engine.relu_from_view(engine.AtlasView(at, 40, 16, 12))
         torch.cuda.synchronize()
         print("conv_s8_ex atlas views ok", flush=True)
     if only in ("", "model"):
