@@ -320,6 +320,43 @@ typedef struct {
 } odtk_wgrad_t;
 long long odtk_conv_wgrad(const odtk_wgrad_t *desc, void *workspace, size_t workspace_size, odtk_stream_t stream);
 
+/* Weight gradient of one FPN convolution (1x1 stride 1, 3x3 stride 1 pad 1, or 3x3 stride 2 pad 1) whose output is ONE
+ * level of the gradient atlas and whose input is a dense tensor:
+ *   dw[co, ci, ky, kx] = sum over images and level pixels (r, c) of g[r, c, co] * x[s (r - g_row0) + ky - p, s c + kx - p, ci]
+ * (zero padding), db[co] = the sum of g over the level's rows only; fp32 results in the reference's layouts ([cout, cin,
+ * ksize, ksize], [cout]).
+ *   g   NHWC fp16 atlas [n, g_rows, g_width, cout_pad]: cout_pad a multiple of 64; zero outside the level's pixels within
+ *       the level's tiles and in the channels >= cout (the other levels' rows may hold anything)
+ *   x   NHWC fp16 [n, x_h, x_width, cin], cin % 128 == 0; the level is (x_h - 1) / s + 1 rows from g_row0 by
+ *       (x_width - 1) / s + 1 columns
+ *   tile_tab / tab_tiles   the level's tiles of the atlas tile table of odtk_conv_t (a contiguous slice of it)
+ * Any other (ksize, stride) returns ODTK_E_UNSUPPORTED.  Deterministic and with the workspace query of odtk_conv_wgrad. */
+typedef struct {
+  const void *g;
+  const void *x;
+  float *dw;            /* fp32 [cout, cin, ksize, ksize]                                                    */
+  float *db;            /* fp32 [cout] or NULL                                                               */
+  int n, g_rows, g_width, g_row0, cout_pad;
+  int x_h, x_width, cin, cout;
+  int ksize, stride;
+  const void *tile_tab;
+  int tab_tiles;
+} odtk_wgrad_ex_t;
+long long odtk_conv_wgrad_ex(const odtk_wgrad_ex_t *desc, void *workspace, size_t workspace_size, odtk_stream_t stream);
+
+/* The FPN's top-down pathway backward and pyramid7's input gradient, on fp16 NHWC atlases [n, rows, width, c], c % 8 == 0,
+ * levels given as (row0, h, w) at columns [0, w):
+ *   odtk_pool_add_f16   dst level += the pool x pool window sums of the src level (pool 2: the backward of the nearest 2x
+ *                       upsample-add, dP_l += sumpool2x2(dP_{l-1}); pool 1: a plain add), rounded once:
+ *                       fp16_rn((float)dst + ((s00 + s01) + (s10 + s11))); source pixels past the src level count as 0.
+ *                       src == dst is allowed when the two levels' rows are disjoint.
+ *   odtk_dilate_f16     dst[dst_row0 + 2y, 2x] = src[src_row0 + y, x] for the src_h x src_w level; nothing else of dst is
+ *                       written, so a zeroed dst keeps zeros at the odd positions                                       */
+int odtk_pool_add_f16(const void *src, void *dst, int n, int rows, int width, int c, int src_row0, int src_h, int src_w,
+                      int dst_row0, int dst_h, int dst_w, int pool, odtk_stream_t stream);
+int odtk_dilate_f16(const void *src, void *dst, int n, int rows, int width, int c, int src_row0, int src_h, int src_w,
+                    int dst_row0, odtk_stream_t stream);
+
 /* Loss gradients -> fp16 gradient atlas: level l's fp32 NCHW gradient [batch, channels, height, width] times *scale (a
  * DEVICE fp32 scalar, NULL for 1: the upstream autograd factor, e.g. a GradScaler scale, read without a host sync) lands at rows [row0, row0 + height) x columns [0, width) of the NHWC
  * fp16 atlas [batch, rows, atlas_width, cout_pad], channels >= `channels` as zeros.  Nothing else of the atlas is written:

@@ -57,6 +57,9 @@ SIGNATURES = {
                                [ctypes.c_longlong] * 4 + [ctypes.c_void_p]),
     "odtk_conv2d_f32": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     "odtk_conv_wgrad": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "odtk_conv_wgrad_ex": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "odtk_pool_add_f16": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 11 + [ctypes.c_void_p]),
+    "odtk_dilate_f16": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 8 + [ctypes.c_void_p]),
     "odtk_grad_to_atlas": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "odtk_conv2d_dgrad": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),

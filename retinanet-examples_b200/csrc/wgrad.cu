@@ -13,6 +13,13 @@
 //                   dimension of the NHWC boxes): 128B-swizzled MN-major descriptors + the transpose immediates.
 // Each CTA writes its fp32 partial tile; one reduce kernel sums the partials in split order and writes the [Cout, Cin, 3, 3]
 // parameter layout, so the result is bit-identical run to run.  The bias gradient is a fixed-order column sum of G.
+//
+// odtk_conv_wgrad_ex (the FPN layers) is a second compile-time instance of the same kernel: G is one level of the gradient
+// atlas (the level's slice of the tile table, first row g_row0), X a DENSE tensor read at (s * (r - g_row0) + ky - p,
+// s * c + kx - p) -- 1x1 (one tap, N = Cin), 3x3 stride 1, or 3x3 stride 2 through element-strided boxes (elementStrides 2
+// in H and W, as conv.cu loads odd-size stride-2 activations).  G is zero outside the level (gap rows, columns right of a
+// narrow level), so the in-bounds X values under it contribute nothing; the hardware zero fill outside X is the padding.
+// Its bias gradient sums the level's rows only.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -42,9 +49,11 @@ struct WgradParams {
   int n_tiles, mn_tiles;  // N tiles (9 * cin / 128); M x N tiles
   int cin, cout_pad;
   int ktiles, splits;     // K tiles (images x tiles) and the CTAs each output tile is split over
-  float *ws;              // fp32 partials [splits, cout_pad, 9 * cin]
+  float *ws;              // fp32 partials [splits, cout_pad, taps * cin]
+  int ksize, stride, g_row0;   // the wgrad_ex instance only: taps ksize^2, X pixel s * (r - g_row0) + tap - ksize / 2
 };
 
+template <bool kEx>
 __global__ void __launch_bounds__(kWThreads, 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX,
              const __grid_constant__ WgradParams p) {
@@ -72,7 +81,8 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
   if (wg == 0) {
     // ===================================== TMA producer =====================================
     if (tid != 0) return;
-    const int dy = tap / 3 - 1, dx = tap % 3 - 1;
+    int dy = tap / 3 - 1, dx = tap % 3 - 1;
+    if constexpr (kEx) { dy = tap / p.ksize - p.ksize / 2; dx = tap % p.ksize - p.ksize / 2; }
     int stage = 0;
     uint32_t phase = 0;
     for (int kt = k_begin; kt < k_end; kt++) {
@@ -85,8 +95,10 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
       mbar_arrive_expect_tx(&full[stage], (uint32_t)kWStageBytes);
       tma_load_4d(s, &tmG, &full[stage], m0, w0, h0, img);
       tma_load_4d(s + kBox, &tmG, &full[stage], m0 + 64, w0, h0, img);   // past cout_pad: zero-filled, never stored
-      tma_load_4d(s + 2 * kBox, &tmX, &full[stage], ci0, w0 + dx, h0 + dy, img);
-      tma_load_4d(s + 3 * kBox, &tmX, &full[stage], ci0 + 64, w0 + dx, h0 + dy, img);
+      int xw = w0 + dx, xh = h0 + dy;
+      if constexpr (kEx) { xw = p.stride * w0 + dx; xh = p.stride * (h0 - p.g_row0) + dy; }
+      tma_load_4d(s + 2 * kBox, &tmX, &full[stage], ci0, xw, xh, img);
+      tma_load_4d(s + 3 * kBox, &tmX, &full[stage], ci0 + 64, xw, xh, img);
       if (++stage == kWStages) { stage = 0; phase ^= 1u; }
     }
     return;
@@ -118,7 +130,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
   wgmma_wait<0>();
 
   // thread holds rows (output channels) r and r + 8, columns 8 j + 2 q (+1)
-  const int N = 9 * p.cin;
+  const int N = (kEx ? p.ksize * p.ksize : 9) * p.cin;
   float *ws = p.ws + (size_t)split * p.cout_pad * N;
 #pragma unroll
   for (int i = 0; i < 2; i++) {
@@ -148,18 +160,41 @@ __global__ void bgrad_partial_kernel(const __half *g, long long rows, int cpad, 
   }
 }
 
+// bias gradient of one atlas level, pass 1: the level's pixels of all images in order (img, row, column), `slab` = rows x
+// atlas width of them per image, images `pitch` elements apart (g points at the level's first row); block b sums pixels
+// [px * b / B, px * (b + 1) / B), one thread per channel pair
+__global__ void bgrad_level_partial_kernel(const __half *g, long long px, long long slab, long long pitch, int cpad,
+                                           float *part) {
+  const long long r0 = px * blockIdx.x / gridDim.x, r1 = px * (blockIdx.x + 1) / gridDim.x;
+  for (int c = 2 * threadIdx.x; c < cpad; c += 2 * blockDim.x) {
+    float s0 = 0.0f, s1 = 0.0f;
+    const long long img = r0 / slab;
+    long long rem = r0 - img * slab;
+    const __half *col = g + img * pitch + c;
+    for (long long r = r0; r < r1; r++) {
+      const float2 v = __half22float2(*reinterpret_cast<const __half2 *>(col + rem * cpad));
+      s0 += v.x;
+      s1 += v.y;
+      if (++rem == slab) { rem = 0; col += pitch; }
+    }
+    part[(size_t)blockIdx.x * cpad + c] = s0;
+    part[(size_t)blockIdx.x * cpad + c + 1] = s1;
+  }
+}
+
 // dw[co, ci, tap] = sum over splits (in order) of ws[split, co, tap * cin + ci]; db[co] = sum over blocks of part[b, co]
+template <int kTaps>
 __global__ void wgrad_reduce_kernel(const float *ws, int splits, int cout, int cout_pad, int cin, float *dw,
                                     const float *part, int nparts, float *db) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  const long long N = 9ll * cin;
+  const long long N = (long long)kTaps * cin;
   if (i < (long long)cout * cin) {
     const int co = (int)(i / cin), ci = (int)(i - (long long)co * cin);
-    for (int t = 0; t < 9; t++) {
+    for (int t = 0; t < kTaps; t++) {
       const float *src = ws + (long long)co * N + (long long)t * cin + ci;
       float s = 0.0f;
       for (int k = 0; k < splits; k++) s += src[(long long)k * cout_pad * N];
-      dw[i * 9 + t] = s;
+      dw[i * kTaps + t] = s;
     }
   }
   if (db && i < cout) {
@@ -214,7 +249,9 @@ bool wgrad_device_ready() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return false;
   std::lock_guard<std::mutex> lk(g_wgrad_mu);
   if (g_wgrad_ready[dev]) return true;
-  if (cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSmem) != cudaSuccess) return false;
+  if (cudaFuncSetAttribute(wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSmem) != cudaSuccess ||
+      cudaFuncSetAttribute(wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSmem) != cudaSuccess)
+    return false;
   g_wgrad_ready[dev] = true;
   return true;
 }
@@ -289,12 +326,12 @@ extern "C" long long odtk_conv_wgrad(const odtk_wgrad_t *d, void *workspace, siz
   float *part = (float *)((char *)workspace + ws_part);
   {
     OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    wgrad_kernel<<<mn_tiles * splits, kWThreads, kWSmem, stream>>>(tmG, tmX, p);
+    wgrad_kernel<false><<<mn_tiles * splits, kWThreads, kWSmem, stream>>>(tmG, tmX, p);
     if (d->db)
       bgrad_partial_kernel<<<kBiasBlocks, 128, 0, stream>>>((const __half *)d->g, (long long)d->n * d->h * d->width,
                                                            d->cout_pad, part);
     const long long elems = (long long)d->cout * d->cin;
-    wgrad_reduce_kernel<<<(unsigned)((elems + 255) / 256), 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin,
+    wgrad_reduce_kernel<9><<<(unsigned)((elems + 255) / 256), 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin,
                                                                              d->dw, part, kBiasBlocks, d->db);
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
@@ -325,6 +362,185 @@ extern "C" int odtk_grad_to_atlas(int batch, int num_levels, const odtk_grad_lev
     OdtkProfScope prof(ODTK_PROF_LAYER, stream);
     grad_to_atlas_kernel<<<dim3((unsigned)blocks, (unsigned)(cout_pad / 32), (unsigned)batch), dim3(32, 8), 0, stream>>>(
         L, num_levels, channels, scale, (__half *)atlas, rows, atlas_width, cout_pad);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" long long odtk_conv_wgrad_ex(const odtk_wgrad_ex_t *d, void *workspace, size_t workspace_size, odtk_stream_t stream_) {
+  if (!d || !d->g || !d->x || !d->dw || !d->tile_tab) return ODTK_E_INVALID;
+  const bool mode_ok = (d->ksize == 1 && d->stride == 1) || (d->ksize == 3 && (d->stride == 1 || d->stride == 2));
+  if (!mode_ok) return ODTK_E_UNSUPPORTED;
+  if (d->n <= 0 || d->g_rows <= 0 || d->g_width <= 0 || d->g_row0 < 0 || d->x_h <= 0 || d->x_width <= 0 || d->cin <= 0 ||
+      d->cout <= 0 || d->cout_pad <= 0 || d->tab_tiles <= 0)
+    return ODTK_E_INVALID;
+  if (d->cout > d->cout_pad) return ODTK_E_INVALID;
+  if (d->cin % 128 || d->cout_pad % 64) return ODTK_E_UNSUPPORTED;   // 128-wide N tiles inside one tap; 64-channel G boxes
+  // the level is the convolution's output: (x - 1) / s + 1 rows and columns from row g_row0 of the atlas
+  const int lh = (d->x_h - 1) / d->stride + 1, lw = (d->x_width - 1) / d->stride + 1;
+  if ((long long)d->g_row0 + lh > d->g_rows || lw > d->g_width) return ODTK_E_INVALID;
+  if ((long long)d->n * d->g_rows * d->g_width >= (1ll << 31) || (long long)d->n * d->x_h * d->x_width >= (1ll << 31))
+    return ODTK_E_UNSUPPORTED;
+  if (((uintptr_t)d->g | (uintptr_t)d->x | (uintptr_t)d->tile_tab) & 15) return ODTK_E_INVALID;
+  const long long ktiles = (long long)d->n * d->tab_tiles;
+  if (ktiles >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  const int taps = d->ksize * d->ksize;
+  const int N = taps * d->cin;
+  const int n_tiles = N / 128, m_tiles = (d->cout_pad + 127) / 128;
+  const int mn_tiles = m_tiles * n_tiles;
+  const int sms = odtk_sm_count();
+  const int splits = choose_splits(mn_tiles, (int)ktiles, sms);
+  const size_t ws_part = odtk_align_up((size_t)splits * d->cout_pad * N * sizeof(float));
+  const size_t ws_bias = odtk_align_up((size_t)kBiasBlocks * d->cout_pad * sizeof(float));
+  const size_t need = ws_part + ws_bias;
+  if (!workspace || workspace_size == 0) return (long long)need;
+  if (workspace_size < need) return ODTK_E_WORKSPACE;
+  if (!wgrad_device_ready()) return ODTK_E_CUDA;
+  cudaStream_t stream = (cudaStream_t)stream_;
+
+  CUtensorMap tmG, tmX;
+  {
+    const uint64_t C = (uint64_t)d->cout_pad, W = (uint64_t)d->g_width, H = (uint64_t)d->g_rows;
+    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
+    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
+    uint32_t box[4] = {64, 16, 8, 1};
+    if (!encode_map(&tmG, d->g, 4, dims, str, box)) return ODTK_E_CUDA;
+  }
+  {
+    // stride 2: boxDim = 2 x the pixels, elementStrides 2 -- the TMA unit loads every second pixel of a 32 x 16 window
+    const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->x_width, H = (uint64_t)d->x_h;
+    const uint32_t s = (uint32_t)d->stride;
+    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
+    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
+    uint32_t box[4] = {64, 16 * s, 8 * s, 1};
+    uint32_t estr[4] = {1, s, s, 1};
+    if (!encode_map(&tmX, d->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, estr)) return ODTK_E_CUDA;
+  }
+  WgradParams p;
+  memset(&p, 0, sizeof p);
+  p.tile_tab = (const int4 *)d->tile_tab;
+  p.tab_tiles = d->tab_tiles;
+  p.n_tiles = n_tiles;
+  p.mn_tiles = mn_tiles;
+  p.cin = d->cin;
+  p.cout_pad = d->cout_pad;
+  p.ktiles = (int)ktiles;
+  p.splits = splits;
+  p.ws = (float *)workspace;
+  p.ksize = d->ksize;
+  p.stride = d->stride;
+  p.g_row0 = d->g_row0;
+  float *part = (float *)((char *)workspace + ws_part);
+  {
+    OdtkProfScope prof(ODTK_PROF_CONV, stream);
+    wgrad_kernel<true><<<mn_tiles * splits, kWThreads, kWSmem, stream>>>(tmG, tmX, p);
+    if (d->db) {
+      const long long slab = (long long)lh * d->g_width;
+      bgrad_level_partial_kernel<<<kBiasBlocks, 128, 0, stream>>>(
+          (const __half *)d->g + (size_t)d->g_row0 * d->g_width * d->cout_pad, (long long)d->n * slab, slab,
+          (long long)d->g_rows * d->g_width * d->cout_pad, d->cout_pad, part);
+    }
+    const long long elems = (long long)d->cout * d->cin;
+    const unsigned blocks = (unsigned)((elems + 255) / 256);
+    if (taps == 1)
+      wgrad_reduce_kernel<1><<<blocks, 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin, d->dw, part, kBiasBlocks, d->db);
+    else
+      wgrad_reduce_kernel<9><<<blocks, 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin, d->dw, part, kBiasBlocks, d->db);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+// ---- the FPN's top-down pathway and pyramid7's input gradient: two small HBM-bound kernels over fp16 NHWC atlases -------
+namespace {
+
+// dst level (row0, h, w) += the pool x pool sums of src (row0, h, w) in fp32, 8 channels per thread:
+//   out = fp16_rn((float)dst + ((s00 + s01) + (s10 + s11)))   (pool 2; pool 1: fp16_rn((float)dst + s00))
+// source pixels past the source level count as 0
+__global__ void pool_add_kernel(const __half *src, __half *dst, int n, int rows, int width, int c8, int sr0, int sh, int sw,
+                                int dr0, int dh, int dw, int pool) {
+  const long long total = (long long)n * dh * dw * c8;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int ch = (int)(i % c8);
+  long long t = i / c8;
+  const int x = (int)(t % dw);
+  t /= dw;
+  const int y = (int)(t % dh);
+  const int img = (int)(t / dh);
+  const long long img0 = (long long)img * rows;
+  float s[4][8];
+#pragma unroll
+  for (int k = 0; k < 4; k++) {
+    const int sy = pool * y + (k >> 1), sx = pool * x + (k & 1);
+    const bool in = (k == 0 || pool == 2) && sy < sh && sx < sw;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (in) v = *reinterpret_cast<const uint4 *>(src + (((img0 + sr0 + sy) * width + sx) * c8 + ch) * 8);
+    const __half2 *h2 = reinterpret_cast<const __half2 *>(&v);
+#pragma unroll
+    for (int j = 0; j < 4; j++) { const float2 f = __half22float2(h2[j]); s[k][2 * j] = f.x; s[k][2 * j + 1] = f.y; }
+  }
+  __half *o = dst + (((img0 + dr0 + y) * width + x) * c8 + ch) * 8;
+  uint4 v = *reinterpret_cast<const uint4 *>(o);
+  __half2 *h2 = reinterpret_cast<__half2 *>(&v);
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    const float2 f = __half22float2(h2[j]);
+    const float a = f.x + ((s[0][2 * j] + s[1][2 * j]) + (s[2][2 * j] + s[3][2 * j]));
+    const float b = f.y + ((s[0][2 * j + 1] + s[1][2 * j + 1]) + (s[2][2 * j + 1] + s[3][2 * j + 1]));
+    h2[j] = __floats2half2_rn(a, b);
+  }
+  *reinterpret_cast<uint4 *>(o) = v;
+}
+
+// dst[dr0 + 2y, 2x] = src[sr0 + y, x] over the h x w source level; nothing else of dst is written
+__global__ void dilate_kernel(const __half *src, __half *dst, int n, int rows, int width, int c8, int sr0, int h, int w, int dr0) {
+  const long long total = (long long)n * h * w * c8;
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int ch = (int)(i % c8);
+  long long t = i / c8;
+  const int x = (int)(t % w);
+  t /= w;
+  const int y = (int)(t % h);
+  const long long img0 = (t / h) * rows;
+  *reinterpret_cast<uint4 *>(dst + (((img0 + dr0 + 2 * y) * width + 2 * x) * c8 + ch) * 8) =
+      *reinterpret_cast<const uint4 *>(src + (((img0 + sr0 + y) * width + x) * c8 + ch) * 8);
+}
+
+}  // namespace
+
+extern "C" int odtk_pool_add_f16(const void *src, void *dst, int n, int rows, int width, int c, int src_row0, int src_h,
+                                 int src_w, int dst_row0, int dst_h, int dst_w, int pool, odtk_stream_t stream_) {
+  if (!src || !dst || n <= 0 || rows <= 0 || width <= 0 || c <= 0 || (c % 8)) return ODTK_E_INVALID;
+  if (pool != 1 && pool != 2) return ODTK_E_UNSUPPORTED;
+  if (src_row0 < 0 || src_h <= 0 || src_w <= 0 || dst_row0 < 0 || dst_h <= 0 || dst_w <= 0) return ODTK_E_INVALID;
+  if ((long long)src_row0 + src_h > rows || src_w > width || (long long)dst_row0 + dst_h > rows || dst_w > width)
+    return ODTK_E_INVALID;
+  if (src == dst && src_row0 < dst_row0 + dst_h && dst_row0 < src_row0 + src_h) return ODTK_E_INVALID;   // in place: disjoint levels
+  if (((uintptr_t)src | (uintptr_t)dst) & 15) return ODTK_E_INVALID;
+  const long long total = (long long)n * dst_h * dst_w * (c / 8);
+  if ((long long)n * rows * width * c >= (1ll << 40)) return ODTK_E_UNSUPPORTED;
+  {
+    OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+    pool_add_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(
+        (const __half *)src, (__half *)dst, n, rows, width, c / 8, src_row0, src_h, src_w, dst_row0, dst_h, dst_w, pool);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_dilate_f16(const void *src, void *dst, int n, int rows, int width, int c, int src_row0, int src_h,
+                               int src_w, int dst_row0, odtk_stream_t stream_) {
+  if (!src || !dst || n <= 0 || rows <= 0 || width <= 0 || c <= 0 || (c % 8)) return ODTK_E_INVALID;
+  if (src_row0 < 0 || src_h <= 0 || src_w <= 0 || dst_row0 < 0) return ODTK_E_INVALID;
+  if ((long long)src_row0 + src_h > rows || src_w > width || 2ll * (src_w - 1) >= width ||
+      (long long)dst_row0 + 2ll * (src_h - 1) >= rows)
+    return ODTK_E_INVALID;
+  if (((uintptr_t)src | (uintptr_t)dst) & 15) return ODTK_E_INVALID;
+  const long long total = (long long)n * src_h * src_w * (c / 8);
+  if ((long long)n * rows * width * c >= (1ll << 40)) return ODTK_E_UNSUPPORTED;
+  {
+    OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+    dilate_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(
+        (const __half *)src, (__half *)dst, n, rows, width, c / 8, src_row0, src_h, src_w, dst_row0);
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }

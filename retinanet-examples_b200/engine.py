@@ -856,6 +856,85 @@ def conv_wgrad(g, x, cout, tile_tab=None, bias=True):
     return dw, db
 
 
+class WgradExDesc(ctypes.Structure):
+    """odtk_wgrad_ex_t (include/odtk_b200.h)."""
+    _fields_ = [("g", ctypes.c_void_p), ("x", ctypes.c_void_p), ("dw", ctypes.c_void_p), ("db", ctypes.c_void_p)] + \
+               [(f, ctypes.c_int) for f in ("n", "g_rows", "g_width", "g_row0", "cout_pad", "x_h", "x_width", "cin", "cout",
+                                            "ksize", "stride")] + \
+               [("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int)]
+
+
+def conv_wgrad_ex(g, x, cout, ksize, stride, tile_tab, g_row0, bias=True):
+    """Weight (and bias) gradient of an FPN convolution (odtk_conv_wgrad_ex): 1x1 stride 1, 3x3 stride 1 or 3x3 stride 2
+    (pad ksize // 2).  g: the NHWC fp16 gradient atlas [N, rows, width, Cout_pad] whose level at row g_row0 is the
+    convolution's output ((H - 1) // stride + 1 rows and columns; zero in its tiles outside the level and in the channels
+    >= cout), tile_tab: that level's slice of the atlas tile table, x: the dense NHWC fp16 input [N, H, W, Cin].  Returns
+    fp32 (dw [cout, Cin, k, k], db [cout] or None: the level's rows only), bit-identical run to run."""
+    assert g.is_cuda and g.dtype == torch.float16 and g.is_contiguous()
+    assert x.is_cuda and x.dtype == torch.float16 and x.is_contiguous() and x.device == g.device
+    assert tile_tab is not None and tile_tab.is_contiguous() and tile_tab.device == g.device
+    n, rows, aw, cpad = g.shape
+    xn, xh, xw, cin = x.shape
+    assert xn == n
+    dw = torch.empty((cout, cin, ksize, ksize), dtype=torch.float32, device=g.device)
+    db = torch.empty((cout,), dtype=torch.float32, device=g.device) if bias else None
+    d = WgradExDesc()
+    d.g, d.x, d.dw, d.db = g.data_ptr(), x.data_ptr(), dw.data_ptr(), (db.data_ptr() if db is not None else None)
+    d.n, d.g_rows, d.g_width, d.g_row0, d.cout_pad = n, rows, aw, int(g_row0), cpad
+    d.x_h, d.x_width, d.cin, d.cout, d.ksize, d.stride = xh, xw, cin, cout, ksize, stride
+    d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    L = _lib.lib()
+    size = _lib.check(L.odtk_conv_wgrad_ex(ctypes.byref(d), None, 0, None), "conv_wgrad_ex (workspace query)")
+    ws = torch.empty(int(size), dtype=torch.uint8, device=g.device)
+    _lib.check(L.odtk_conv_wgrad_ex(ctypes.byref(d), ctypes.c_void_p(ws.data_ptr()), size, _stream()), "conv_wgrad_ex")
+    STATS["launches"] += 1
+    if STATS["trace"] is not None:
+        px = n * ((xh - 1) // stride + 1) * ((xw - 1) // stride + 1)
+        # the level's G once, X once per tap (1x1 and stride 2: the pixels it samples), the fp32 partials and the result
+        xpx = n * xh * xw if (ksize == 3 and stride == 1) else px
+        _trace("wgrad%dx%d%s" % (ksize, ksize, "s2" if stride == 2 else ""), 2 * px * cout * ksize * ksize * cin,
+               px * cpad * 2 + xpx * cin * 2 + int(size) * 2 + dw.numel() * 4, n=n, h=xh, w=xw, cin=cin, cout=cout,
+               stride=stride)
+    return dw, db
+
+
+def _level_args(atlas, level):
+    n, rows, aw, c = atlas.shape
+    return [n, rows, aw, c] + [int(v) for v in level]
+
+
+def pool_add(src, dst, src_level, dst_level, pool=2):
+    """dst level += the pool x pool window sums of the src level (odtk_pool_add_f16), both NHWC fp16 atlases of one
+    geometry, levels (row0, h, w): pool 2 is the backward of the FPN's nearest 2x upsample-add, pool 1 a plain add.
+    fp16_rn((float)dst + ((s00 + s01) + (s10 + s11))).  src may be dst when the levels' rows are disjoint."""
+    for t in (src, dst):
+        assert t.is_cuda and t.dtype == torch.float16 and t.is_contiguous() and t.shape == dst.shape
+    args = _level_args(dst, src_level) + [int(v) for v in dst_level] + [pool]
+    _lib.check(_lib.lib().odtk_pool_add_f16(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(dst.data_ptr()), *args,
+                                            _stream()), "pool_add_f16")
+    STATS["launches"] += 1
+    n, _, _, c = dst.shape
+    px = n * int(dst_level[1]) * int(dst_level[2])
+    _trace("pool_add", px * c * pool * pool, px * c * 2 * (2 + pool * pool), n=n, h=int(dst_level[1]), w=int(dst_level[2]),
+           cin=c, cout=c)
+    return dst
+
+
+def dilate(src, dst, src_level, dst_row0):
+    """dst[dst_row0 + 2y, 2x] = src level (row0, h, w) [y, x] (odtk_dilate_f16), NHWC fp16 atlases of one geometry;
+    nothing else of dst is written."""
+    for t in (src, dst):
+        assert t.is_cuda and t.dtype == torch.float16 and t.is_contiguous() and t.shape == dst.shape
+    args = _level_args(dst, src_level) + [int(dst_row0)]
+    _lib.check(_lib.lib().odtk_dilate_f16(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(dst.data_ptr()), *args, _stream()),
+               "dilate_f16")
+    STATS["launches"] += 1
+    n, _, _, c = dst.shape
+    px = n * int(src_level[1]) * int(src_level[2])
+    _trace("dilate", 0, px * c * 4, n=n, h=int(src_level[1]), w=int(src_level[2]), cin=c, cout=c)
+    return dst
+
+
 def grad_to_atlas(grads, rows0, scale, atlas):
     """Per-level fp32 NCHW loss gradients [B, C, H_l, W_l] * scale (a number, or a one-element fp32 tensor on the atlas's
     device, read there without a host sync) -> the fp16 NHWC gradient atlas [B, rows, width, C_pad]

@@ -309,9 +309,12 @@ class _ConvF32:
                                  tile_tab=tile_tab)
 
 
+FPN_LAYERS = ("lateral3", "lateral4", "lateral5", "pyramid6", "pyramid7", "smooth3", "smooth4", "smooth5")   # fpn.py:26-33
+
+
 class _HeadsTrain(torch.autograd.Function):
-    """(cls_loss, box_loss) of the training forward as a function of the head parameters (Model._train_forward /
-    Model._train_backward)."""
+    """(cls_loss, box_loss) of the training forward as a function of the parameters of the training scope (the heads, or
+    the FPN and the heads: Model._train_forward / Model._train_backward)."""
 
     @staticmethod
     def forward(ctx, model, x, targets, *params):
@@ -375,10 +378,11 @@ class Model:
         self._calib_hook = None
         self._calib_net = False       # calibration also records the network scope's tensors
         self._f32 = None              # full precision: split-TF32 weights of every layer (packed on first use)
-        self._params = None           # trainable head parameters (created by named_parameters / parameters)
-        self._param_versions = {}     # (head, layer index) -> the parameters' _version when their fp16 weights were packed
+        self._params = None           # trainable parameters by name (created by named_parameters / parameters)
+        self.train_scope = "heads"    # "heads" or "fpn": which parameters named_parameters lists (set_train_scope)
+        self._param_versions = {}     # weight name -> the layer's (weight, bias) _version when its fp16 weights were packed
         self._sd_versions = {}        # parameter name -> its _version when it was last copied into the state dict
-        self._dgrad_w = {}            # (head, layer index) -> (weight _version, input-gradient weights of pack_weight_dgrad)
+        self._dgrad_w = {}            # (head, layer index) / FPN layer -> (weight _version, pack_weight_dgrad weights)
         self._fwd_gen = 0             # counts forward passes: a backward must follow its own forward
         # test hooks, both only while want_atlas_grad is set: the training backward also computes d(loss)/d(atlas) into
         # last_atlas_grad, which ALIASES a gradient buffer of the atlas geometry (the next backward overwrites it), and
@@ -454,28 +458,64 @@ class Model:
             self._sd_versions = {n: p._version for n, p in self._params.items()}
         return self
 
-    # ---- trainable head parameters ----------------------------------------------------------------------------------
+    # ---- trainable parameters ---------------------------------------------------------------------------------------
     def _head_param_names(self):
         return ["%s.%d.%s" % (head, i, k) for head in ("cls_head", "box_head") for i in (0, 2, 4, 6, 8) for k in ("weight", "bias")]
 
+    def _fpn_param_names(self):
+        return ["backbones.%s.%s.%s" % (self.backbone, l, k) for l in FPN_LAYERS for k in ("weight", "bias")]
+
+    def _param_names(self):
+        """The training scope's parameter names in the reference's named_parameters() order: the FPN's before the heads'."""
+        return (self._fpn_param_names() if self.train_scope == "fpn" else []) + self._head_param_names()
+
+    def _trainable_layers(self):
+        """(packed-layer key, index in a head list or None, stride, weight name, bias name) of every layer whose
+        parameters exist."""
+        layers = [(l, None, 2 if l.startswith("pyramid") else 1, "backbones.%s.%s.weight" % (self.backbone, l),
+                   "backbones.%s.%s.bias" % (self.backbone, l)) for l in FPN_LAYERS]
+        layers += [(head, k, 1, "%s.%d.weight" % (head, i), "%s.%d.bias" % (head, i))
+                   for head in ("cls_head", "box_head") for k, i in enumerate((0, 2, 4, 6, 8))]
+        return [t for t in layers if self._params is not None and t[3] in self._params]
+
+    def set_train_scope(self, scope):
+        """What training updates: "heads" (default: the class and box heads, the backbone and the FPN frozen) or "fpn"
+        (the FPN's 16 tensors as well; ResNet18/34/50/101/152 and ResNeXt FPNs -- not MobileNetV2FPN, whose 64-channel
+        padded C3 does not fit the weight-gradient GEMM's 128-channel tiles).  named_parameters / parameters list the
+        scope's tensors, so build the optimizer after this call.  A parameter keeps its identity across scope changes.
+        Returns self."""
+        if scope not in ("heads", "fpn"):
+            raise ValueError("training scope must be 'heads' or 'fpn', got %r" % (scope,))
+        if scope == "fpn" and self.backbone in MOBILENET:
+            raise ValueError("the fpn training scope needs C3 with a multiple of 128 channels; %s's padded C3 has 64 channels"
+                             % self.backbone)
+        self.train_scope = scope
+        return self
+
     def named_parameters(self, prefix="", recurse=True):
-        """(name, parameter) of the class and box heads, with the reference's names, shapes and order
-        (cls_head.{0,2,4,6,8}.{weight,bias}, then box_head.*): fp32 CUDA leaf tensors, created from the state dict on the
-        first call (after .cuda()).  The backbone and the FPN are frozen: they have no backward kernels here and are not
-        listed.  Once the parameters exist, the training-mode forward returns losses connected to them (the head
-        backward runs on the sm_90a kernels: odtk_conv_wgrad, odtk_conv2d_dgrad), and every forward uses their current
-        values (the fp16 weights are repacked when a parameter changed, e.g. after optimizer.step())."""
-        if self._params is None:
+        """(name, parameter) of the training scope (set_train_scope), with the reference's names, shapes and order: the
+        default scope "heads" lists cls_head.{0,2,4,6,8}.{weight,bias}, then box_head.*; scope "fpn" lists
+        backbones.<backbone>.{lateral3,lateral4,lateral5,pyramid6,pyramid7,smooth3,smooth4,smooth5}.{weight,bias} first.
+        fp32 CUDA leaf tensors, created from the state dict on first request (after .cuda()).  The backbone is frozen: it
+        has no backward kernels here and is never listed.  Once the parameters exist, the training-mode forward returns
+        losses connected to them (the backward runs on the sm_90a kernels: odtk_conv_wgrad, odtk_conv_wgrad_ex,
+        odtk_conv2d_dgrad, odtk_pool_add_f16, odtk_dilate_f16), and every forward uses their current values (the fp16
+        weights are repacked when a parameter changed, e.g. after optimizer.step())."""
+        names = self._param_names()
+        if self._params is None or any(n not in self._params for n in names):
             if self._packed is None or self.device is None:
                 raise RuntimeError("call .cuda() before asking for parameters: they are CUDA tensors")
-            self._params = {n: torch.nn.Parameter(self._sd[n].to(self.device, torch.float32).clone())
-                            for n in self._head_param_names()}
-            self._param_versions = {(head, i): (self._params["%s.%d.weight" % (head, i)]._version,
-                                                self._params["%s.%d.bias" % (head, i)]._version)
-                                    for head in ("cls_head", "box_head") for i in (0, 2, 4, 6, 8)}
-            self._sd_versions = {n: p._version for n, p in self._params.items()}
-        for n, p in self._params.items():
-            yield prefix + n, p
+            if self._params is None:
+                self._params = {}
+            for n in names:
+                if n not in self._params:
+                    self._params[n] = torch.nn.Parameter(self._sd[n].to(self.device, torch.float32).clone())
+                    self._sd_versions[n] = self._params[n]._version
+            for _, _, _, wn, bn in self._trainable_layers():
+                if wn not in self._param_versions:      # the packed layer holds the state dict's values
+                    self._param_versions[wn] = (self._params[wn]._version, self._params[bn]._version)
+        for n in names:
+            yield prefix + n, self._params[n]
 
     def parameters(self, recurse=True):
         for _, p in self.named_parameters():
@@ -489,7 +529,7 @@ class Model:
                 p.grad.zero_()
 
     def _params_to_sd(self):
-        """Copy every head parameter that changed since its last copy into the state dict (read by state_dict(), save()
+        """Copy every parameter that changed since its last copy into the state dict (read by state_dict(), save()
         and the fp32 / INT8 weight packing)."""
         if self._params is not None:
             for n, p in self._params.items():
@@ -498,21 +538,24 @@ class Model:
                     self._sd_versions[n] = p._version
 
     def _sync_params(self):
-        """Repack the fp16 weights of every head layer whose parameters changed since they were packed; counts the
-        forward pass."""
+        """Repack the fp16 weights of every head or FPN layer whose parameters changed since they were packed (then the
+        fp32 weights are dropped, the INT8 network is rebuilt and CUDA graphs are recaptured); counts the forward pass."""
         self._fwd_gen += 1
         if self._params is None or self._packed is None:
             return
         P, changed = self._packed, False
-        for head in ("cls_head", "box_head"):
-            for k, i in enumerate((0, 2, 4, 6, 8)):
-                w, b = self._params["%s.%d.weight" % (head, i)], self._params["%s.%d.bias" % (head, i)]
-                v = (w._version, b._version)
-                if self._param_versions.get((head, i)) != v:
-                    with torch.no_grad():
-                        P[head][k] = _Conv(w.detach(), b.detach().clone(), 1, self.device)
-                    self._param_versions[(head, i)] = v
-                    changed = True
+        for key, k, stride, wn, bn in self._trainable_layers():
+            w, b = self._params[wn], self._params[bn]
+            v = (w._version, b._version)
+            if self._param_versions.get(wn) != v:
+                with torch.no_grad():
+                    conv = _Conv(w.detach(), b.detach().clone(), stride, self.device)
+                if k is None:
+                    P[key] = conv
+                else:
+                    P[key][k] = conv
+                self._param_versions[wn] = v
+                changed = True
         if changed:
             self._f32 = None
             if self._int8 is not None:
@@ -539,8 +582,10 @@ class Model:
 
     def train(self, mode=True):
         """Training-mode forward (odtk/model.py:130-138): `model([images, targets])` returns (cls_loss, box_loss).  Once
-        the head parameters exist (named_parameters / parameters), the losses are connected to them and .backward()
-        fills their .grad on the sm_90a backward kernels; the backbone and the FPN are frozen (no backward kernels).
+        the parameters of the training scope exist (set_train_scope, then named_parameters / parameters), the losses are
+        connected to them and .backward() fills their .grad on the sm_90a backward kernels: the heads, and in scope "fpn"
+        the FPN too; the backbone is frozen (no backward kernels).  An INT8 network table calibrated before training
+        describes the old weights: recalibrate after training.
         Without them, the losses and -- `_compute_loss(..., with_grad=True)` -- their gradients w.r.t. the head outputs
         are what this provides.  The training forward runs in fp16 over the pyramid atlas whatever set_precision chose."""
         self.training = bool(mode)
@@ -571,6 +616,7 @@ class Model:
         self._int8 = None
         if self._int8_table is None or self.device is None:
             return
+        self._params_to_sd()              # trained parameters
         S, sd, dev = self._int8_table["scales"], self._sd, self.device
         names = calib.table_tensors(self.backbone, self.int8_scope)
         walk = network_walk(self.backbone)
@@ -814,8 +860,8 @@ class Model:
             return self._features(self._stem(padded=(xp, x.shape[2], x.shape[3]))), (x.shape[2], x.shape[3])
         return self._features(self._stem(self._to_nhwc_half(x))), (x.shape[2], x.shape[3])
 
-    def _features(self, x):
-        """`x`: the POOLED stem output [N, H/4, W/4, C] (from _stem).  The residual blocks, then the FPN.  fp16 blocks whose
+    def _features(self, x, keep=None):
+        """`x`: the POOLED stem output [N, H/4, W/4, C] (from _stem).  The residual blocks, then the FPN (`keep`: see _fpn).  fp16 blocks whose
         shapes fit take the fused bottleneck kernels; every other block runs its downsample, then its convolutions with
         the residual added in the last one's epilogue.  The INT8 network quantises C3 once, at its first s8 block."""
         if self.backbone in MOBILENET:
@@ -882,12 +928,13 @@ class Model:
                 outs[blk["level"]] = x
         if hook is not None:
             hook("backbones.%s.features.layer2" % self.backbone, outs[3])
-        return self._fpn(outs[3], outs[4], outs[5])
+        return self._fpn(outs[3], outs[4], outs[5], keep)
 
-    def _fpn(self, c3, c4, c5):
+    def _fpn(self, c3, c4, c5, keep=None):
         """FPN (odtk/backbones/fpn.py:45-61) on the three backbone taps, into the pyramid atlas: the five levels stacked in
         ONE zero-separated NHWC buffer of the activation dtype, so that every head-tower layer is one launch over all
-        levels instead of five.  Returns the five level views."""
+        levels instead of five.  Returns the five level views; a `keep` dict receives what the FPN backward reads: c3-c5,
+        the pre-smooth p3-p5 and relu(P6)."""
         P = self._net()
         p5 = P["lateral5"](c5)
         p4 = P["lateral4"](c4, upsample=p5)
@@ -905,7 +952,10 @@ class Model:
         P["smooth4"](p4, out=v[1])
         P["smooth5"](p5, out=v[2])
         P["pyramid6"](c5, out=v[3])
-        P["pyramid7"](engine.relu_from_view(v[3]), out=v[4])
+        r6 = engine.relu_from_view(v[3])
+        P["pyramid7"](r6, out=v[4])
+        if keep is not None:
+            keep.update(c3=c3, c4=c4, c5=c5, p3=p3, p4=p4, p5=p5, r6=r6)
         return v
 
     def _atlas_for(self, n, sizes, device):
@@ -1129,7 +1179,8 @@ class Model:
         and the state the backward needs."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
-        views = self._features(self._stem(self._to_nhwc_half(x)))
+        keep = {} if self.train_scope == "fpn" else None
+        views = self._features(self._stem(self._to_nhwc_half(x)), keep)
         P = self._packed
         atlas0 = views[0].atlas
         at = self._atlas_for(atlas0.shape[0], tuple((v.h, v.w) for v in views), atlas0.device)
@@ -1145,30 +1196,32 @@ class Model:
                           for l, v in enumerate(views)]
         cls_loss, box_loss, cls_grads, box_grads = self._compute_loss(x, outs["cls_head"], outs["box_head"], targets,
                                                                       with_grad=True)
-        state = {"gen": self._fwd_gen, "at": at, "views": views, "heads": outs,
+        state = {"gen": self._fwd_gen, "at": at, "views": views, "heads": outs, "fpn": keep, "names": self._param_names(),
                  "grads": {"cls_head": cls_grads, "box_head": box_grads}}
         self.last_train = state if self.want_atlas_grad else None
         return cls_loss.clone(), box_loss.clone(), state
 
     def _train_backward(self, state, g_cls, g_box, needs):
-        """Gradients of the head parameters (None where `needs` is False) for upstream gradients g_cls / g_box of the two
-        losses.  Per head, from the last layer down: the loss gradients times the upstream factor into the fp16 gradient
-        atlas, then per layer the weight / bias gradient (odtk_conv_wgrad) and the input gradient masked by the ReLU of
-        the layer's input (odtk_conv2d_dgrad).  The first tower layer's input gradient, d(atlas), is only computed when
-        want_atlas_grad is set (the box tower's with the class tower's as its residual addend)."""
+        """Gradients of the training forward's parameters (state["names"]; None where `needs` is False) for upstream
+        gradients g_cls / g_box of the two losses.  Per head, from the last layer down: the loss gradients times the
+        upstream factor into the fp16 gradient atlas, then per layer the weight / bias gradient (odtk_conv_wgrad) and the
+        input gradient masked by the ReLU of the layer's input (odtk_conv2d_dgrad).  The first tower layer's input
+        gradient, d(atlas), is only computed when an FPN parameter needs a gradient or want_atlas_grad is set (the box
+        tower's with the class tower's as its residual addend); then the FPN backward (_fpn_backward) runs from it."""
         if state["gen"] != self._fwd_gen:
             raise RuntimeError("the model ran another forward pass after this training forward: its saved activations "
                                "are gone; call backward() before the next forward")
         at, tab = state["at"], state["at"]["tab"]
         P, params = self._packed, self._params
-        names = list(params)
+        names = state["names"]
         need = dict(zip(names, needs))
+        need_fpn = any(need.get(n, False) for n in self._fpn_param_names())
         got = {}
         atlas0 = state["views"][0].atlas
         if "gbuf" not in at:
             at["gbuf"] = [torch.zeros_like(atlas0) for _ in range(4)]    # tower gradient ping-pong + d(atlas) (cls, sum)
         gbuf, d_atlas = at["gbuf"], None
-        want_atlas = self.want_atlas_grad
+        want_atlas = self.want_atlas_grad or need_fpn
         for head, g in (("cls_head", g_cls), ("box_head", g_box)):
             lname = ["%s.%d" % (head, i) for i in (0, 2, 4, 6, 8)]
             needed = [need[n + ".weight"] or need[n + ".bias"] for n in lname]
@@ -1200,15 +1253,78 @@ class Model:
                 else:
                     d_atlas = engine.conv2d_dgrad(G, wpk, 256, residual=d_atlas, tile_tab=tab,
                                                   out=gbuf[2] if d_atlas is None else gbuf[3])
-        self.last_atlas_grad = d_atlas if want_atlas else None
+        if need_fpn and d_atlas is not None:
+            self._fpn_backward(state, d_atlas, need, got)
+        self.last_atlas_grad = d_atlas if self.want_atlas_grad else None
         return [got.get(n) for n in names]
+
+    def _fpn_backward(self, state, d_atlas, need, got):
+        """The FPN's weight and bias gradients from d(atlas), the gradient w.r.t. the five FPN outputs, into `got`:
+        pyramid7 (odtk_conv_wgrad_ex, stride 2 over relu(P6)); dP6 = d(atlas)'s P6 level + the input gradient of pyramid7 --
+        dP7 dilated into P6's geometry (odtk_dilate_f16), the stride-1 masked dgrad over P6's tiles, then the plain add
+        (odtk_pool_add_f16, pool 1: the dgrad's mask would also zero a residual addend); pyramid6 (stride 2 over C5);
+        smooth3-5 (3x3 over the pre-smooth p3-p5); their unmasked input gradients into a pre-smooth gradient atlas, the
+        top-down pathway's upsample-add backward (pool 2, level 0 -> 1, then 1 -> 2), then lateral3-5 (1x1 over C3-C5).
+        Only the launches whose results a needed gradient reads run; the backbone gets no gradient."""
+        S, at, views, params = state["fpn"], state["at"], state["views"], self._params
+        pre = "backbones.%s." % self.backbone
+        rows = at["rows"]
+        lv = [(r, v.h, v.w) for r, v in zip(rows, views)]
+        if "tabs" not in at:          # the tile table is ordered by level: one contiguous slice per level
+            counts = [((h + 7) // 8) * ((w + 15) // 16) for _, h, w in lv]
+            starts = np.cumsum([0] + counts).tolist()
+            at["tabs"] = [at["tab"][starts[l]:starts[l + 1]] for l in range(5)]
+        tabs, atlas0 = at["tabs"], views[0].atlas
+
+        def wants(layer):
+            return need.get(pre + layer + ".weight", False) or need.get(pre + layer + ".bias", False)
+
+        def wgrad(layer, g, x, ksize, stride, l):
+            wn, bn = pre + layer + ".weight", pre + layer + ".bias"
+            if wants(layer):
+                dw, db = engine.conv_wgrad_ex(g, x, 256, ksize, stride, tabs[l], rows[l], bias=need.get(bn, False))
+                if need.get(wn, False):
+                    got[wn] = dw
+                if need.get(bn, False):
+                    got[bn] = db
+
+        def dgrad_weights(layer):
+            p = params[pre + layer + ".weight"]
+            cached = self._dgrad_w.get(layer)
+            if cached is None or cached[0] != (p._version, id(p)):
+                cached = self._dgrad_w[layer] = ((p._version, id(p)), engine.pack_weight_dgrad(p, 256))
+            return cached[1]
+
+        def buf(name):                # zero-initialised once: only the levels' tiles are ever written
+            if name not in at:
+                at[name] = torch.zeros_like(atlas0)
+            return at[name]
+
+        wgrad("pyramid7", d_atlas, S["r6"], 3, 2, 4)
+        if wants("pyramid6"):
+            gd = engine.dilate(d_atlas, buf("fpn_dilated"), lv[4], rows[3])
+            dp6 = engine.conv2d_dgrad(gd, dgrad_weights("pyramid7"), 256, mask=atlas0, tile_tab=tabs[3], out=buf("fpn_dp6"))
+            engine.pool_add(d_atlas, dp6, lv[3], lv[3], pool=1)
+            wgrad("pyramid6", dp6, S["c5"], 3, 2, 3)
+        for l in range(3):
+            wgrad("smooth%d" % (l + 3), d_atlas, S["p%d" % (l + 3)], 3, 1, l)
+        top = max([l for l in range(3) if wants("lateral%d" % (l + 3))], default=-1)    # lateral l reads levels 0..l
+        if top >= 0:
+            dpre = buf("fpn_dpre")
+            for l in range(top + 1):
+                engine.conv2d_dgrad(d_atlas, dgrad_weights("smooth%d" % (l + 3)), 256, tile_tab=tabs[l], out=dpre)
+            for l in range(top):
+                engine.pool_add(dpre, dpre, lv[l], lv[l + 1], pool=2)
+            for l in range(top + 1):
+                wgrad("lateral%d" % (l + 3), dpre, S["c%d" % (l + 3)], 1, 1, l)
 
     def forward(self, x, rotated_bbox=None):
         self._sync_params()
         if self.training:
             x, targets = x
-            if self._params is not None and torch.is_grad_enabled() and any(p.requires_grad for p in self._params.values()):
-                return _HeadsTrain.apply(self, x, targets.float().to(x.device), *self._params.values())
+            params = [p for _, p in self.named_parameters()] if self._params is not None else []
+            if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+                return _HeadsTrain.apply(self, x, targets.float().to(x.device), *params)
             cls_heads, box_heads = self.forward_heads(x, sigmoid=False)
             return self._compute_loss(x, cls_heads, box_heads, targets.float().to(cls_heads[0].device))
         if self.fused_candidates and not self.exporting:

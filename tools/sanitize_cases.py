@@ -11,7 +11,9 @@ input and output) and the INT8 heads and network scope of the model, the split-T
 3, N tiles 64 / 128, several tiles per CTA so the A_lo side buffers and the named barrier cycle, tile table and level views,
 fp32 addends, NCHW / sigmoid / candidate epilogues, the fp32 small kernels, the fp32 model), decode (filter / gather / select), NMS (shared-memory aliasing of the sort scratch), rotated NMS,
 iou, target assignment, the cooperative loss kernel, and head training (`train`: the weight-gradient kernel, the bias-gradient
-and reduce kernels, the gradient atlas, the masked input-gradient conv instance, one SGD step of the model)."""
+and reduce kernels, the gradient atlas, the masked input-gradient conv instance, one SGD step of the model), and FPN
+training (`train_fpn`: the wgrad_ex instance in its three modes, the level bias-gradient and 1-tap reduce kernels, the
+pool-add and dilation kernels, one SGD step of the model in the "fpn" scope)."""
 import os
 import sys
 
@@ -142,10 +144,48 @@ def train_cases():
     print("train step ok", flush=True)
 
 
+def train_fpn_cases():
+    """FPN training: wgrad_kernel<true> (1x1, 3x3 stride 1, 3x3 stride 2 element-strided boxes, a level at a nonzero
+    g_row0, odd level sizes), bgrad_level_partial / wgrad_reduce<1>, pool_add (pool 2 in place with a missing source row,
+    pool 1), dilate, and one SGD step of the model in the "fpn" scope."""
+    sizes = ((16, 24), (8, 12), (7, 10), (4, 5), (2, 3))
+    at = Model("ResNet18FPN", classes=1)._atlas_for(2, sizes, torch.device(DEV))
+    n, ha, wa = at["buf"][0].shape[:3]
+    counts = [((h + 7) // 8) * ((w + 15) // 16) for h, w in sizes]
+    starts = [sum(counts[:l]) for l in range(6)]
+    tabs = [at["tab"][starts[l]:starts[l + 1]] for l in range(5)]
+    gg = rnd(n, ha, wa, 256, scale=0.1)
+    engine.conv_wgrad_ex(gg, rnd(n, 8, 12, 512), 256, 1, 1, tabs[1], at["rows"][1])
+    engine.conv_wgrad_ex(gg, rnd(n, 7, 10, 256), 256, 3, 1, tabs[2], at["rows"][2])
+    engine.conv_wgrad_ex(gg, rnd(n, 7, 10, 256), 256, 3, 2, tabs[3], at["rows"][3], bias=False)
+    engine.conv_wgrad_ex(gg, rnd(n, 4, 5, 128), 256, 3, 2, tabs[4], at["rows"][4])
+    torch.cuda.synchronize()
+    print("wgrad_ex ok", flush=True)
+    lv = [(r, h, w) for r, (h, w) in zip(at["rows"], sizes)]
+    engine.pool_add(gg, gg, lv[0], lv[1], pool=2)
+    engine.pool_add(gg, gg, lv[3], lv[4], pool=2)
+    engine.pool_add(rnd(n, ha, wa, 256), gg, lv[2], lv[2], pool=1)
+    engine.dilate(gg, torch.zeros_like(gg), lv[4], at["rows"][3])
+    torch.cuda.synchronize()
+    print("pool_add / dilate ok", flush=True)
+    m = Model("ResNet18FPN", classes=3).load_state_dict(make_state_dict("ResNet18FPN", 3, 9, False, seed=1)).cuda(0)
+    opt = torch.optim.SGD(m.set_train_scope("fpn").parameters(), lr=0.01, momentum=0.9)
+    m.train()
+    x = torch.randn((2, 3, 128, 256), generator=g).to(DEV)
+    t = torch.tensor([[[20., 30., 60., 40., 1.], [100., 10., 50., 90., 2.]], [[5., 5., 100., 100., 0.], [-1.] * 5]]).to(DEV)
+    cls_loss, box_loss = m([x, t])
+    ((cls_loss + box_loss) * 1024.0).backward()
+    opt.step()
+    torch.cuda.synchronize()
+    print("train fpn step ok", flush=True)
+
+
 def main():
     only = sys.argv[1] if len(sys.argv) > 1 else ""
     if only in ("", "train"):
         train_cases()
+    if only in ("", "train_fpn"):
+        train_fpn_cases()
     if only in ("", "conv"):
         conv(2, 16, 16, 64, 64, 1, relu=True)                              # mode 0
         conv(2, 16, 16, 256, 256, 1, relu=True, residual=True)             # residual epilogue

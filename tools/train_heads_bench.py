@@ -3,7 +3,11 @@ frozen).  Reports the step time split into forward (backbone, FPN, towers and fi
 fused loss launch) and backward (gradient atlas, weight and input gradients of the ten head layers), and per-launch
 TFLOP/s of a tower layer's forward, weight-gradient and input-gradient launches over the pyramid atlas (CUDA events around
 repeated launches, FLOPs = 2 * pixels of the levels * 256 * 9 * 256).
-    python tools/train_heads_bench.py [--batch 8] [--steps 10]"""
+--scope fpn trains the FPN as well (Model.set_train_scope("fpn")) and reports the step split into forward, loss, head
+backward (the same step with every FPN parameter frozen but d(atlas) computed) and FPN backward (the rest), and per
+launch the time and TFLOP/s of each FPN layer's weight gradient (odtk_conv_wgrad_ex) next to its forward launch (FLOPs =
+2 * output pixels * 256 * k^2 * Cin).
+    python tools/train_heads_bench.py [--batch 8] [--steps 10] [--scope heads|fpn]"""
 import argparse
 import json
 import os
@@ -34,11 +38,13 @@ def main():
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--classes", type=int, default=80)
+    ap.add_argument("--scope", choices=("heads", "fpn"), default="heads")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "this benchmark needs a GPU"
     dev = "cuda:0"
     g = torch.Generator().manual_seed(0)
     m = Model("ResNet50FPN", classes=args.classes).load_state_dict(make_state_dict("ResNet50FPN", args.classes, 9, False)).cuda(0)
+    m.set_train_scope(args.scope)
     opt = torch.optim.SGD(m.parameters(), lr=1e-4, weight_decay=1e-4, momentum=0.9)
     scaler = torch.amp.GradScaler("cuda")
     x = torch.randn((args.batch, 3, 800, 1280), generator=g).to(dev)
@@ -96,15 +102,59 @@ def main():
         fn()
         ms = timed(fn, 20)
         per_launch[k] = {"ms": round(ms, 4), "tflops": round(flops / ms / 1e9, 1)}
+    head_bwd = None
+    if args.scope == "fpn":
+        params = dict(m.named_parameters())
+        fpn = m._fpn_param_names()
+        for k in fpn:                     # the heads' share: the same backward with d(atlas) but no FPN gradient
+            params[k].requires_grad_(False)
+        m.want_atlas_grad = True
+        split_h = []
+        for _ in range(args.steps):
+            step(split_h)
+        m.want_atlas_grad = False
+        for k in fpn:
+            params[k].requires_grad_(True)
+        head_bwd = sum(s[1] for s in split_h) / len(split_h)
+        S, views = st["fpn"], st["views"]
+        rows, tab = at["rows"], at["tab"]
+        counts = [((v.h + 7) // 8) * ((v.w + 15) // 16) for v in views]
+        starts = [sum(counts[:l]) for l in range(6)]
+        tabs = [tab[starts[l]:starts[l + 1]] for l in range(5)]
+        ga = (torch.randn(a0.shape, generator=g) * 0.01).half().to(dev)
+        p5v = engine.AtlasView(gbuf, rows[2], views[2].h, views[2].w)
+        # layer: (input, ksize, stride, level, forward launch)
+        layers = {
+            "lateral3": (S["c3"], 1, 1, 0, lambda: P["lateral3"](S["c3"], upsample=S["p4"])),
+            "lateral4": (S["c4"], 1, 1, 1, lambda: P["lateral4"](S["c4"], upsample=S["p5"])),
+            "lateral5": (S["c5"], 1, 1, 2, lambda: P["lateral5"](S["c5"])),
+            "smooth3": (S["p3"], 3, 1, 0, lambda: P["smooth3"](S["p3"], out=engine.AtlasView(gbuf, rows[0], views[0].h, views[0].w))),
+            "smooth4": (S["p4"], 3, 1, 1, lambda: P["smooth4"](S["p4"], out=engine.AtlasView(gbuf, rows[1], views[1].h, views[1].w))),
+            "smooth5": (S["p5"], 3, 1, 2, lambda: P["smooth5"](S["p5"], out=p5v)),
+            "pyramid6": (S["c5"], 3, 2, 3, lambda: P["pyramid6"](S["c5"], out=engine.AtlasView(gbuf, rows[3], views[3].h, views[3].w))),
+            "pyramid7": (S["r6"], 3, 2, 4, lambda: P["pyramid7"](S["r6"], out=engine.AtlasView(gbuf, rows[4], views[4].h, views[4].w))),
+        }
+        for name, (xin, ks, stride, l, fwd) in layers.items():
+            fl = 2 * args.batch * views[l].h * views[l].w * 256 * ks * ks * xin.shape[3]
+            wg = lambda: engine.conv_wgrad_ex(ga, xin, 256, ks, stride, tabs[l], rows[l])   # noqa: E731
+            for key, fn in (("forward", fwd), ("wgrad", wg)):
+                fn()
+                ms = timed(fn, 20)
+                per_launch["%s_%s" % (name, key)] = {"ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}
     try:
         gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
                              capture_output=True, text=True, timeout=20).stdout.strip()
     except (OSError, subprocess.SubprocessError):
         gpu = torch.cuda.get_device_name(0)
-    print(json.dumps({"workload": "ResNet50FPN heads training, %d x 3x800x1280, %d classes" % (args.batch, args.classes),
-                      "gpu": gpu, "step_ms": round(step_ms, 3), "forward_ms": round(fwd_loss - loss_ms, 3),
-                      "loss_ms": round(loss_ms, 3), "backward_ms": round(bwd, 3), "tower_launches": per_launch,
-                      "tower_layer_gflop": round(flops / 1e9, 1)}))
+    out = {"workload": "ResNet50FPN heads training, %d x 3x800x1280, %d classes" % (args.batch, args.classes),
+           "gpu": gpu, "step_ms": round(step_ms, 3), "forward_ms": round(fwd_loss - loss_ms, 3),
+           "loss_ms": round(loss_ms, 3), "backward_ms": round(bwd, 3), "tower_launches": per_launch,
+           "tower_layer_gflop": round(flops / 1e9, 1)}
+    if head_bwd is not None:
+        out["workload"] = out["workload"].replace("heads training", "FPN + heads training")
+        out["head_backward_ms"] = round(head_bwd, 3)
+        out["fpn_backward_ms"] = round(bwd - head_bwd, 3)
+    print(json.dumps(out))
 
 
 if __name__ == "__main__":
