@@ -1,25 +1,28 @@
-// wgrad.cu -- backward of the 3x3 stride-1 head convolutions (sm_90a): the weight-gradient GEMM over the pyramid atlas,
-// the bias gradient, and the packing of the loss gradients into the fp16 gradient atlas.  The input gradient runs on
-// conv_gemm_kernel (odtk_conv2d_dgrad, conv.cu).
+// wgrad.cu -- backward of the head and FPN convolutions (sm_90a): the weight-gradient GEMM over the gradient atlas, the
+// bias gradient, the packing of the loss gradients into the fp16 gradient atlas, and the FPN's top-down pathway backward.
+// The input gradient runs on conv_gemm_kernel (odtk_conv2d_dgrad, conv.cu).
 //
-//   dW[co, tap, ci] = sum over images and pixels p of  G[p, co] * X[p + tap - (1, 1), ci]
+//   dW[co, tap, ci] = sum over images and pixels (r, c) of  G[r, c, co] * X[s * (r - g_row0) + ky - p, s * c + kx - p, ci]
 //
-// is a GEMM with M = Cout, N = 9 * Cin and K = pixels.  One CTA owns a 128 x 128 (co, tap-ci) output tile and a contiguous
-// range of the atlas tiles (K split over CTAs so that 36 output tiles still fill the SMs):
-//   warpgroup 0     TMA producer: per 8 x 16 pixel tile, two 64-channel boxes of G (the gradient atlas) and two of X (the
-//                   layer's input atlas, the same box shifted by the tap; the hardware zero fill and the zero gap rows /
-//                   columns of the atlas are the padding, exactly as in the forward pass).
+// (tap = ky * k + kx, p = k / 2) is a GEMM with M = Cout, N = k^2 * Cin and K = pixels.  One CTA owns a 128 x 128
+// (co, tap-ci) output tile and a contiguous range of G's 8 x 16 pixel tiles (K split over CTAs so that 36 output tiles
+// still fill the SMs):
+//   warpgroup 0     TMA producer: per tile, two 64-channel boxes of G and two of X (the box under the tile, shifted by the
+//                   tap; stride 2 through element-strided boxes, elementStrides 2 in H and W, as conv.cu loads odd-size
+//                   stride-2 activations).
 //   warpgroups 1-2  64 output channels each: wgmma m64n128k16 with BOTH operands MN-major (pixels are K, the outer
 //                   dimension of the NHWC boxes): 128B-swizzled MN-major descriptors + the transpose immediates.
-// Each CTA writes its fp32 partial tile; one reduce kernel sums the partials in split order and writes the [Cout, Cin, 3, 3]
-// parameter layout, so the result is bit-identical run to run.  The bias gradient is a fixed-order column sum of G.
+// Each CTA writes its fp32 partial tile; one reduce kernel sums the partials in split order and writes the [Cout, Cin, k, k]
+// parameter layout, so the result is bit-identical run to run.  The bias gradient is a fixed-order column sum of G's level.
 //
-// odtk_conv_wgrad_ex (the FPN layers) is a second compile-time instance of the same kernel: G is one level of the gradient
-// atlas (the level's slice of the tile table, first row g_row0), X a DENSE tensor read at (s * (r - g_row0) + ky - p,
-// s * c + kx - p) -- 1x1 (one tap, N = Cin), 3x3 stride 1, or 3x3 stride 2 through element-strided boxes (elementStrides 2
-// in H and W, as conv.cu loads odd-size stride-2 activations).  G is zero outside the level (gap rows, columns right of a
-// narrow level), so the in-bounds X values under it contribute nothing; the hardware zero fill outside X is the padding.
-// Its bias gradient sums the level's rows only.
+// Both entry points run the same launch routine:
+//   odtk_conv_wgrad     (head layers) 3x3 stride 1: G and X are whole atlases of one geometry (g_row0 0) and the tile table
+//                       lists every level's tiles, or both are dense tensors; the atlas's zero gap rows / columns and the
+//                       hardware zero fill are the padding, exactly as in the forward pass.
+//   odtk_conv_wgrad_ex  (FPN layers) 1x1, 3x3 stride 1 or 3x3 stride 2: G is one level of the gradient atlas (the level's
+//                       slice of the tile table, first row g_row0), X a dense tensor.  G is zero outside the level (gap
+//                       rows, columns right of a narrow level), so the in-bounds X values under it contribute nothing; the
+//                       hardware zero fill outside X is the padding.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -46,14 +49,13 @@ struct WgradParams {
   const int4 *tile_tab;   // atlas tile table (h0, w0, row limit, column limit) or NULL
   int tab_tiles;          // tiles per image
   int tiles_w;            // dense mode: tiles per tile row
-  int n_tiles, mn_tiles;  // N tiles (9 * cin / 128); M x N tiles
+  int n_tiles, mn_tiles;  // N tiles (taps * cin / 128); M x N tiles
   int cin, cout_pad;
   int ktiles, splits;     // K tiles (images x tiles) and the CTAs each output tile is split over
   float *ws;              // fp32 partials [splits, cout_pad, taps * cin]
-  int ksize, stride, g_row0;   // the wgrad_ex instance only: taps ksize^2, X pixel s * (r - g_row0) + tap - ksize / 2
+  int ksize, stride, g_row0;   // taps ksize^2; X pixel s * (r - g_row0) + tap - ksize / 2
 };
 
-template <bool kEx>
 __global__ void __launch_bounds__(kWThreads, 1)
 wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CUtensorMap tmX,
              const __grid_constant__ WgradParams p) {
@@ -81,8 +83,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
   if (wg == 0) {
     // ===================================== TMA producer =====================================
     if (tid != 0) return;
-    int dy = tap / 3 - 1, dx = tap % 3 - 1;
-    if constexpr (kEx) { dy = tap / p.ksize - p.ksize / 2; dx = tap % p.ksize - p.ksize / 2; }
+    const int dy = tap / p.ksize - p.ksize / 2, dx = tap % p.ksize - p.ksize / 2;
     int stage = 0;
     uint32_t phase = 0;
     for (int kt = k_begin; kt < k_end; kt++) {
@@ -95,8 +96,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
       mbar_arrive_expect_tx(&full[stage], (uint32_t)kWStageBytes);
       tma_load_4d(s, &tmG, &full[stage], m0, w0, h0, img);
       tma_load_4d(s + kBox, &tmG, &full[stage], m0 + 64, w0, h0, img);   // past cout_pad: zero-filled, never stored
-      int xw = w0 + dx, xh = h0 + dy;
-      if constexpr (kEx) { xw = p.stride * w0 + dx; xh = p.stride * (h0 - p.g_row0) + dy; }
+      const int xw = p.stride * w0 + dx, xh = p.stride * (h0 - p.g_row0) + dy;
       tma_load_4d(s + 2 * kBox, &tmX, &full[stage], ci0, xw, xh, img);
       tma_load_4d(s + 3 * kBox, &tmX, &full[stage], ci0 + 64, xw, xh, img);
       if (++stage == kWStages) { stage = 0; phase ^= 1u; }
@@ -130,7 +130,7 @@ wgrad_kernel(const __grid_constant__ CUtensorMap tmG, const __grid_constant__ CU
   wgmma_wait<0>();
 
   // thread holds rows (output channels) r and r + 8, columns 8 j + 2 q (+1)
-  const int N = (kEx ? p.ksize * p.ksize : 9) * p.cin;
+  const int N = p.ksize * p.ksize * p.cin;
   float *ws = p.ws + (size_t)split * p.cout_pad * N;
 #pragma unroll
   for (int i = 0; i < 2; i++) {
@@ -249,9 +249,7 @@ bool wgrad_device_ready() {
   if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) return false;
   std::lock_guard<std::mutex> lk(g_wgrad_mu);
   if (g_wgrad_ready[dev]) return true;
-  if (cudaFuncSetAttribute(wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSmem) != cudaSuccess ||
-      cudaFuncSetAttribute(wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSmem) != cudaSuccess)
-    return false;
+  if (cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kWSmem) != cudaSuccess) return false;
   g_wgrad_ready[dev] = true;
   return true;
 }
@@ -269,6 +267,80 @@ int choose_splits(int mn_tiles, int ktiles, int sms) {
   return best;
 }
 
+// One weight-gradient launch of either entry point, its arguments checked: G [n, g_rows, g_width, cout_pad], X [n, x_h,
+// x_width, cin], the tiles of G from tile_tab (tab_tiles per image) or, tile_tab NULL, the dense 8 x 16 tiles of the
+// g_rows x g_width image (tab_tiles = their count).  workspace NULL or workspace_size 0: returns the bytes needed.
+long long wgrad_run(const odtk_wgrad_ex_t &d, void *workspace, size_t workspace_size, odtk_stream_t stream_) {
+  const long long ktiles = (long long)d.n * d.tab_tiles;
+  const int taps = d.ksize * d.ksize;
+  const int N = taps * d.cin;
+  const int n_tiles = N / 128, m_tiles = (d.cout_pad + 127) / 128;
+  const int mn_tiles = m_tiles * n_tiles;
+  const int sms = odtk_sm_count();
+  const int splits = choose_splits(mn_tiles, (int)ktiles, sms);
+  const size_t ws_part = odtk_align_up((size_t)splits * d.cout_pad * N * sizeof(float));
+  const size_t ws_bias = odtk_align_up((size_t)kBiasBlocks * d.cout_pad * sizeof(float));
+  const size_t need = ws_part + ws_bias;
+  if (!workspace || workspace_size == 0) return (long long)need;
+  if (workspace_size < need) return ODTK_E_WORKSPACE;
+  if (!wgrad_device_ready()) return ODTK_E_CUDA;
+  cudaStream_t stream = (cudaStream_t)stream_;
+
+  CUtensorMap tmG, tmX;
+  {
+    const uint64_t C = (uint64_t)d.cout_pad, W = (uint64_t)d.g_width, H = (uint64_t)d.g_rows;
+    uint64_t dims[4] = {C, W, H, (uint64_t)d.n};
+    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
+    uint32_t box[4] = {64, 16, 8, 1};
+    if (!encode_map(&tmG, d.g, 4, dims, str, box)) return ODTK_E_CUDA;
+  }
+  {
+    // stride 2: boxDim = 2 x the pixels, elementStrides 2 -- the TMA unit loads every second pixel of a 32 x 16 window
+    const uint64_t C = (uint64_t)d.cin, W = (uint64_t)d.x_width, H = (uint64_t)d.x_h;
+    const uint32_t s = (uint32_t)d.stride;
+    uint64_t dims[4] = {C, W, H, (uint64_t)d.n};
+    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
+    uint32_t box[4] = {64, 16 * s, 8 * s, 1};
+    uint32_t estr[4] = {1, s, s, 1};
+    if (!encode_map(&tmX, d.x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, estr)) return ODTK_E_CUDA;
+  }
+  WgradParams p;
+  memset(&p, 0, sizeof p);
+  p.tile_tab = (const int4 *)d.tile_tab;
+  p.tab_tiles = d.tab_tiles;
+  p.tiles_w = (d.g_width + 15) / 16;
+  p.n_tiles = n_tiles;
+  p.mn_tiles = mn_tiles;
+  p.cin = d.cin;
+  p.cout_pad = d.cout_pad;
+  p.ktiles = (int)ktiles;
+  p.splits = splits;
+  p.ws = (float *)workspace;
+  p.ksize = d.ksize;
+  p.stride = d.stride;
+  p.g_row0 = d.g_row0;
+  float *part = (float *)((char *)workspace + ws_part);
+  {
+    OdtkProfScope prof(ODTK_PROF_CONV, stream);
+    wgrad_kernel<<<mn_tiles * splits, kWThreads, kWSmem, stream>>>(tmG, tmX, p);
+    const int lh = (d.x_h - 1) / d.stride + 1;   // the level's rows
+    if (d.db && lh == d.g_rows)                  // G is one level: its rows of all images are contiguous
+      bgrad_partial_kernel<<<kBiasBlocks, 128, 0, stream>>>((const __half *)d.g, (long long)d.n * lh * d.g_width,
+                                                           d.cout_pad, part);
+    else if (d.db)
+      bgrad_level_partial_kernel<<<kBiasBlocks, 128, 0, stream>>>(
+          (const __half *)d.g + (size_t)d.g_row0 * d.g_width * d.cout_pad, (long long)d.n * lh * d.g_width,
+          (long long)lh * d.g_width, (long long)d.g_rows * d.g_width * d.cout_pad, d.cout_pad, part);
+    const long long elems = (long long)d.cout * d.cin;
+    const unsigned blocks = (unsigned)((elems + 255) / 256);
+    if (taps == 1)
+      wgrad_reduce_kernel<1><<<blocks, 256, 0, stream>>>(p.ws, splits, d.cout, d.cout_pad, d.cin, d.dw, part, kBiasBlocks, d.db);
+    else
+      wgrad_reduce_kernel<9><<<blocks, 256, 0, stream>>>(p.ws, splits, d.cout, d.cout_pad, d.cin, d.dw, part, kBiasBlocks, d.db);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
 }  // namespace
 
 extern "C" long long odtk_conv_wgrad(const odtk_wgrad_t *d, void *workspace, size_t workspace_size, odtk_stream_t stream_) {
@@ -281,60 +353,15 @@ extern "C" long long odtk_conv_wgrad(const odtk_wgrad_t *d, void *workspace, siz
   if (d->tile_tab && d->tab_tiles <= 0) return ODTK_E_INVALID;
   const int tiles_w = (d->width + 15) / 16;
   const int per_img = d->tile_tab ? d->tab_tiles : ((d->h + 7) / 8) * tiles_w;
-  const long long ktiles = (long long)d->n * per_img;
-  if (ktiles >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  const int N = 9 * d->cin;
-  const int n_tiles = N / 128, m_tiles = (d->cout_pad + 127) / 128;
-  const int mn_tiles = m_tiles * n_tiles;
-  const int sms = odtk_sm_count();
-  const int splits = choose_splits(mn_tiles, (int)ktiles, sms);
-  const size_t ws_part = odtk_align_up((size_t)splits * d->cout_pad * N * sizeof(float));
-  const size_t ws_bias = odtk_align_up((size_t)kBiasBlocks * d->cout_pad * sizeof(float));
-  const size_t need = ws_part + ws_bias;
-  if (!workspace || workspace_size == 0) return (long long)need;
-  if (workspace_size < need) return ODTK_E_WORKSPACE;
-  if (!wgrad_device_ready()) return ODTK_E_CUDA;
-  cudaStream_t stream = (cudaStream_t)stream_;
-
-  CUtensorMap tmG, tmX;
-  {
-    const uint64_t C = (uint64_t)d->cout_pad, W = (uint64_t)d->width, H = (uint64_t)d->h;
-    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
-    uint32_t box[4] = {64, 16, 8, 1};
-    if (!encode_map(&tmG, d->g, 4, dims, str, box)) return ODTK_E_CUDA;
-  }
-  {
-    const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->width, H = (uint64_t)d->h;
-    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
-    uint32_t box[4] = {64, 16, 8, 1};
-    if (!encode_map(&tmX, d->x, 4, dims, str, box)) return ODTK_E_CUDA;
-  }
-  WgradParams p;
-  memset(&p, 0, sizeof p);
-  p.tile_tab = (const int4 *)d->tile_tab;
-  p.tab_tiles = per_img;
-  p.tiles_w = tiles_w;
-  p.n_tiles = n_tiles;
-  p.mn_tiles = mn_tiles;
-  p.cin = d->cin;
-  p.cout_pad = d->cout_pad;
-  p.ktiles = (int)ktiles;
-  p.splits = splits;
-  p.ws = (float *)workspace;
-  float *part = (float *)((char *)workspace + ws_part);
-  {
-    OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    wgrad_kernel<false><<<mn_tiles * splits, kWThreads, kWSmem, stream>>>(tmG, tmX, p);
-    if (d->db)
-      bgrad_partial_kernel<<<kBiasBlocks, 128, 0, stream>>>((const __half *)d->g, (long long)d->n * d->h * d->width,
-                                                           d->cout_pad, part);
-    const long long elems = (long long)d->cout * d->cin;
-    wgrad_reduce_kernel<9><<<(unsigned)((elems + 255) / 256), 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin,
-                                                                             d->dw, part, kBiasBlocks, d->db);
-  }
-  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+  if ((long long)d->n * per_img >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
+  odtk_wgrad_ex_t e;
+  memset(&e, 0, sizeof e);
+  e.g = d->g; e.x = d->x; e.dw = d->dw; e.db = d->db;
+  e.n = d->n; e.g_rows = e.x_h = d->h; e.g_width = e.x_width = d->width;
+  e.cin = d->cin; e.cout = d->cout; e.cout_pad = d->cout_pad;
+  e.ksize = 3; e.stride = 1;
+  e.tile_tab = d->tile_tab; e.tab_tiles = per_img;
+  return wgrad_run(e, workspace, workspace_size, stream_);
 }
 
 extern "C" int odtk_grad_to_atlas(int batch, int num_levels, const odtk_grad_level_t *levels, int channels, const float *scale,
@@ -383,70 +410,7 @@ extern "C" long long odtk_conv_wgrad_ex(const odtk_wgrad_ex_t *d, void *workspac
   if (((uintptr_t)d->g | (uintptr_t)d->x | (uintptr_t)d->tile_tab) & 15) return ODTK_E_INVALID;
   const long long ktiles = (long long)d->n * d->tab_tiles;
   if (ktiles >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  const int taps = d->ksize * d->ksize;
-  const int N = taps * d->cin;
-  const int n_tiles = N / 128, m_tiles = (d->cout_pad + 127) / 128;
-  const int mn_tiles = m_tiles * n_tiles;
-  const int sms = odtk_sm_count();
-  const int splits = choose_splits(mn_tiles, (int)ktiles, sms);
-  const size_t ws_part = odtk_align_up((size_t)splits * d->cout_pad * N * sizeof(float));
-  const size_t ws_bias = odtk_align_up((size_t)kBiasBlocks * d->cout_pad * sizeof(float));
-  const size_t need = ws_part + ws_bias;
-  if (!workspace || workspace_size == 0) return (long long)need;
-  if (workspace_size < need) return ODTK_E_WORKSPACE;
-  if (!wgrad_device_ready()) return ODTK_E_CUDA;
-  cudaStream_t stream = (cudaStream_t)stream_;
-
-  CUtensorMap tmG, tmX;
-  {
-    const uint64_t C = (uint64_t)d->cout_pad, W = (uint64_t)d->g_width, H = (uint64_t)d->g_rows;
-    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
-    uint32_t box[4] = {64, 16, 8, 1};
-    if (!encode_map(&tmG, d->g, 4, dims, str, box)) return ODTK_E_CUDA;
-  }
-  {
-    // stride 2: boxDim = 2 x the pixels, elementStrides 2 -- the TMA unit loads every second pixel of a 32 x 16 window
-    const uint64_t C = (uint64_t)d->cin, W = (uint64_t)d->x_width, H = (uint64_t)d->x_h;
-    const uint32_t s = (uint32_t)d->stride;
-    uint64_t dims[4] = {C, W, H, (uint64_t)d->n};
-    uint64_t str[3] = {C * 2, W * C * 2, H * W * C * 2};
-    uint32_t box[4] = {64, 16 * s, 8 * s, 1};
-    uint32_t estr[4] = {1, s, s, 1};
-    if (!encode_map(&tmX, d->x, 4, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B, estr)) return ODTK_E_CUDA;
-  }
-  WgradParams p;
-  memset(&p, 0, sizeof p);
-  p.tile_tab = (const int4 *)d->tile_tab;
-  p.tab_tiles = d->tab_tiles;
-  p.n_tiles = n_tiles;
-  p.mn_tiles = mn_tiles;
-  p.cin = d->cin;
-  p.cout_pad = d->cout_pad;
-  p.ktiles = (int)ktiles;
-  p.splits = splits;
-  p.ws = (float *)workspace;
-  p.ksize = d->ksize;
-  p.stride = d->stride;
-  p.g_row0 = d->g_row0;
-  float *part = (float *)((char *)workspace + ws_part);
-  {
-    OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    wgrad_kernel<true><<<mn_tiles * splits, kWThreads, kWSmem, stream>>>(tmG, tmX, p);
-    if (d->db) {
-      const long long slab = (long long)lh * d->g_width;
-      bgrad_level_partial_kernel<<<kBiasBlocks, 128, 0, stream>>>(
-          (const __half *)d->g + (size_t)d->g_row0 * d->g_width * d->cout_pad, (long long)d->n * slab, slab,
-          (long long)d->g_rows * d->g_width * d->cout_pad, d->cout_pad, part);
-    }
-    const long long elems = (long long)d->cout * d->cin;
-    const unsigned blocks = (unsigned)((elems + 255) / 256);
-    if (taps == 1)
-      wgrad_reduce_kernel<1><<<blocks, 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin, d->dw, part, kBiasBlocks, d->db);
-    else
-      wgrad_reduce_kernel<9><<<blocks, 256, 0, stream>>>(p.ws, splits, d->cout, d->cout_pad, d->cin, d->dw, part, kBiasBlocks, d->db);
-  }
-  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+  return wgrad_run(*d, workspace, workspace_size, stream_);
 }
 
 // ---- the FPN's top-down pathway and pyramid7's input gradient: two small HBM-bound kernels over fp16 NHWC atlases -------

@@ -826,6 +826,19 @@ def pack_weight_dgrad(weight, cout_pad=None):
     return out
 
 
+def _wgrad_launch(name, d, g, x, cout, ksize, bias):
+    """odtk_<name> on descriptor d (its geometry filled) into new fp32 dw [cout, Cin, k, k], db [cout] or None."""
+    dw = torch.empty((cout, x.shape[3], ksize, ksize), dtype=torch.float32, device=g.device)
+    db = torch.empty((cout,), dtype=torch.float32, device=g.device) if bias else None
+    d.g, d.x, d.dw, d.db = g.data_ptr(), x.data_ptr(), dw.data_ptr(), (db.data_ptr() if db is not None else None)
+    f = getattr(_lib.lib(), "odtk_" + name)
+    size = _lib.check(f(ctypes.byref(d), None, 0, None), name + " (workspace query)")
+    ws = torch.empty(int(size), dtype=torch.uint8, device=g.device)
+    _lib.check(f(ctypes.byref(d), ctypes.c_void_p(ws.data_ptr()), size, _stream()), name)
+    STATS["launches"] += 1
+    return dw, db, size
+
+
 def conv_wgrad(g, x, cout, tile_tab=None, bias=True):
     """Weight (and bias) gradient of a 3x3 stride-1 pad-1 convolution (odtk_conv_wgrad): g NHWC fp16 [N, H, W, Cout_pad]
     (the gradient w.r.t. its output before the ReLU, zero outside the levels and in the channels >= cout), x NHWC fp16
@@ -836,18 +849,11 @@ def conv_wgrad(g, x, cout, tile_tab=None, bias=True):
     n, h, wd, cpad = g.shape
     cin = x.shape[3]
     assert tuple(x.shape[:3]) == (n, h, wd)
-    dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=g.device)
-    db = torch.empty((cout,), dtype=torch.float32, device=g.device) if bias else None
     d = WgradDesc()
-    d.g, d.x, d.dw, d.db = g.data_ptr(), x.data_ptr(), dw.data_ptr(), (db.data_ptr() if db is not None else None)
     d.n, d.h, d.width, d.cin, d.cout, d.cout_pad = n, h, wd, cin, cout, cpad
     if tile_tab is not None:
         d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
-    L = _lib.lib()
-    size = _lib.check(L.odtk_conv_wgrad(ctypes.byref(d), None, 0, None), "conv_wgrad (workspace query)")
-    ws = torch.empty(int(size), dtype=torch.uint8, device=g.device)
-    _lib.check(L.odtk_conv_wgrad(ctypes.byref(d), ctypes.c_void_p(ws.data_ptr()), size, _stream()), "conv_wgrad")
-    STATS["launches"] += 1
+    dw, db, size = _wgrad_launch("conv_wgrad", d, g, x, cout, 3, bias)
     if STATS["trace"] is not None:
         px = _tab_px(n, h, wd, tile_tab)
         # G once per output-channel tile row, X once per tap; the fp32 partials and the result
@@ -876,18 +882,11 @@ def conv_wgrad_ex(g, x, cout, ksize, stride, tile_tab, g_row0, bias=True):
     n, rows, aw, cpad = g.shape
     xn, xh, xw, cin = x.shape
     assert xn == n
-    dw = torch.empty((cout, cin, ksize, ksize), dtype=torch.float32, device=g.device)
-    db = torch.empty((cout,), dtype=torch.float32, device=g.device) if bias else None
     d = WgradExDesc()
-    d.g, d.x, d.dw, d.db = g.data_ptr(), x.data_ptr(), dw.data_ptr(), (db.data_ptr() if db is not None else None)
     d.n, d.g_rows, d.g_width, d.g_row0, d.cout_pad = n, rows, aw, int(g_row0), cpad
     d.x_h, d.x_width, d.cin, d.cout, d.ksize, d.stride = xh, xw, cin, cout, ksize, stride
     d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
-    L = _lib.lib()
-    size = _lib.check(L.odtk_conv_wgrad_ex(ctypes.byref(d), None, 0, None), "conv_wgrad_ex (workspace query)")
-    ws = torch.empty(int(size), dtype=torch.uint8, device=g.device)
-    _lib.check(L.odtk_conv_wgrad_ex(ctypes.byref(d), ctypes.c_void_p(ws.data_ptr()), size, _stream()), "conv_wgrad_ex")
-    STATS["launches"] += 1
+    dw, db, size = _wgrad_launch("conv_wgrad_ex", d, g, x, cout, ksize, bias)
     if STATS["trace"] is not None:
         px = n * ((xh - 1) // stride + 1) * ((xw - 1) // stride + 1)
         # the level's G once, X once per tap (1x1 and stride 2: the pixels it samples), the fp32 partials and the result

@@ -105,17 +105,7 @@ def conv_specs(backbone, classes=80, num_anchors=9, rotated=False):
                           (p + "downsample.1", "bn", planes * exp)]
             inplanes = planes * exp
     ch = [128, 256, 512] if block == "basic" else [512, 1024, 2048]
-    n = "backbones.%s." % backbone
-    specs += [(n + "lateral3", "convb", (256, ch[0], 1, 1)), (n + "lateral4", "convb", (256, ch[1], 1, 1)),
-              (n + "lateral5", "convb", (256, ch[2], 1, 1)), (n + "pyramid6", "convb", (256, ch[2], 3, 3)),
-              (n + "pyramid7", "convb", (256, 256, 3, 3)), (n + "smooth3", "convb", (256, 256, 3, 3)),
-              (n + "smooth4", "convb", (256, 256, 3, 3)), (n + "smooth5", "convb", (256, 256, 3, 3))]
-    nbox = 6 if rotated else 4
-    for head, out in (("cls_head", classes * num_anchors), ("box_head", nbox * num_anchors)):
-        for i in (0, 2, 4, 6):
-            specs.append(("%s.%d" % (head, i), "convb", (256, 256, 3, 3)))
-        specs.append(("%s.8" % head, "convb_final", (out, 256, 3, 3)))
-    return specs
+    return specs + _fpn_specs("backbones.%s." % backbone, ch) + _head_specs(classes, num_anchors, rotated)
 
 
 def make_state_dict(backbone="ResNet50FPN", classes=80, num_anchors=9, rotated=False, seed=0, cls_prior=0.01):
@@ -379,10 +369,11 @@ class Model:
         self._calib_net = False       # calibration also records the network scope's tensors
         self._f32 = None              # full precision: split-TF32 weights of every layer (packed on first use)
         self._params = None           # trainable parameters by name (created by named_parameters / parameters)
+        self._walk = network_walk(backbones)   # read by every training forward (_trainable_layers)
         self.train_scope = "heads"    # "heads" or "fpn": which parameters named_parameters lists (set_train_scope)
         self._param_versions = {}     # weight name -> the layer's (weight, bias) _version when its fp16 weights were packed
         self._sd_versions = {}        # parameter name -> its _version when it was last copied into the state dict
-        self._dgrad_w = {}            # (head, layer index) / FPN layer -> (weight _version, pack_weight_dgrad weights)
+        self._dgrad_w = {}            # weight name -> ((_version, id), pack_weight_dgrad weights)
         self._fwd_gen = 0             # counts forward passes: a backward must follow its own forward
         # test hooks, both only while want_atlas_grad is set: the training backward also computes d(loss)/d(atlas) into
         # last_atlas_grad, which ALIASES a gradient buffer of the atlas geometry (the next backward overwrites it), and
@@ -471,12 +462,12 @@ class Model:
 
     def _trainable_layers(self):
         """(packed-layer key, index in a head list or None, stride, weight name, bias name) of every layer whose
-        parameters exist."""
-        layers = [(l, None, 2 if l.startswith("pyramid") else 1, "backbones.%s.%s.weight" % (self.backbone, l),
-                   "backbones.%s.%s.bias" % (self.backbone, l)) for l in FPN_LAYERS]
-        layers += [(head, k, 1, "%s.%d.weight" % (head, i), "%s.%d.bias" % (head, i))
-                   for head in ("cls_head", "box_head") for k, i in enumerate((0, 2, 4, 6, 8))]
-        return [t for t in layers if self._params is not None and t[3] in self._params]
+        parameters exist, the FPN's before the heads'."""
+        walk = self._walk
+        layers = [(l, None, walk[l]) for l in FPN_LAYERS if l in walk]
+        layers += [(head, k, c) for head in calib.HEADS for k, c in enumerate(walk[head])]
+        return [(key, k, c["stride"], c["conv"] + ".weight", c["conv"] + ".bias") for key, k, c in layers
+                if self._params is not None and c["conv"] + ".weight" in self._params]
 
     def set_train_scope(self, scope):
         """What training updates: "heads" (default: the class and box heads, the backbone and the FPN frozen) or "fpn"
@@ -963,7 +954,7 @@ class Model:
         Level l occupies rows [rows[l], rows[l] + h_l) x columns [0, w_l); level starts are multiples of 8 (the tile
         height) with at least one gap row in between; gap rows / columns are never written and stay zero (they ARE the
         convolutions' zero padding between levels).  tab: every 8 x 16 tile of one image as (row0, col0, row_limit,
-        col_limit)."""
+        col_limit), ordered by level; tabs: each level's contiguous slice of it."""
         key = (n, sizes, str(device))
         at = self._atlas.get(key)
         if at is None:
@@ -974,8 +965,10 @@ class Model:
             ha, wa = rows[-1] + sizes[-1][0], max(w for _, w in sizes)
             tiles = [(r0 + 8 * ty, 16 * tx, r0 + h, w) for (h, w), r0 in zip(sizes, rows)
                      for ty in range((h + 7) // 8) for tx in range((w + 15) // 16)]
-            at = {"rows": rows, "ha": ha, "wa": wa, "px": n * sum(h * w for h, w in sizes),
-                  "tab": torch.tensor(tiles, dtype=torch.int32, device=device),
+            tab = torch.tensor(tiles, dtype=torch.int32, device=device)
+            starts = np.cumsum([0] + [((h + 7) // 8) * ((w + 15) // 16) for h, w in sizes]).tolist()
+            at = {"rows": rows, "ha": ha, "wa": wa, "px": n * sum(h * w for h, w in sizes), "tab": tab,
+                  "tabs": [tab[starts[l]:starts[l + 1]] for l in range(len(sizes))],
                   "buf": [torch.zeros((n, ha, wa, 256), dtype=torch.float16, device=device) for _ in range(5)]}
             self._atlas[key] = at
         return at
@@ -1212,15 +1205,14 @@ class Model:
             raise RuntimeError("the model ran another forward pass after this training forward: its saved activations "
                                "are gone; call backward() before the next forward")
         at, tab = state["at"], state["at"]["tab"]
-        P, params = self._packed, self._params
+        P = self._packed
         names = state["names"]
         need = dict(zip(names, needs))
         need_fpn = any(need.get(n, False) for n in self._fpn_param_names())
         got = {}
         atlas0 = state["views"][0].atlas
-        if "gbuf" not in at:
-            at["gbuf"] = [torch.zeros_like(atlas0) for _ in range(4)]    # tower gradient ping-pong + d(atlas) (cls, sum)
-        gbuf, d_atlas = at["gbuf"], None
+        gbuf = [self._atlas_zeros(at, "gbuf%d" % i) for i in range(4)]    # tower gradient ping-pong + d(atlas) (cls, sum)
+        d_atlas = None
         want_atlas = self.want_atlas_grad or need_fpn
         for head, g in (("cls_head", g_cls), ("box_head", g_box)):
             lname = ["%s.%d" % (head, i) for i in (0, 2, 4, 6, 8)]
@@ -1228,26 +1220,14 @@ class Model:
             if g is None or not (any(needed) or want_atlas):
                 continue
             cpad = engine.pad64(P[head][-1].cout)
-            key = "grad%d" % cpad
-            if key not in at:
-                at[key] = torch.zeros(atlas0.shape[:3] + (cpad,), dtype=torch.float16, device=atlas0.device)
-            G = engine.grad_to_atlas(state["grads"][head], at["rows"], g, at[key])   # g stays on the device: no sync
+            G = self._atlas_zeros(at, "grad%d" % cpad, cpad)
+            G = engine.grad_to_atlas(state["grads"][head], at["rows"], g, G)   # g stays on the device: no sync
             inputs = [atlas0] + at["train"][head]
             for k in range(4, -1, -1):
-                wn, bn = lname[k] + ".weight", lname[k] + ".bias"
-                if need[wn] or need[bn]:
-                    dw, db = engine.conv_wgrad(G, inputs[k], P[head][k].cout, tile_tab=tab, bias=need[bn])
-                    if need[wn]:
-                        got[wn] = dw
-                    if need[bn]:
-                        got[bn] = db
+                self._wgrad(need, got, lname[k], engine.conv_wgrad, G, inputs[k], P[head][k].cout, tile_tab=tab)
                 if not (want_atlas or any(needed[:k])):
                     break
-                cached = self._dgrad_w.get((head, k))
-                if cached is None or cached[0] != (params[wn]._version, id(params[wn])):
-                    cached = self._dgrad_w[(head, k)] = ((params[wn]._version, id(params[wn])),
-                                                         engine.pack_weight_dgrad(params[wn], cpad if k == 4 else 256))
-                wpk = cached[1]
+                wpk = self._dgrad_weights(lname[k] + ".weight", cpad if k == 4 else 256)
                 if k > 0:
                     G = engine.conv2d_dgrad(G, wpk, 256, mask=inputs[k], tile_tab=tab, out=gbuf[k & 1])
                 else:
@@ -1266,57 +1246,65 @@ class Model:
         smooth3-5 (3x3 over the pre-smooth p3-p5); their unmasked input gradients into a pre-smooth gradient atlas, the
         top-down pathway's upsample-add backward (pool 2, level 0 -> 1, then 1 -> 2), then lateral3-5 (1x1 over C3-C5).
         Only the launches whose results a needed gradient reads run; the backbone gets no gradient."""
-        S, at, views, params = state["fpn"], state["at"], state["views"], self._params
+        S, at, views = state["fpn"], state["at"], state["views"]
         pre = "backbones.%s." % self.backbone
-        rows = at["rows"]
+        rows, tabs, atlas0 = at["rows"], at["tabs"], views[0].atlas
         lv = [(r, v.h, v.w) for r, v in zip(rows, views)]
-        if "tabs" not in at:          # the tile table is ordered by level: one contiguous slice per level
-            counts = [((h + 7) // 8) * ((w + 15) // 16) for _, h, w in lv]
-            starts = np.cumsum([0] + counts).tolist()
-            at["tabs"] = [at["tab"][starts[l]:starts[l + 1]] for l in range(5)]
-        tabs, atlas0 = at["tabs"], views[0].atlas
 
         def wants(layer):
             return need.get(pre + layer + ".weight", False) or need.get(pre + layer + ".bias", False)
 
         def wgrad(layer, g, x, ksize, stride, l):
-            wn, bn = pre + layer + ".weight", pre + layer + ".bias"
-            if wants(layer):
-                dw, db = engine.conv_wgrad_ex(g, x, 256, ksize, stride, tabs[l], rows[l], bias=need.get(bn, False))
-                if need.get(wn, False):
-                    got[wn] = dw
-                if need.get(bn, False):
-                    got[bn] = db
-
-        def dgrad_weights(layer):
-            p = params[pre + layer + ".weight"]
-            cached = self._dgrad_w.get(layer)
-            if cached is None or cached[0] != (p._version, id(p)):
-                cached = self._dgrad_w[layer] = ((p._version, id(p)), engine.pack_weight_dgrad(p, 256))
-            return cached[1]
-
-        def buf(name):                # zero-initialised once: only the levels' tiles are ever written
-            if name not in at:
-                at[name] = torch.zeros_like(atlas0)
-            return at[name]
+            self._wgrad(need, got, pre + layer, engine.conv_wgrad_ex, g, x, 256, ksize, stride, tabs[l], rows[l])
 
         wgrad("pyramid7", d_atlas, S["r6"], 3, 2, 4)
         if wants("pyramid6"):
-            gd = engine.dilate(d_atlas, buf("fpn_dilated"), lv[4], rows[3])
-            dp6 = engine.conv2d_dgrad(gd, dgrad_weights("pyramid7"), 256, mask=atlas0, tile_tab=tabs[3], out=buf("fpn_dp6"))
+            gd = engine.dilate(d_atlas, self._atlas_zeros(at, "fpn_dilated"), lv[4], rows[3])
+            dp6 = engine.conv2d_dgrad(gd, self._dgrad_weights(pre + "pyramid7.weight", 256), 256, mask=atlas0,
+                                      tile_tab=tabs[3], out=self._atlas_zeros(at, "fpn_dp6"))
             engine.pool_add(d_atlas, dp6, lv[3], lv[3], pool=1)
             wgrad("pyramid6", dp6, S["c5"], 3, 2, 3)
         for l in range(3):
             wgrad("smooth%d" % (l + 3), d_atlas, S["p%d" % (l + 3)], 3, 1, l)
         top = max([l for l in range(3) if wants("lateral%d" % (l + 3))], default=-1)    # lateral l reads levels 0..l
         if top >= 0:
-            dpre = buf("fpn_dpre")
+            dpre = self._atlas_zeros(at, "fpn_dpre")
             for l in range(top + 1):
-                engine.conv2d_dgrad(d_atlas, dgrad_weights("smooth%d" % (l + 3)), 256, tile_tab=tabs[l], out=dpre)
+                engine.conv2d_dgrad(d_atlas, self._dgrad_weights(pre + "smooth%d.weight" % (l + 3), 256), 256,
+                                    tile_tab=tabs[l], out=dpre)
             for l in range(top):
                 engine.pool_add(dpre, dpre, lv[l], lv[l + 1], pool=2)
             for l in range(top + 1):
                 wgrad("lateral%d" % (l + 3), dpre, S["c%d" % (l + 3)], 1, 1, l)
+
+    @staticmethod
+    def _wgrad(need, got, layer, launch, *args, **kwargs):
+        """Weight and bias gradient of `layer` (a parameter prefix) by launch(*args, bias=...) -> (dw, db), run only when
+        one of them is needed, stored into `got`."""
+        wn, bn = layer + ".weight", layer + ".bias"
+        if need.get(wn, False) or need.get(bn, False):
+            dw, db = launch(*args, bias=need.get(bn, False), **kwargs)
+            if need.get(wn, False):
+                got[wn] = dw
+            if need.get(bn, False):
+                got[bn] = db
+
+    def _dgrad_weights(self, name, cout_pad):
+        """engine.pack_weight_dgrad of parameter `name`, cached until the parameter changes."""
+        p = self._params[name]
+        cached = self._dgrad_w.get(name)
+        if cached is None or cached[0] != (p._version, id(p)):
+            cached = self._dgrad_w[name] = ((p._version, id(p)), engine.pack_weight_dgrad(p, cout_pad))
+        return cached[1]
+
+    @staticmethod
+    def _atlas_zeros(at, key, channels=256):
+        """at[key]: an fp16 buffer of the atlas geometry with `channels` channels, zero-initialised on first use (the
+        backward writes only the levels' tiles, so everything else stays zero)."""
+        if key not in at:
+            a = at["buf"][0]
+            at[key] = torch.zeros(a.shape[:3] + (channels,), dtype=torch.float16, device=a.device)
+        return at[key]
 
     def forward(self, x, rotated_bbox=None):
         self._sync_params()

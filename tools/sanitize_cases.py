@@ -145,15 +145,13 @@ def train_cases():
 
 
 def train_fpn_cases():
-    """FPN training: wgrad_kernel<true> (1x1, 3x3 stride 1, 3x3 stride 2 element-strided boxes, a level at a nonzero
-    g_row0, odd level sizes), bgrad_level_partial / wgrad_reduce<1>, pool_add (pool 2 in place with a missing source row,
-    pool 1), dilate, and one SGD step of the model in the "fpn" scope."""
+    """FPN training: wgrad_kernel through odtk_conv_wgrad_ex (1x1, 3x3 stride 1, 3x3 stride 2 element-strided boxes, a
+    level at a nonzero g_row0, odd level sizes), bgrad_level_partial / wgrad_reduce<1>, pool_add (pool 2 in place with a
+    missing source row, pool 1), dilate, and one SGD step of the model in the "fpn" scope."""
     sizes = ((16, 24), (8, 12), (7, 10), (4, 5), (2, 3))
     at = Model("ResNet18FPN", classes=1)._atlas_for(2, sizes, torch.device(DEV))
     n, ha, wa = at["buf"][0].shape[:3]
-    counts = [((h + 7) // 8) * ((w + 15) // 16) for h, w in sizes]
-    starts = [sum(counts[:l]) for l in range(6)]
-    tabs = [at["tab"][starts[l]:starts[l + 1]] for l in range(5)]
+    tabs = at["tabs"]
     gg = rnd(n, ha, wa, 256, scale=0.1)
     engine.conv_wgrad_ex(gg, rnd(n, 8, 12, 512), 256, 1, 1, tabs[1], at["rows"][1])
     engine.conv_wgrad_ex(gg, rnd(n, 7, 10, 256), 256, 3, 1, tabs[2], at["rows"][2])

@@ -117,10 +117,7 @@ def main():
             params[k].requires_grad_(True)
         head_bwd = sum(s[1] for s in split_h) / len(split_h)
         S, views = st["fpn"], st["views"]
-        rows, tab = at["rows"], at["tab"]
-        counts = [((v.h + 7) // 8) * ((v.w + 15) // 16) for v in views]
-        starts = [sum(counts[:l]) for l in range(6)]
-        tabs = [tab[starts[l]:starts[l + 1]] for l in range(5)]
+        rows, tabs = at["rows"], at["tabs"]
         ga = (torch.randn(a0.shape, generator=g) * 0.01).half().to(dev)
         p5v = engine.AtlasView(gbuf, rows[2], views[2].h, views[2].w)
         # layer: (input, ksize, stride, level, forward launch)
