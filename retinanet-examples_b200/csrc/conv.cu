@@ -10,8 +10,8 @@
 //                   from the NHWC tensor (the hardware zero-fills out-of-bounds rows/columns == conv padding: no
 //                   im2col, no border code) and of the weight blocks (2-D map over [Cout, taps*Cin]) into swizzled
 //                   shared memory, guarded by full/empty mbarriers.
-//   warpgroups 1-2  MMA + epilogue, 64 accumulator rows (output pixels) each: wgmma.mma_async m64nNk16 (N = BN = 64
-//                   or 128), fp32 accumulation in registers; the stage is released as soon as the next K block's
+//   warpgroups 1-2  MMA + epilogue, 64 accumulator rows (output pixels) each: wgmma.mma_async m64nNk16 (N = BN = 64,
+//                   128 or, fp16 forward only, 256), fp32 accumulation in registers; the stage is released as soon as the next K block's
 //                   MMAs are in flight.  The epilogue works on the registers: + bias, + residual / FPN nearest-
 //                   upsample, ReLU / ReLU6, fp16 NHWC store -- or, for the last convolution of a head, (sigmoid +)
 //                   fp32 NCHW in the layout the reference's decode entry point expects -- or, class head on the
@@ -125,6 +125,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   if (wg == 0) {
     // ===================================== TMA producer =====================================
+    // BN 256: the 128 fp32 accumulators per consumer thread need more than the 168 registers of a 384-thread CTA; the
+    // producer warpgroup hands its registers back (40 each) and the consumers take 232: 232 * 256 + 40 * 128 <= 64 K.
+    if constexpr (BN == 256) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (tid != 0) return;
     const uint32_t a_bytes = (uint32_t)((p.mode == 0 ? 128 : p.TH * p.TW) * rb), b_bytes = (uint32_t)(BR * rb);
     const int kelems = S8 ? rb : F32 ? rb >> 2 : rb >> 1;   // K elements per block: 64 (SW128) or 32 (SW64); s8: 128; fp32: 32
@@ -172,6 +175,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 
   // ===================================== MMA + epilogue ======================================
+  if constexpr (BN == 256) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   const int cw = wg - 1, warp = tid >> 5, lane = tid & 31;
   const int q = lane & 3;
   const int hw = p.H * p.W, patch = p.TH * p.TW;
@@ -521,9 +525,9 @@ template <int BN, int OP>
 constexpr Instance instance() {
   return {BN, OP, (const void *)conv_gemm_kernel<BN, OP>, launch_bn<BN, OP>, OP == kOpTF32x3 ? kSmemBytesF32 : kSmemBytes};
 }
-const Instance kInstances[] = {instance<64, kOpF16>(),     instance<128, kOpF16>(),     instance<64, kOpS8>(),
-                               instance<128, kOpS8>(),     instance<64, kOpTF32x3>(),   instance<128, kOpTF32x3>(),
-                               instance<64, kOpF16Mask>(), instance<128, kOpF16Mask>()};
+const Instance kInstances[] = {instance<64, kOpF16>(),     instance<128, kOpF16>(),     instance<256, kOpF16>(),
+                               instance<64, kOpS8>(),      instance<128, kOpS8>(),      instance<64, kOpTF32x3>(),
+                               instance<128, kOpTF32x3>(), instance<64, kOpF16Mask>(),  instance<128, kOpF16Mask>()};
 
 // Per-device state (one process may drive several GPUs): the > 48 KB dynamic-shared-memory opt-in of every kernel
 // instance is a per-device function attribute.
@@ -547,6 +551,17 @@ thread_local odtk_conv_plan_t g_last_plan;
 void set_stages(ConvParams &p, int BN, int op) {
   p.nstages = kPipeBytes / ((128 + (op == kOpTF32x3 ? 2 * BN : BN)) * p.row_bytes);
   if (p.nstages > kMaxStages) p.nstages = kMaxStages;
+}
+
+// BN 256 loads each A box once per 128 x 256 tile instead of once per 128-wide N tile (a 3x3 256 -> 256 layer moves 25 %
+// fewer bytes from L2 into shared memory) and issues half the wgmma instructions.  The tiles are twice as long, so the
+// last, partial wave costs twice as much: they must fill at least kWideWaves waves of the launch's SMs.  Measured per
+// launch at batch 32 (DESIGN §6): 1x1, 3x3 and stride-2 layers of 15-61 waves ran 2-11 % faster at BN 256, a 3x3 of 2
+// waves 3 % slower; the candidate epilogue of the class output layer (P3, 91 waves) ran 4 % slower and keeps BN 128.
+constexpr int kWideWaves = 12;
+bool wide_tiles_pay(const ConvParams &p, int cout) {
+  return p.out_mode != ODTK_OUT_CANDIDATES &&
+         (long long)p.num_m_tiles * ((cout + 255) / 256) >= (long long)kWideWaves * odtk_sm_count();
 }
 
 int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
@@ -810,10 +825,12 @@ int conv_run(const ConvArgs &a, const OpSpec &s, cudaStream_t stream) {
   p.oR = a.y_row_off > 0 ? a.y_row_off : 0;
   p.oW = a.y_width > 0 ? a.y_width : p.W;
   if ((long long)a.n * p.oH * p.oW >= (1ll << 31) || p.oR + p.H > p.oH || p.W > p.oW) return ODTK_E_INVALID;
-  // N tile: 64 or 128 output channels.  128 halves the A-operand traffic; 64 when Cout is narrow, for grouped convs (one
-  // 64-channel chunk per tile), or when 128-wide tiles would leave SMs idle.
+  // N tile: 64, 128 or 256 output channels.  128 halves the A-operand traffic; 64 when Cout is narrow, for grouped convs
+  // (one 64-channel chunk per tile), or when 128-wide tiles would leave SMs idle; 256 (fp16 forward) for the wide layers
+  // with enough tiles (wide_tiles_pay).
   int BN = (groups > 1 || a.cout <= 64) ? 64 : 128;
   if (BN == 128 && (long long)p.num_m_tiles * ((a.cout + 127) / 128) < odtk_sm_count()) BN = 64;
+  if (BN == 128 && op == kOpF16 && a.cout > 128 && wide_tiles_pay(p, a.cout)) BN = 256;
   p.num_n_tiles = (a.cout + BN - 1) / BN;
   set_stages(p, BN, op);
   CUtensorMap tmB, tmA2 = tmA, tmB2;

@@ -3,7 +3,7 @@
     compute-sanitizer --tool racecheck python tools/sanitize_cases.py
     compute-sanitizer --tool synccheck python tools/sanitize_cases.py
 Shapes are tiny (the tools slow kernels down 10-100x) but chosen to reach each variant of the wgmma kernels and their
-mbarrier rings: conv modes 0 / 1 / 2 / 3 with N tiles 64 and 128, ragged M and N tiles, residual / upsample / ReLU6 /
+mbarrier rings: conv modes 0 / 1 / 2 / 3 with N tiles 64 and 128 (and 256 in modes 0 / 1), ragged M and N tiles, residual / upsample / ReLU6 /
 fp32 / sigmoid / candidate epilogues, the fused stem + pool (stem.cu: halo rows at the image edges), the fused bottleneck
 tail (bottleneck.cu: C1 64 / 128, projected identity, GEMM3 with 64 / 128 outputs -- shared-memory A operands written
 by the epilogues), the s8 instantiation of the conv kernel (stride 2 in modes 3 and 1, residual / upsample addends, level-view
@@ -22,7 +22,7 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
-from retinanet_examples_b200 import _C, box, engine, loss, synth  # noqa: E402
+from retinanet_examples_b200 import _C, _lib, box, engine, loss, synth  # noqa: E402
 from retinanet_examples_b200.model import Model, make_state_dict  # noqa: E402
 
 DEV = "cuda:0"
@@ -192,6 +192,13 @@ def main():
         conv(1, 16, 24, 64, 64, 3, relu=True)                              # mode 1, N tile 64
         conv(1, 7, 10, 256, 256, 3, relu=True)                             # mode 1, patch of 70 pixels
         conv(10, 48, 64, 256, 256, 3, relu=True)                           # mode 1, N tile 128, several tiles per CTA
+        _lib.lib().odtk_set_sm_budget(2)                                   # N tile 256: a 2-SM budget makes few tiles enough
+        try:
+            conv(2, 48, 64, 256, 256, 3, relu=True)                        # mode 1, several tiles per CTA
+            conv(1, 32, 48, 256, 720, 3, out_mode=engine.OUT_NCHW_F32_SIGMOID)   # ragged third N tile
+            conv(1, 50, 60, 512, 1024, 1, relu=True, residual=True)        # mode 0, ragged last M tile, residual
+        finally:
+            _lib.lib().odtk_set_sm_budget(0)
         conv(2, 100, 160, 256, 36, 3, out_mode=engine.OUT_NCHW_F32)        # narrow head output, ragged N tile
         conv(1, 24, 32, 256, 720, 3, out_mode=engine.OUT_NCHW_F32_SIGMOID)
         conv(2, 26, 40, 128, 128, 3, relu=True, stride=2)                  # parity-split stride 2
