@@ -65,6 +65,18 @@ __device__ __forceinline__ void mma_block(float (&acc)[N / 2], uint64_t da, uint
   wgmma_commit();
 }
 
+// acc += bias of columns c0 + 8 j + 2 q (+1), in both accumulator rows: every bias load of an epilogue ahead of its stores.
+// No bias adds 0.0f, as the epilogues always have (-0.0f + 0.0f is +0.0f).
+template <int N>
+__device__ __forceinline__ void add_bias(float (&acc)[N / 2], const float *bias, int c0, int q) {
+#pragma unroll
+  for (int j = 0; j < N / 8; j++) {
+    const int col = c0 + 8 * j + 2 * q;
+    const float b0 = bias ? __ldg(bias + col) : 0.0f, b1 = bias ? __ldg(bias + col + 1) : 0.0f;
+    acc[4 * j] += b0; acc[4 * j + 1] += b1; acc[4 * j + 2] += b0; acc[4 * j + 3] += b1;
+  }
+}
+
 template <int C1, int N3>
 __global__ void __launch_bounds__(kThreads, 1)
 bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW2,
@@ -94,6 +106,9 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 
   if (wg == 0) {
     // ===================================== TMA producer =====================================
+    // the producer warpgroup hands its registers back (40 each) and the consumers take 232 (232 * 256 + 40 * 128 <= 64 K):
+    // GEMM3's accumulators of <64, 128> next to the prefetched identity do not fit in the 168 of a 384-thread CTA
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (tid != 0) return;
     Ring ring;
     ring.n = p.nstages;
@@ -137,6 +152,7 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
   }
 
   // ===================================== MMA + epilogues ====================================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
   const int cw = wg - 1, warp = tid >> 5, lane = tid & 31, q = lane & 3;
   const uint32_t mid_s = smem_u32(smem + p.mid_off), ysm_s = smem_u32(smem + p.ysm_off);
   const uint32_t rows = (uint32_t)(cw * 64 * 128);   // this warpgroup's 64 rows inside a [128][64] operand chunk
@@ -181,13 +197,13 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     }
     named_sync(1 + cw);   // the previous tile's GEMM2 / GEMM3 of every warp of this warpgroup read `mid` / `ysm`
     // ---- epilogue 1: mid = fp16(relu(acc1 + b2)) -> the A operand of GEMM2 ----
+    add_bias<C1>(acc1, p.b2, 0, q);
 #pragma unroll
     for (int j = 0; j < C1 / 8; j++) {
       const int col = 8 * j + 2 * q;
-      const float b0 = p.b2 ? __ldg(p.b2 + col) : 0.0f, b1 = p.b2 ? __ldg(p.b2 + col + 1) : 0.0f;
 #pragma unroll
       for (int i = 0; i < 2; i++) {
-        const __half2 v = __hmax2(__floats2half2_rn(acc1[4 * j + 2 * i] + b0, acc1[4 * j + 2 * i + 1] + b1), __float2half2_rn(0.0f));
+        const __half2 v = __hmax2(__floats2half2_rn(acc1[4 * j + 2 * i], acc1[4 * j + 2 * i + 1]), __float2half2_rn(0.0f));
         sts32(mid_s + (uint32_t)((col >> 6) * kChunk) + swz_off(prow[i], col), h2u(v));
       }
     }
@@ -195,6 +211,15 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     named_sync(1 + cw);
     // ---- GEMM2 per 128-channel output tile, + identity, epilogue 2 ----
     for (int n2 = 0; n2 < n2tiles; n2++) {
+      // the residual of this output tile is loaded before its MMAs and ahead of every store of y, which the compiler
+      // must assume may alias it
+      __half2 rv[2][16];
+      if (!p.proj)
+#pragma unroll
+        for (int i = 0; i < 2; i++)
+#pragma unroll
+          for (int j = 0; j < 16; j++)
+            if (valid[i]) rv[i][j] = *reinterpret_cast<const __half2 *>(p.residual + pix[i] * p.C2 + n2 * 128 + 8 * j + 2 * q);
       float acc2[64];
       for (int kb = 0; kb < KC1; kb++) {
         mbar_wait(&full[ring.stage], ring.phase);
@@ -209,15 +234,15 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
         consumed();
       }
       drain();
+      add_bias<128>(acc2, p.b3, n2 * 128, q);
 #pragma unroll
       for (int j = 0; j < 16; j++) {
         const int col = n2 * 128 + 8 * j + 2 * q;
-        const float b0 = p.b3 ? __ldg(p.b3 + col) : 0.0f, b1 = p.b3 ? __ldg(p.b3 + col + 1) : 0.0f;
 #pragma unroll
         for (int i = 0; i < 2; i++) {
-          float v0 = acc2[4 * j + 2 * i] + b0, v1 = acc2[4 * j + 2 * i + 1] + b1;
+          float v0 = acc2[4 * j + 2 * i], v1 = acc2[4 * j + 2 * i + 1];
           if (!p.proj && valid[i]) {
-            const float2 r = __half22float2(*reinterpret_cast<const __half2 *>(p.residual + pix[i] * p.C2 + col));
+            const float2 r = __half22float2(rv[i][j]);
             v0 += r.x; v1 += r.y;
           }
           __half2 y = __floats2half2_rn(v0, v1);
@@ -239,15 +264,15 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
         consumed();
       }
       drain();
+      add_bias<N3>(acc3, p.bn, 0, q);
 #pragma unroll
       for (int j = 0; j < N3 / 8; j++) {
         const int col = 8 * j + 2 * q;
-        const float b0 = p.bn ? __ldg(p.bn + col) : 0.0f, b1 = p.bn ? __ldg(p.bn + col + 1) : 0.0f;
 #pragma unroll
         for (int i = 0; i < 2; i++)
           if (valid[i])
             *reinterpret_cast<__half2 *>(p.z + pix[i] * N3 + col) =
-                __hmax2(__floats2half2_rn(acc3[4 * j + 2 * i] + b0, acc3[4 * j + 2 * i + 1] + b1), __float2half2_rn(0.0f));
+                __hmax2(__floats2half2_rn(acc3[4 * j + 2 * i], acc3[4 * j + 2 * i + 1]), __float2half2_rn(0.0f));
       }
     }
   }

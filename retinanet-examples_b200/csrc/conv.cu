@@ -245,11 +245,32 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     if (prev >= 0 && lane == 0) mbar_arrive(&bars->empty[prev]);
 
     // ---- epilogue: thread holds rows r and r + 8, columns 8 j + 2 q (+1) ----
+    // fp16: + bias goes into the accumulators first, all of the tile's bias loads ahead of any store.  Every global store
+    // below may alias a later load as far as the compiler knows, so a load left behind a store waits for it.
+    constexpr bool F16 = OP == kOpF16 || OP == kOpF16Mask;
+    if constexpr (F16) {
+      if (p.bias) {
+#pragma unroll
+        for (int j = 0; j < BN / 8; j++)
+#pragma unroll
+          for (int k = 0; k < 2; k++) {
+            const int col = n0 + 8 * j + 2 * q + k;
+            if (col >= p.Cout) continue;
+            const float b = __ldg(p.bias + col);
+            acc[4 * j + k] += b;
+            acc[4 * j + 2 + k] += b;
+          }
+      }
+    }
     // fp32 value of accumulator a in column col before the activation: + bias; s8: fmaf(acc, alpha, bias) (dequantise)
     auto head_val = [&](int a, int col) -> float {
-      const float b = p.bias ? __ldg(p.bias + col) : 0.0f;
-      if constexpr (S8) return fmaf((float)acc[a], __ldg(p.alpha + col), b);
-      else return acc[a] + b;
+      if constexpr (F16) {
+        return acc[a];
+      } else {
+        const float b = p.bias ? __ldg(p.bias + col) : 0.0f;
+        if constexpr (S8) return fmaf((float)acc[a], __ldg(p.alpha + col), b);
+        else return acc[a] + b;
+      }
     };
 #pragma unroll
     for (int i = 0; i < 2; i++) {
@@ -329,27 +350,41 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const __half *up = p.upsample ? p.upsample + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
         const __half *msk = nullptr;
         if constexpr (OP == kOpF16Mask) msk = p.mask ? p.mask + m * p.Cout : nullptr;
+        // 64 columns at a time: first every addend of the chunk into registers, then the stores -- one DRAM round trip per
+        // chunk instead of one per column pair.  Wider chunks spill at BN 256 and in the masked instance.
+        constexpr int kJ = 8;
 #pragma unroll
-        for (int j = 0; j < BN / 8; j++) {
-          const int col = n0 + 8 * j + 2 * q;
-          if (col >= p.Cout) continue;   // Cout % 16 == 0: both columns of the pair are in range or neither
-          float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
-          if (p.bias) { v0 += __ldg(p.bias + col); v1 += __ldg(p.bias + col + 1); }
-          if (res) { const float2 r = __half22float2(*reinterpret_cast<const __half2 *>(res + col)); v0 += r.x; v1 += r.y; }
-          if (up) { const float2 u = __half22float2(*reinterpret_cast<const __half2 *>(up + col)); v0 += u.x; v1 += u.y; }
-          if constexpr (OP == kOpF16Mask) {
-            if (msk) {   // a select, not a product: an inf gradient where the input was <= 0 still becomes 0
-              const __half2 mm = *reinterpret_cast<const __half2 *>(msk + col);
-              if (!(__low2float(mm) > 0.0f)) v0 = 0.0f;
-              if (!(__high2float(mm) > 0.0f)) v1 = 0.0f;
+        for (int j0 = 0; j0 < BN / 8; j0 += kJ) {
+          __half2 rv[kJ], uv[kJ], mv[kJ];
+#pragma unroll
+          for (int jj = 0; jj < kJ; jj++) {
+            const int col = n0 + 8 * (j0 + jj) + 2 * q;
+            if (col >= p.Cout) continue;   // Cout % 16 == 0: both columns of the pair are in range or neither
+            if (res) rv[jj] = *reinterpret_cast<const __half2 *>(res + col);
+            if (up) uv[jj] = *reinterpret_cast<const __half2 *>(up + col);
+            if constexpr (OP == kOpF16Mask)
+              if (msk) mv[jj] = *reinterpret_cast<const __half2 *>(msk + col);
+          }
+#pragma unroll
+          for (int jj = 0; jj < kJ; jj++) {
+            const int j = j0 + jj, col = n0 + 8 * j + 2 * q;
+            if (col >= p.Cout) continue;
+            float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+            if (res) { const float2 r = __half22float2(rv[jj]); v0 += r.x; v1 += r.y; }
+            if (up) { const float2 u = __half22float2(uv[jj]); v0 += u.x; v1 += u.y; }
+            if constexpr (OP == kOpF16Mask) {
+              if (msk) {   // a select, not a product: an inf gradient where the input was <= 0 still becomes 0
+                if (!(__low2float(mv[jj]) > 0.0f)) v0 = 0.0f;
+                if (!(__high2float(mv[jj]) > 0.0f)) v1 = 0.0f;
+              }
             }
+            __half2 y = __floats2half2_rn(v0, v1);
+            if (p.relu) {   // on the packed halves: max(round(x), 0) == round(max(x, 0))
+              y = __hmax2(y, __float2half2_rn(0.0f));
+              if (p.relu == 2) y = __hmin2(y, __float2half2_rn(6.0f));   // ReLU6: 6.0 is exact in fp16
+            }
+            *reinterpret_cast<__half2 *>(o + col) = y;
           }
-          __half2 y = __floats2half2_rn(v0, v1);
-          if (p.relu) {   // on the packed halves: max(round(x), 0) == round(max(x, 0))
-            y = __hmax2(y, __float2half2_rn(0.0f));
-            if (p.relu == 2) y = __hmin2(y, __float2half2_rn(6.0f));   // ReLU6: 6.0 is exact in fp16
-          }
-          *reinterpret_cast<__half2 *>(o + col) = y;
         }
       } else if (p.out_mode == ODTK_OUT_CANDIDATES) {
         // class-head final layer: only the scores above the threshold leave the SM, appended to the decode workspace as
