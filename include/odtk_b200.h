@@ -396,8 +396,9 @@ int odtk_relu_copy_rows_f32(const void *x, void *y, int n, int rows, int row_ele
 int odtk_quantize_f16_s8(const void *x, void *y, long long n, float inv_scale, odtk_stream_t stream);
 /* Introspection (tests): the kernel variant the last odtk_conv2d / odtk_stem_conv call of the calling host thread
  * launched.  mode: 0 GEMM rows (1x1), 1 shifted box per tap (3x3, odd-size stride 2), 2 stem, 3 even-size stride 2;
- * bn: N tile (64 or 128); grid: persistent CTAs.  cluster, npatch, tile_t, b_resident, bias_mma, res_mma, tma_store and
- * up_mma are always 0 on sm_90a (kept for ABI stability).  res_mma: 1 residual tile as one I * R
+ * bn: N tile (64, 128 or 256); grid: persistent CTAs; tma_store: 1 if the fp16 NHWC epilogue stores its tiles with TMA
+ * from shared memory (odtk_set_tma_store).  cluster, npatch, tile_t, b_resident, bias_mma, res_mma and up_mma are always
+ * 0 on sm_90a (kept for ABI stability).  res_mma: 1 residual tile as one I * R
  * product, 2 residual chunks through the pipeline stages (R_j * I64), 0 residual (if any) added in the epilogue.  */
 typedef struct {
   int mode, cluster, bn, num_m_tiles, num_n_tiles, nstages, npatch, tile_t, b_resident, bias_mma, res_mma, tma_store;
@@ -411,6 +412,10 @@ int odtk_conv_map_cache_stats(long long *hits, long long *misses);
  * head towers of one half batch next to the HBM-bound backbone layers of the other (Model.forward, pipelined mode).  A CUDA
  * graph keeps the grids it was captured with.                                                                          */
 int odtk_set_sm_budget(int sms);
+/* fp16 NHWC outputs of odtk_conv2d, odtk_stem_conv and odtk_bottleneck_tail: 1 (default) stores each tile with TMA from
+ * shared memory, 0 with direct stores from the registers; both give the same bytes.  Process-wide, read at launch time
+ * (a CUDA graph keeps what it captured); returns the previous setting.                                                  */
+int odtk_set_tma_store(int on);
 
 /* Buffers shared between the GPU processes of one node (CUDA IPC): odtk_peer_alloc = cudaMalloc + zero fill + a 64-byte
  * handle to send to the other ranks (any transport); odtk_peer_open maps a received handle into the CALLING process with

@@ -83,6 +83,7 @@ SIGNATURES = {
     "odtk_stem_pool": (ctypes.c_int, [ctypes.c_void_p] * 4 + [ctypes.c_int] * 5 + [ctypes.c_void_p]),
     "odtk_bottleneck_tail": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),
     "odtk_set_sm_budget": (ctypes.c_int, [ctypes.c_int]),
+    "odtk_set_tma_store": (ctypes.c_int, [ctypes.c_int]),
     "odtk_peer_alloc": (ctypes.c_int, [ctypes.c_size_t, ctypes.POINTER(ctypes.c_void_p), ctypes.c_void_p]),
     "odtk_peer_open": (ctypes.c_int, [ctypes.c_void_p, ctypes.POINTER(ctypes.c_void_p)]),
     "odtk_peer_close": (ctypes.c_int, [ctypes.c_void_p]),

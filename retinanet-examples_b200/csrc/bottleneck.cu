@@ -13,7 +13,9 @@
 //                   then Wn blocks, through one ring of full / empty mbarrier stages -- in the order the consumers use them.
 //   warpgroups 1-2  64 pixels of the 128-pixel tile each: wgmma.mma_async, fp32 accumulators in registers, epilogues.
 //                   Every A row a warpgroup reads from shared memory it wrote itself, so a 128-thread named barrier
-//                   (plus fence.proxy.async: generic-proxy stores -> async-proxy wgmma reads) is the only hand-over.
+//                   (plus fence.proxy.async: generic-proxy stores -> async-proxy wgmma reads) is the only hand-over
+//                   between MMAs.  y and z leave by TMA stores of whole 128-row chunks (stmatrix into shared memory,
+//                   then one thread issues the store), so those take a barrier of both consumer warpgroups.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -36,7 +38,8 @@ constexpr int kChunk = 16384;            // one 64-channel chunk of a [128 pixel
 
 struct BtParams {
   int N, H, W, C2, TH, TW, tiles_h, tiles_w, total_tiles, nstages, relu, proj;
-  int mid_off, ysm_off;                  // byte offsets of the mid / block-output operands in shared memory
+  int mid_off, ysm_off, bar_off;         // byte offsets of the mid / block-output operands and the barriers in shared memory
+  int tma_store;                         // y (and z) leave by TMA stores from ysm (odtk_set_tma_store)
   const float *b2, *b3, *bn;
   const __half *residual;
   __half *y, *z;
@@ -50,11 +53,8 @@ struct Ring {
 };
 
 __device__ __forceinline__ void named_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 3, 256;" ::: "memory"); }
 __device__ __forceinline__ void sts32(uint32_t saddr, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(saddr), "r"(v) : "memory"); }
-// (row, col) of a [128][64 k] 128B-swizzled K-major chunk: the 16-byte unit (col / 8) is XOR-ed with row % 8
-__device__ __forceinline__ uint32_t swz_off(int row, int col) {
-  return (uint32_t)(row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2);
-}
 __device__ __forceinline__ uint32_t h2u(__half2 h) { return *reinterpret_cast<uint32_t *>(&h); }
 
 template <int N>
@@ -82,10 +82,11 @@ __global__ void __launch_bounds__(kThreads, 1)
 bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW2,
                        const __grid_constant__ CUtensorMap tmW3, const __grid_constant__ CUtensorMap tmXp,
                        const __grid_constant__ CUtensorMap tmWp, const __grid_constant__ CUtensorMap tmWn,
-                       const __grid_constant__ BtParams p) {
+                       const __grid_constant__ BtParams p, const __grid_constant__ CUtensorMap tmY,
+                       const __grid_constant__ CUtensorMap tmZ) {
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t *full = reinterpret_cast<uint64_t *>(smem + p.ysm_off + (N3 ? (p.C2 / 64) * kChunk : 0));
+  uint64_t *full = reinterpret_cast<uint64_t *>(smem + p.bar_off);
   uint64_t *empty = full + kMaxStages;
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0), tid = threadIdx.x & 127;
   if (threadIdx.x == 0) {
@@ -156,6 +157,9 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
   const int cw = wg - 1, warp = tid >> 5, lane = tid & 31, q = lane & 3;
   const uint32_t mid_s = smem_u32(smem + p.mid_off), ysm_s = smem_u32(smem + p.ysm_off);
   const uint32_t rows = (uint32_t)(cw * 64 * 128);   // this warpgroup's 64 rows inside a [128][64] operand chunk
+  // stmatrix row address of this lane (TMA-store epilogues): row lane % 8 of matrix lane / 8; matrices 1 and 3 are the
+  // rows + 8, 2 and 3 the next 8 columns
+  const int srow = cw * 64 + warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, scol = (lane >> 4) * 8;
   Ring ring;
   ring.n = p.nstages;
   int prev = -1;
@@ -204,7 +208,7 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
 #pragma unroll
       for (int i = 0; i < 2; i++) {
         const __half2 v = __hmax2(__floats2half2_rn(acc1[4 * j + 2 * i], acc1[4 * j + 2 * i + 1]), __float2half2_rn(0.0f));
-        sts32(mid_s + (uint32_t)((col >> 6) * kChunk) + swz_off(prow[i], col), h2u(v));
+        sts32(mid_s + (uint32_t)((col >> 6) * kChunk) + swz128_off(prow[i], col), h2u(v));
       }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -235,6 +239,43 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
       }
       drain();
       add_bias<128>(acc2, p.b3, n2 * 128, q);
+      if (p.tma_store) {
+        // y by TMA, 64 columns at a time: stmatrix into its ysm chunk (GEMM3's operand) or, without GEMM3, into the one
+        // staging chunk, then one bulk tensor store of the TMA box {64, TW, TH, 1}, clipped at the image's edges
+#pragma unroll
+        for (int c = 0; c < 2; c++) {
+          const int k = 2 * n2 + c;
+          const uint32_t dst = ysm_s + (uint32_t)((N3 ? k : 0) * kChunk);
+          if (N3 == 0 || k == 0) {   // the previous stores from this chunk (the last tile's z, with GEMM3) have read it
+            if (threadIdx.x == 128) bulk_wait_read<0>();
+            consumers_sync();
+          }
+#pragma unroll
+          for (int jj = 0; jj < 8; jj += 2) {
+            uint32_t r[4];
+#pragma unroll
+            for (int t = 0; t < 4; t++) {
+              const int i = t & 1, j = 8 * c + jj + (t >> 1);
+              float v0 = acc2[4 * j + 2 * i], v1 = acc2[4 * j + 2 * i + 1];
+              if (!p.proj && valid[i]) {
+                const float2 r2 = __half22float2(rv[i][j]);
+                v0 += r2.x; v1 += r2.y;
+              }
+              __half2 y = __floats2half2_rn(v0, v1);
+              if (p.relu) y = __hmax2(y, __float2half2_rn(0.0f));
+              r[t] = h2u(y);
+            }
+            stmatrix_x4(dst + swz128_off(srow, 8 * jj + scol), r[0], r[1], r[2], r[3]);
+          }
+          fence_proxy_async();
+          consumers_sync();
+          if (threadIdx.x == 128) {
+            tma_store_4d(&tmY, dst, 64 * k, w0, h0, img);
+            bulk_commit();
+          }
+        }
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < 16; j++) {
         const int col = n2 * 128 + 8 * j + 2 * q;
@@ -248,7 +289,7 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
           __half2 y = __floats2half2_rn(v0, v1);
           if (p.relu) y = __hmax2(y, __float2half2_rn(0.0f));
           if (valid[i]) *reinterpret_cast<__half2 *>(p.y + pix[i] * p.C2 + col) = y;
-          if (N3) sts32(ysm_s + (uint32_t)((col >> 6) * kChunk) + swz_off(prow[i], col), h2u(y));
+          if (N3) sts32(ysm_s + (uint32_t)((col >> 6) * kChunk) + swz128_off(prow[i], col), h2u(y));
         }
       }
     }
@@ -265,6 +306,29 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
       }
       drain();
       add_bias<N3>(acc3, p.bn, 0, q);
+      if (p.tma_store) {
+        // z by TMA from ysm: once the y stores have read it (each warpgroup's GEMM3 read only its own rows, which only it
+        // overwrites)
+        if (threadIdx.x == 128) bulk_wait_read<0>();
+        consumers_sync();
+#pragma unroll
+        for (int jj = 0; jj < N3 / 8; jj += 2) {
+          uint32_t r[4];
+#pragma unroll
+          for (int t = 0; t < 4; t++) {
+            const int i = t & 1, j = jj + (t >> 1);
+            r[t] = h2u(__hmax2(__floats2half2_rn(acc3[4 * j + 2 * i], acc3[4 * j + 2 * i + 1]), __float2half2_rn(0.0f)));
+          }
+          stmatrix_x4(ysm_s + (uint32_t)((jj >> 3) * kChunk) + swz128_off(srow, 8 * (jj & 7) + scol), r[0], r[1], r[2], r[3]);
+        }
+        fence_proxy_async();
+        consumers_sync();
+        if (threadIdx.x == 128) {
+          for (int c = 0; c < N3 / 64; c++) tma_store_4d(&tmZ, ysm_s + (uint32_t)(c * kChunk), 64 * c, w0, h0, img);
+          bulk_commit();
+        }
+        continue;
+      }
 #pragma unroll
       for (int j = 0; j < N3 / 8; j++) {
         const int col = 8 * j + 2 * q;
@@ -276,6 +340,8 @@ bottleneck_tail_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
       }
     }
   }
+  // the bulk stores must have written y and z before the grid completes (the next kernel's griddepcontrol.wait)
+  if (threadIdx.x == 128) bulk_wait_all<0>();
 }
 
 template <int C1, int N3>
@@ -304,7 +370,7 @@ int launch(int grid, int smem_bytes, cudaStream_t stream, const CUtensorMap *tm,
   cfg.numAttrs = odtk_pdl_on() ? 1 : 0;
   {
     OdtkProfScope prof(ODTK_PROF_CONV, stream);
-    cudaLaunchKernelEx(&cfg, bottleneck_tail_kernel<C1, N3>, tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p);
+    cudaLaunchKernelEx(&cfg, bottleneck_tail_kernel<C1, N3>, tm[0], tm[1], tm[2], tm[3], tm[4], tm[5], p, tm[6], tm[7]);
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
@@ -333,17 +399,20 @@ extern "C" int odtk_bottleneck_tail(const odtk_bneck_t *d, odtk_stream_t stream_
   p.relu = d->relu; p.proj = proj;
   p.b2 = d->b2; p.b3 = d->b3; p.bn = d->b_next;
   p.residual = (const __half *)d->residual; p.y = (__half *)d->y; p.z = (__half *)d->z;
-  // shared memory: stages | mid [128][C1] | block output [128][C2] (GEMM3 only) | barriers
-  const int mid_bytes = (d->c1 / 64) * kChunk, ysm_bytes = n3 ? (d->c2 / 64) * kChunk : 0;
+  // shared memory: stages | mid [128][C1] | block output [128][C2] (GEMM3), or one 64-channel staging chunk of y for its
+  // TMA stores | barriers
+  p.tma_store = g_odtk_tma_store;
+  const int mid_bytes = (d->c1 / 64) * kChunk, ysm_bytes = n3 ? (d->c2 / 64) * kChunk : p.tma_store ? kChunk : 0;
   int nst = (kSmemLimit - 1024 - 256 - mid_bytes - ysm_bytes) / kStageBytes;
   if (nst > kMaxStages) nst = kMaxStages;
   if (nst < 2) return ODTK_E_UNSUPPORTED;
   p.nstages = nst;
   p.mid_off = nst * kStageBytes;
   p.ysm_off = p.mid_off + mid_bytes;
+  p.bar_off = p.ysm_off + ysm_bytes;
   const int smem_bytes = 1024 + p.ysm_off + ysm_bytes + 2 * kMaxStages * 8;
   const uint64_t C1 = (uint64_t)d->c1, C2 = (uint64_t)d->c2, H = (uint64_t)d->h, W = (uint64_t)d->width, N = (uint64_t)d->n;
-  CUtensorMap tm[6];
+  CUtensorMap tm[8];
   {
     uint64_t dims[4] = {C1, W, H, N}, str[3] = {C1 * 2, W * C1 * 2, H * W * C1 * 2};
     uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
@@ -371,6 +440,15 @@ extern "C" int odtk_bottleneck_tail(const odtk_bneck_t *d, odtk_stream_t stream_
     uint64_t dims[2] = {C2, (uint64_t)n3}, str[1] = {C2 * 2};
     uint32_t box[2] = {64, (uint32_t)n3};
     if (!encode_map(&tm[5], d->w_next, 2, dims, str, box)) return ODTK_E_CUDA;
+  }
+  tm[6] = tm[0]; tm[7] = tm[0];
+  if (p.tma_store) {   // y [n, h, width, c2] and z [n, h, width, n3] in boxes of 64 channels x the patch
+    uint64_t dims[4] = {C2, W, H, N}, str[3] = {C2 * 2, W * C2 * 2, H * W * C2 * 2};
+    uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+    if (!encode_map(&tm[6], d->y, 4, dims, str, box)) return ODTK_E_CUDA;
+    const uint64_t N3 = (uint64_t)n3;
+    uint64_t dimsZ[4] = {N3, W, H, N}, strZ[3] = {N3 * 2, W * N3 * 2, H * W * N3 * 2};
+    if (n3 && !encode_map(&tm[7], d->z, 4, dimsZ, strZ, box)) return ODTK_E_CUDA;
   }
   const int sms = odtk_sm_count();
   const int grid = p.total_tiles < sms ? p.total_tiles : sms;

@@ -15,6 +15,9 @@ static inline size_t odtk_align_up(size_t x) { return (x + ODTK_ALIGN - 1) / ODT
 // odtk_sm_count(), so two streams given complementary budgets run their kernels side by side on disjoint SMs
 // (odtk_set_sm_budget, include/odtk_b200.h).  Defined in version.cu.
 extern int g_odtk_sm_budget;
+// 1 (default): the fp16 NHWC epilogues store their tiles with TMA from shared memory; 0: direct stores from the registers
+// (odtk_set_tma_store).  Defined in version.cu.
+extern int g_odtk_tma_store;
 
 // SM count of the CURRENT device (cached per device ordinal; grids are sized from it, never from a constant)
 static inline int odtk_sm_count_device() {

@@ -13,7 +13,8 @@
 //   warpgroups 1-2  MMA + epilogue, 64 accumulator rows (output pixels) each: wgmma.mma_async m64nNk16 (N = BN = 64,
 //                   128 or, fp16 forward only, 256), fp32 accumulation in registers; the stage is released as soon as the next K block's
 //                   MMAs are in flight.  The epilogue works on the registers: + bias, + residual / FPN nearest-
-//                   upsample, ReLU / ReLU6, fp16 NHWC store -- or, for the last convolution of a head, (sigmoid +)
+//                   upsample, ReLU / ReLU6, fp16 NHWC store (fp16: stmatrix into shared memory, then a TMA store per
+//                   64 columns; a mode-0 residual arrives through the ring) -- or, for the last convolution of a head, (sigmoid +)
 //                   fp32 NCHW in the layout the reference's decode entry point expects -- or, class head on the
 //                   inference path, sigmoid + threshold + candidate append straight into the decode workspace.
 //
@@ -60,9 +61,15 @@ constexpr int kLoBytes = 64 * 128;
 constexpr int kSplitBytes = 2 * 2 * kLoBytes;
 constexpr int kSmemBytesF32 = kPipeBytes + kSplitBytes + 1024 + 256;
 static_assert(kSmemBytesF32 <= 227 * 1024, "fp32 instance exceeds the opt-in shared memory");
+// fp16 forward instances: after the stages, the two staging chunks of the TMA-store epilogue, [128 rows][64 channels] fp16
+// each in the 128-byte swizzle of a TMA box (one is filled while the bulk store of the other still reads it)
+constexpr int kStoreChunk = 128 * 128;
+constexpr int kSmemBytesF16 = kPipeBytes + 2 * kStoreChunk + 1024 + 256;
+static_assert(kSmemBytesF16 <= 227 * 1024, "fp16 instance exceeds the opt-in shared memory");
 
 // operand types of conv_gemm_kernel; kOpF16Mask: fp16 with the ReLU-derivative mask of the input gradient (odtk_conv2d_dgrad)
 enum ConvOp { kOpF16 = 0, kOpS8 = 1, kOpTF32x3 = 2, kOpF16Mask = 3 };
+constexpr int smem_bytes(int op) { return op == kOpTF32x3 ? kSmemBytesF32 : op == kOpF16 ? kSmemBytesF16 : kSmemBytes; }
 
 // round to the nearest tf32 value, ties away from zero (low 13 bits cleared)
 __device__ __forceinline__ float tf32_rna(float x) {
@@ -82,16 +89,22 @@ static_assert(sizeof(Barriers) <= 256, "barrier block too small");
 // MMAs are the integer m64nNk32 form with exact s32 accumulators, and the epilogue dequantises with fmaf(acc, alpha, bias).
 // OP kOpTF32x3: fp32 operands (odtk_conv2d_f32).  A K block is one 128-byte row of 32 channels; a stage holds A, then
 // B_hi and B_lo (tmB / tmB2); the MMAs are three m64nNk8 tf32 products per k8 step (see the file comment).
+// tmY (fp16 forward with p.tma_store): the NHWC output, written by TMA stores from shared memory (host: out_map); tmR (with
+// p.res_tma): the mode-0 residual [M, ldr], loaded by the producer into the ring after each tile's K blocks.  They come
+// after p so that the other instances keep their parameter offsets.
 template <int BN, int OP>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
-                 const __grid_constant__ ConvParams p) {
+                 const __grid_constant__ ConvParams p, const __grid_constant__ CUtensorMap tmY,
+                 const __grid_constant__ CUtensorMap tmR) {
   constexpr bool S8 = OP == kOpS8, F32 = OP == kOpTF32x3;
+  // residual boxes ([128 rows][64 channels], 16 KB) per ring stage: stages hold 24, 32 or 48 KB at BN 64, 128, 256
+  constexpr int kResPerStage = BN == 64 ? 1 : 2;
   constexpr int BR = F32 ? 2 * BN : BN;   // B rows per stage: fp32 carries w_hi and w_lo
   extern __shared__ unsigned char smem_raw[];
   unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  Barriers *bars = reinterpret_cast<Barriers *>(smem + kPipeBytes + (F32 ? kSplitBytes : 0));
+  Barriers *bars = reinterpret_cast<Barriers *>(smem + kPipeBytes + (F32 ? kSplitBytes : OP == kOpF16 ? 2 * kStoreChunk : 0));
   const int kStages = p.nstages, rb = p.row_bytes;
   const int stage_bytes = (128 + BR) * rb;
   const int wg = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 7), 0), tid = threadIdx.x & 127;
@@ -170,6 +183,18 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         tma_load_2d(sa + 128 * 128, &tmB2, &bars->full[stage], j * 64, n0);
         if (++stage == kStages) { stage = 0; phase ^= 1u; }
       }
+      if constexpr (OP == kOpF16) {
+        if (p.res_tma) {   // the tile's residual, while its MMAs still run; rows past M and columns past Cout read as 0
+          for (int c = 0; c < BN / 64; c += kResPerStage) {
+            mbar_wait(&bars->empty[stage], phase ^ 1u);
+            unsigned char *sr = smem + stage * stage_bytes;
+            mbar_arrive_expect_tx(&bars->full[stage], (uint32_t)(kResPerStage * kStoreChunk));
+            for (int k = 0; k < kResPerStage; k++)
+              tma_load_2d(sr + k * kStoreChunk, &tmR, &bars->full[stage], n0 + 64 * (c + k), m_tile * 128);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+        }
+      }
     }
     return;
   }
@@ -182,6 +207,7 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   typename std::conditional<S8, int, float>::type acc[BN / 2];
   int stage = 0;
   uint32_t phase = 0;
+  int sbuf = 0;   // TMA-store epilogue: the staging chunk the next 64 columns go to
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     int m_tile, n_tile, img0, h0, w0, hlim, wlim;
     tile_origin(tile, m_tile, n_tile, img0, h0, w0, hlim, wlim);
@@ -272,6 +298,99 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         else return acc[a] + b;
       }
     };
+    if constexpr (OP == kOpF16) {
+      // TMA-store epilogue, 64 columns at a time: both consumer warpgroups write the chunk's fp16 values into a staging
+      // chunk with stmatrix (its fragment layout is the accumulator's), then one thread stores the chunk with one bulk
+      // tensor store.  The map clips the box at the output's edges (rows past M, the image or the level, columns past
+      // Cout), so only tile-table tiles that end inside the atlas's gaps keep the direct stores below.  A residual comes
+      // through the ring (p.res_tma; the host sends launches whose residual cannot to the direct path) and is read with
+      // ldmatrix in the same layout; the upsample addend is loaded into registers.
+      if (p.tma_store && (!p.tile_tab || (h0 + p.TH <= hlim && w0 + p.TW <= wlim))) {
+        const __half *up[2];
+#pragma unroll
+        for (int i = 0; i < 2; i++) {
+          const int row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;
+          int img = img0, h, w;
+          bool valid;
+          if (p.mode != 0) {
+            const int dh = row / p.TW, dw = row - dh * p.TW;
+            h = h0 + dh; w = w0 + dw;
+            valid = row < patch && h < hlim && w < wlim;
+          } else {
+            const long long m = (long long)m_tile * 128 + row;
+            valid = m < p.M;
+            img = (int)(m / hw);
+            const int rem = (int)(m - (long long)img * hw);
+            h = rem / p.W;
+            w = rem - h * p.W;
+          }
+          up[i] = p.upsample && valid ? p.upsample + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
+        }
+        // ldmatrix / stmatrix row address of this lane: row lane % 8 of matrix lane / 8; matrices 1 and 3 are the rows + 8,
+        // 2 and 3 the next 8 columns
+        const int srow = cw * 64 + warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8, scol = (lane >> 4) * 8;
+        const uint32_t stg = smem_u32(smem + kPipeBytes);
+        // upsample addends of kJ column blocks (8 columns each) and both rows into registers ahead of their stmatrix: one
+        // DRAM round trip per batch.  A whole chunk's batch spills at BN 256.
+        constexpr int kJ = BN == 256 ? 4 : 8;
+#pragma unroll
+        for (int c = 0; c < BN / 64; c++) {
+          const uint32_t buf = stg + (uint32_t)(sbuf * kStoreChunk);
+          const uint32_t rbox = smem_u32(smem + stage * stage_bytes) + (uint32_t)((c % kResPerStage) * kStoreChunk);
+          if (p.res_tma && c % kResPerStage == 0) mbar_wait(&bars->full[stage], phase);
+#pragma unroll
+          for (int jb = 0; jb < 8; jb += kJ) {
+            __half2 uv[2][kJ];
+#pragma unroll
+            for (int jj = 0; jj < kJ; jj++) {
+              const int col = n0 + 64 * c + 8 * (jb + jj) + 2 * q;
+              if (col >= p.Cout) continue;   // Cout % 16 == 0: both columns of the pair are in range or neither
+#pragma unroll
+              for (int i = 0; i < 2; i++)
+                if (up[i]) uv[i][jj] = *reinterpret_cast<const __half2 *>(up[i] + col);
+            }
+            if (jb == 0) {
+              if (threadIdx.x == 128) bulk_wait_read<1>();   // the store issued two chunks ago has read this staging chunk
+              asm volatile("bar.sync 3, 256;" ::: "memory");
+            }
+#pragma unroll
+            for (int jj = 0; jj < kJ; jj += 2) {
+              const uint32_t off = swz128_off(srow, 8 * (jb + jj) + scol);
+              uint32_t r[4];
+              if (p.res_tma) ldmatrix_x4(rbox + off, r[0], r[1], r[2], r[3]);
+#pragma unroll
+              for (int t = 0; t < 4; t++) {
+                const int i = t & 1, jl = jj + (t >> 1), j = 8 * c + jb + jl;
+                float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+                if (p.res_tma) { const float2 a = __half22float2(*reinterpret_cast<const __half2 *>(&r[t])); v0 += a.x; v1 += a.y; }
+                if (up[i] && n0 + 8 * j + 2 * q < p.Cout) { const float2 a = __half22float2(uv[i][jl]); v0 += a.x; v1 += a.y; }
+                __half2 y = __floats2half2_rn(v0, v1);
+                if (p.relu) {   // on the packed halves: max(round(x), 0) == round(max(x, 0))
+                  y = __hmax2(y, __float2half2_rn(0.0f));
+                  if (p.relu == 2) y = __hmin2(y, __float2half2_rn(6.0f));   // ReLU6: 6.0 is exact in fp16
+                }
+                r[t] = *reinterpret_cast<const uint32_t *>(&y);
+              }
+              stmatrix_x4(buf + off, r[0], r[1], r[2], r[3]);
+            }
+          }
+          if (p.res_tma && (c + 1) % kResPerStage == 0) {   // this warp has read the residual stage
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&bars->empty[stage]);
+            if (++stage == kStages) { stage = 0; phase ^= 1u; }
+          }
+          fence_proxy_async();
+          asm volatile("bar.sync 3, 256;" ::: "memory");
+          if (threadIdx.x == 128) {
+            if (p.mode == 0) tma_store_2d(&tmY, buf, n0 + 64 * c, m_tile * 128);
+            else tma_store_4d(&tmY, buf, n0 + 64 * c, w0, h0, img0);
+            bulk_commit();
+          }
+          sbuf ^= 1;
+        }
+        continue;
+      }
+    }
 #pragma unroll
     for (int i = 0; i < 2; i++) {
       const int row = cw * 64 + warp * 16 + (lane >> 2) + 8 * i;
@@ -350,9 +469,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         const __half *up = p.upsample ? p.upsample + (((long long)img * p.up_h + (h >> 1)) * p.up_w + (w >> 1)) * p.Cout : nullptr;
         const __half *msk = nullptr;
         if constexpr (OP == kOpF16Mask) msk = p.mask ? p.mask + m * p.Cout : nullptr;
-        // 64 columns at a time: first every addend of the chunk into registers, then the stores -- one DRAM round trip per
-        // chunk instead of one per column pair.  Wider chunks spill at BN 256 and in the masked instance.
-        constexpr int kJ = 8;
+        // 64 columns at a time (32 at BN 256, next to the TMA-store epilogue): first every addend of the chunk into
+        // registers, then the stores -- one DRAM round trip per chunk instead of one per column pair.  Wider chunks spill.
+        constexpr int kJ = BN == 256 ? 4 : 8;
 #pragma unroll
         for (int j0 = 0; j0 < BN / 8; j0 += kJ) {
           __half2 rv[kJ], uv[kJ], mv[kJ];
@@ -441,6 +560,9 @@ conv_gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       }
     }
   }
+  // the bulk stores must have written the output before the grid completes (the next kernel's griddepcontrol.wait)
+  if constexpr (OP == kOpF16)
+    if (threadIdx.x == 128) bulk_wait_all<0>();
 }
 
 // ---------------------------------------------------------------------------------- host
@@ -534,18 +656,18 @@ namespace {
 
 template <int BN, int OP>
 void launch_bn(int grid, cudaStream_t stream, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
-               const CUtensorMap &tmB2, const ConvParams &p) {
+               const CUtensorMap &tmB2, const ConvParams &p, const CUtensorMap &tmY, const CUtensorMap &tmR) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = OP == kOpTF32x3 ? kSmemBytesF32 : kSmemBytes;
+  cfg.dynamicSmemBytes = smem_bytes(OP);
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
   cfg.numAttrs = odtk_pdl_on() ? 1 : 0;
-  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, OP>, tmA, tmB, tmA2, tmB2, p);
+  cudaLaunchKernelEx(&cfg, conv_gemm_kernel<BN, OP>, tmA, tmB, tmA2, tmB2, p, tmY, tmR);
 }
 
 // Every compile-time instance of conv_gemm_kernel: N tile, operand type, launcher and dynamic shared memory.
@@ -553,12 +675,12 @@ struct Instance {
   int bn, op;
   const void *fn;
   void (*launch)(int, cudaStream_t, const CUtensorMap &, const CUtensorMap &, const CUtensorMap &, const CUtensorMap &,
-                 const ConvParams &);
+                 const ConvParams &, const CUtensorMap &, const CUtensorMap &);
   int smem;
 };
 template <int BN, int OP>
 constexpr Instance instance() {
-  return {BN, OP, (const void *)conv_gemm_kernel<BN, OP>, launch_bn<BN, OP>, OP == kOpTF32x3 ? kSmemBytesF32 : kSmemBytes};
+  return {BN, OP, (const void *)conv_gemm_kernel<BN, OP>, launch_bn<BN, OP>, smem_bytes(OP)};
 }
 const Instance kInstances[] = {instance<64, kOpF16>(),     instance<128, kOpF16>(),     instance<256, kOpF16>(),
                                instance<64, kOpS8>(),      instance<128, kOpS8>(),      instance<64, kOpTF32x3>(),
@@ -599,16 +721,47 @@ bool wide_tiles_pay(const ConvParams &p, int cout) {
          (long long)p.num_m_tiles * ((cout + 255) / 256) >= (long long)kWideWaves * odtk_sm_count();
 }
 
-int launch(const ConvParams &p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
+// Output map of the TMA-store epilogue (fp16 NHWC, row stride ldy, a multiple of 8 elements): mode 0 a 2-D map over the
+// [M, ldy] rows in {64, 128} boxes; the spatial modes a 4-D map {Cout, W, H, N} whose origin is row oR of the output view
+// and whose strides are those of the view, in {64, TW, TH, 1} boxes -- the box is clipped at the level's own W and H, so
+// nothing outside the view's rectangle is written.
+bool out_map(const ConvParams &p, CUtensorMap &tmY) {
+  const uint64_t ldy = (uint64_t)p.ldy * 2;
+  if (p.mode == 0) {
+    uint64_t dims[2] = {(uint64_t)p.Cout, (uint64_t)p.M}, str[1] = {ldy};
+    uint32_t box[2] = {64, 128};
+    return encode_map(&tmY, p.out, 2, dims, str, box);
+  }
+  const unsigned char *base = reinterpret_cast<const unsigned char *>(p.out) + (uint64_t)p.oR * p.oW * ldy;
+  uint64_t dims[4] = {(uint64_t)p.Cout, (uint64_t)p.W, (uint64_t)p.H, (uint64_t)p.N};
+  uint64_t str[3] = {ldy, (uint64_t)p.oW * ldy, (uint64_t)p.oH * p.oW * ldy};
+  uint32_t box[4] = {64, (uint32_t)p.TW, (uint32_t)p.TH, 1};
+  return encode_map(&tmY, base, 4, dims, str, box);
+}
+
+int launch(ConvParams p, int BN, const CUtensorMap &tmA, const CUtensorMap &tmB, const CUtensorMap &tmA2,
            const CUtensorMap &tmB2, cudaStream_t stream, int op) {
   const int total = p.num_m_tiles * p.num_n_tiles;
   const int sms = odtk_sm_count();   // the launch budget (odtk_set_sm_budget) or the whole device
   const int grid = total < sms ? total : sms;
-  g_last_plan = odtk_conv_plan_t{p.mode, 0, BN, p.num_m_tiles, p.num_n_tiles, p.nstages, 0, 0, 0, 0, 0, 0, p.TH, p.TW, grid, 0};
+  CUtensorMap tmY = tmA, tmR = tmA;
+  p.tma_store = op == kOpF16 && p.out_mode == ODTK_OUT_NHWC_F16 && g_odtk_tma_store;
+  if (p.tma_store && p.residual) {
+    // the residual goes through the ring as [M, ldr] rows in {64, 128} boxes: mode 0, 16-byte aligned rows; other
+    // residual launches keep the direct epilogue
+    p.res_tma = p.mode == 0 && !((uintptr_t)p.residual & 15) && p.ldr % 8 == 0;
+    p.tma_store = p.res_tma;
+    uint64_t dims[2] = {(uint64_t)p.Cout, (uint64_t)p.M}, str[1] = {(uint64_t)p.ldr * 2};
+    uint32_t box[2] = {64, 128};
+    if (p.res_tma && !encode_map(&tmR, p.residual, 2, dims, str, box)) return ODTK_E_CUDA;
+  }
+  if (p.tma_store && !out_map(p, tmY)) return ODTK_E_CUDA;
+  g_last_plan = odtk_conv_plan_t{p.mode, 0, BN, p.num_m_tiles, p.num_n_tiles, p.nstages, 0, 0, 0, 0, 0, p.tma_store,
+                                 p.TH, p.TW, grid, 0};
   for (const Instance &k : kInstances)
     if (k.bn == BN && k.op == op) {
       OdtkProfScope prof(ODTK_PROF_CONV, stream);
-      k.launch(grid, stream, tmA, tmB, tmA2, tmB2, p);
+      k.launch(grid, stream, tmA, tmB, tmA2, tmB2, p, tmY, tmR);
       return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
     }
   return ODTK_E_UNSUPPORTED;

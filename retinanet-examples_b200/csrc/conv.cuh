@@ -57,4 +57,7 @@ struct ConvParams {
   // input-gradient instance (odtk_conv2d_dgrad): NHWC fp16 [M, Cout] at the output pixel; an output element whose mask
   // element is not > 0 becomes 0 (the ReLU derivative of the forward layer's input), or NULL
   const __half *mask;
+  // fp16 forward, ODTK_OUT_NHWC_F16: 1 if the epilogue stores through the output tensor map (TMA from shared memory), and
+  // res_tma 1 if the producer then loads the residual (mode 0) into the ring after each tile's K blocks
+  int tma_store, res_tma;
 };

@@ -50,6 +50,42 @@ __device__ __forceinline__ void tma_load_5d(void *dst, const CUtensorMap *map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
       : "memory");
 }
+// TMA stores (shared -> global, bulk-group completion): the box is clipped at the tensor map's bounds.  Only the thread
+// that issued them may wait for them: wait_read<N> until at most N of its groups still read shared memory (the source may
+// then be overwritten), wait_all<0> until their writes are performed.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap *map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap *map, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(map), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// generic-proxy shared-memory writes -> later async-proxy (TMA, wgmma) reads of them
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// four 8x8 fp16 matrices into shared memory: lane t gives the address of row t % 8 of matrix t / 8, register i of lane t
+// holds row t / 4, columns 2 (t % 4) (+1) of matrix i -- the layout of a wgmma accumulator fragment.  No memory clobber:
+// global loads may be scheduled across it; what reads the chunk (TMA, wgmma) follows a fence and a barrier, both volatile.
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3));
+}
+// the inverse of stmatrix_x4: lane t's registers receive its accumulator-fragment elements of the four matrices
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t &r0, uint32_t &r1, uint32_t &r2, uint32_t &r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
+}
+// (row, col) of a [rows][64 fp16] chunk in the 128-byte swizzle of a TMA box / wgmma operand (1024-byte aligned): the
+// 16-byte unit col / 8 is XOR-ed with row % 8
+__device__ __forceinline__ uint32_t swz128_off(int row, int col) {
+  return (uint32_t)(row * 128 + ((((col & 63) >> 3) ^ (row & 7)) << 4) + (col & 7) * 2);
+}
+
 // Programmatic dependent launch: a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may start while
 // its predecessor in the stream is still running.  launch_dependents lets the NEXT kernel's CTAs take the SMs this
 // kernel's CTAs free as they exit (its prologue -- barrier init, descriptor prefetch -- then overlaps this kernel's tail);

@@ -9,3 +9,11 @@ extern "C" int odtk_set_sm_budget(int sms) {
   g_odtk_sm_budget = sms & ~1;
   return ODTK_OK;
 }
+int g_odtk_tma_store = 1;
+// fp16 NHWC convolution / bottleneck-tail outputs: TMA stores from shared memory (1) or direct stores (0); returns the
+// previous setting.  Read at launch time, like the budget.
+extern "C" int odtk_set_tma_store(int on) {
+  const int prev = g_odtk_tma_store;
+  g_odtk_tma_store = on != 0;
+  return prev;
+}

@@ -204,6 +204,12 @@ def main():
         conv(2, 26, 40, 128, 128, 3, relu=True, stride=2)                  # parity-split stride 2
         conv(2, 25, 39, 256, 256, 3, relu=True, stride=2)                  # element-strided boxes
         conv(40, 100, 160, 64, 256, 1, relu=True)                          # enough tiles for 1x1
+        _lib.lib().odtk_set_tma_store(0)                                   # the direct-store epilogues
+        try:
+            conv(2, 16, 16, 256, 256, 1, relu=True, residual=True)
+            conv(1, 7, 10, 256, 256, 3, relu=True)
+        finally:
+            _lib.lib().odtk_set_tma_store(1)
         for c1, proj in ((64, False), (128, False), (64, True)):           # fused bottleneck tail: residual / streamed weights / projected identity
             c2 = 4 * c1
             xx, w2 = rnd(3, 9, 17, c1), engine.pack_weight(torch.randn((c1, c1, 3, 3), generator=g) * 0.05).to(DEV)
