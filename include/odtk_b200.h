@@ -637,6 +637,55 @@ long long odtk_decode_jpeg(const void *in, size_t in_bytes, const odtk_jpeg_imag
                            const odtk_resize_image_t *outs, const odtk_resize_image_t *outs_dev, void *workspace,
                            size_t workspace_bytes, void *y, size_t y_bytes, int *status, odtk_stream_t stream);
 
+/* ---- training input: uint8 resize and augmentation (odtk/data.py:55-123 with training=True) ----------------------
+ * The resize of odtk_preprocess_resize_u8 (same kernel, same Pillow-exact BILINEAR arithmetic) keeping Pillow's uint8
+ * result: image i is written as dst_h x dst_w HWC RGB at y + out_off[i], nothing else is written.
+ *   images / images_dev, x_bytes   as odtk_preprocess_resize_u8;
+ *   out_off / out_off_dev          host / device int64 [n] output offsets: the host copy is validated, never read by the
+ *                                  kernel; every image must lie in [y, y + y_bytes).
+ * Two-phase: y == NULL returns the bytes of the images packed one after another.  ODTK_E_INVALID as
+ * odtk_preprocess_resize_u8, or an output outside [y, y + y_bytes).                                                  */
+long long odtk_resize_u8_packed(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                const odtk_resize_image_t *images_dev, const long long *out_off,
+                                const long long *out_off_dev, int n, void *y, size_t y_bytes, odtk_stream_t stream);
+
+#define ODTK_AUGMENT_BRIGHTNESS 1
+#define ODTK_AUGMENT_CONTRAST 2
+#define ODTK_AUGMENT_HUE 4
+#define ODTK_AUGMENT_SATURATION 8
+
+/* One image of odtk_augment_u8. */
+typedef struct {
+  long long offset;        /* its resized uint8 HWC RGB pixels (h x w) start `offset` bytes into x               */
+  int h, w;                /* resized size                                                                       */
+  int rot;                 /* Image.rotate(90 * rot), counter-clockwise, 0..3                                     */
+  int expand;              /* rotate(..., expand=True): 90 / 270 give a w x h transpose.  0: the size stays h x w  */
+                           /* and a non-square image is resampled NEAREST about its centre with black fill        */
+  int flip;                /* then Image.FLIP_LEFT_RIGHT                                                          */
+  int flags;               /* ODTK_AUGMENT_* adjustments applied, always in the order of the bit values           */
+  float brightness;        /* ImageEnhance factors, as the C float Image.blend takes them, >= 0                   */
+  float contrast;
+  float saturation;
+  int hue_shift;           /* 0..255, added modulo 256 to H of the uint8 HSV round trip                           */
+} odtk_augment_image_t;
+
+/* The per-image augmentations of CocoDataset / RotatedCocoDataset.__getitem__ (odtk/data.py:64-123) on uint8 images,
+ * bit-exact to Pillow and torchvision's PIL functional: rotation, horizontal flip, ImageEnhance.Brightness (blend with
+ * black), ImageEnhance.Contrast (blend with the grey int(mean(L) + 0.5), L the fixed-point convert("L") of the image
+ * after rotation, flip and brightness, rotation fill included), adjust_hue (convert("HSV"), H += hue_shift,
+ * convert("RGB")), ImageEnhance.Color (blend with convert("L")), then the normalisation of odtk_preprocess_u8.  The
+ * result is the collated batch y, fp32 [n, canvas_h, canvas_w, 3] (NCHW's channels_last), every pixel outside an
+ * image's rotated size exactly 0.0.  Two kernels: L sums (only when an image has ODTK_AUGMENT_CONTRAST), then one
+ * thread per canvas pixel.
+ *   images / images_dev  host copy (validated, never read by a kernel) / device copy of the n descriptors;
+ *   workspace            8 bytes per image (the L sums).
+ * Two-phase: workspace == NULL returns the workspace bytes.  ODTK_E_INVALID: a size <= 0, a rotated size larger than
+ * the canvas, an image outside [x, x + x_bytes), rot outside 0..3, unknown flags, a negative or NaN factor, a
+ * hue_shift outside 0..255; ODTK_E_WORKSPACE: workspace_bytes too small.                                              */
+long long odtk_augment_u8(const void *x, size_t x_bytes, const odtk_augment_image_t *images,
+                          const odtk_augment_image_t *images_dev, int n, int canvas_h, int canvas_w, void *workspace,
+                          size_t workspace_bytes, float *y, const float *mean, const float *std, odtk_stream_t stream);
+
 /* ---- per-kernel timing (H100-native addition; the reference has only a wall-clock
  * Profiler without CUDA sync, odtk/utils.py:140-167) ------------------------------
  * When enabled, every launch of a tagged kernel is bracketed by CUDA events on the

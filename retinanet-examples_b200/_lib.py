@@ -106,6 +106,11 @@ SIGNATURES = {
     "odtk_decode_jpeg": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                              ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_size_t,
                                              ctypes.c_void_p, ctypes.c_void_p]),
+    "odtk_resize_u8_packed": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t] + [ctypes.c_void_p] * 4 +
+                              [ctypes.c_int, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
+    "odtk_augment_u8": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, ctypes.c_void_p] +
+                        [ctypes.c_int] * 3 + [ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p, _c_f32p, _c_f32p,
+                                              ctypes.c_void_p]),
     "odtk_prof_enable": (None, [ctypes.c_int]),
     "odtk_prof_reset": (None, []),
     "odtk_prof_get_list": (ctypes.c_longlong, [ctypes.c_int, ctypes.POINTER(ctypes.c_float), ctypes.c_longlong]),
@@ -153,6 +158,15 @@ class ResizeImage(ctypes.Structure):
     """odtk_resize_image_t (include/odtk_b200.h)."""
     _fields_ = [("offset", ctypes.c_longlong), ("src_h", ctypes.c_int), ("src_w", ctypes.c_int), ("dst_h", ctypes.c_int),
                 ("dst_w", ctypes.c_int)]
+
+
+AUGMENT_BRIGHTNESS, AUGMENT_CONTRAST, AUGMENT_HUE, AUGMENT_SATURATION = 1, 2, 4, 8   # ODTK_AUGMENT_*
+
+
+class AugmentImage(ctypes.Structure):
+    """odtk_augment_image_t (include/odtk_b200.h)."""
+    _fields_ = [("offset", ctypes.c_longlong)] + [(f, ctypes.c_int) for f in ("h", "w", "rot", "expand", "flip", "flags")] + \
+               [(f, ctypes.c_float) for f in ("brightness", "contrast", "saturation")] + [("hue_shift", ctypes.c_int)]
 
 
 class JpegImage(ctypes.Structure):

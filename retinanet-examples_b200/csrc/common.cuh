@@ -131,6 +131,11 @@ __device__ __forceinline__ void odtk_find_bstar(const uint32_t *shist, int top_n
   nsel = s_res[1];
 }
 
+// One channel of odtk's input normalisation (reference odtk/data.py:118-121), same operation order as the reference:
+// float(u8) / 255, then - mean, then / std, fp32.  Shared by the preprocess kernels (layers.cu) and the training
+// augmentation (augment.cu).
+__device__ __forceinline__ float normalize_u8(unsigned v, float m, float s) { return ((float)v / 255.0f - m) / s; }
+
 __host__ __device__ __forceinline__ int odtk_next_pow2(int x) {
   int p = 32;
   while (p < x) p <<= 1;

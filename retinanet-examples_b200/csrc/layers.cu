@@ -152,10 +152,6 @@ __global__ void pad_input_rows_kernel(const __half *__restrict__ x, __half *__re
   }
 }
 
-// One channel of odtk infer's input normalisation (reference odtk/data.py:118-121), same operation order as the
-// reference: float(u8) / 255, then - mean, then / std, fp32.
-__device__ __forceinline__ float normalize_u8(unsigned v, float m, float s) { return ((float)v / 255.0f - m) / s; }
-
 // One RGB pixel of it as the stem's 8-byte NHWC4 pixel: one fp16 rounding.
 __device__ __forceinline__ uint2 normalize_rgb_u8(unsigned r8, unsigned g8, unsigned b8, float m0, float m1, float m2,
                                                   float s0, float s1, float s2) {
@@ -256,24 +252,29 @@ __device__ __forceinline__ unsigned resample_clip8(int acc) { return (unsigned)m
 __device__ __forceinline__ int resample_acc_init() { return 1 << (RS_BITS - 1); }
 
 // F32: the full-precision stem buffer, 16-byte fp32 NHWC4 pixels (normalize_rgb_u8_f32) instead of 8-byte fp16 ones.
-template <bool F32>
+// U8: Pillow's uint8 result itself, HWC RGB packed per image at y + out_off[n] (dst_h x dst_w, no border, no canvas), for
+// the training augmentations that run on it; HS / WS and the normalisation are not used, the tile origin is (0, 0).
+template <bool F32, bool U8 = false>
 __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kernel(
     const unsigned char *__restrict__ x, const odtk_resize_image_t *__restrict__ tab,
-    typename std::conditional<F32, float4, uint2>::type *__restrict__ y, int HS, int WS,
-    float m0, float m1, float m2, float s0, float s1, float s2) {
+    typename std::conditional<U8, unsigned char, typename std::conditional<F32, float4, uint2>::type>::type *__restrict__ y,
+    int HS, int WS, float m0, float m1, float m2, float s0, float s1, float s2, const long long *__restrict__ out_off = nullptr) {
   using Pix = typename std::conditional<F32, float4, uint2>::type;
   __shared__ int s_wx[RS_KMAX][RS_TW], s_wy[RS_TH][RS_KMAX];     // column taps tap-major: lanes read consecutive words
   __shared__ int s_lox[RS_TW], s_nx[RS_TW], s_loy[RS_TH], s_ny[RS_TH];
-  __shared__ Pix s_norm[256];   // normalize_rgb_u8(v, v, v): channel c of a pixel is its value's channel c
+  // normalize_rgb_u8(v, v, v): channel c of a pixel is its value's channel c.  The U8 instance neither fills nor reads
+  // it (nor HP / WP); it stays declared here so that the fp16 / fp32 instances keep their exact shared-memory layout.
+  __shared__ Pix s_norm[256];
   const int HP = HS + 6, WP = WS + 8;
   const int n = blockIdx.z;
   const odtk_resize_image_t im = tab[n];
   const int tx = threadIdx.x % RS_TW, ty = threadIdx.x / RS_TW;
-  const int x0 = blockIdx.x * RS_TW - 3, y0 = blockIdx.y * RS_TH - 3;     // tile origin in image coordinates
+  constexpr int B = U8 ? 0 : 3;                                             // stem border
+  const int x0 = blockIdx.x * RS_TW - B, y0 = blockIdx.y * RS_TH - B;     // tile origin in image coordinates
   const int ox = x0 + tx, xp = ox + 3;
   const bool meets = x0 + RS_TW > 0 && x0 < im.dst_w && y0 + RS_TH > 0 && y0 < im.dst_h;                       // block-uniform
   const bool tables = meets && resample_ksize(im.src_w, im.dst_w) <= RS_KMAX && resample_ksize(im.src_h, im.dst_h) <= RS_KMAX;
-  if (meets) {
+  if (meets && !U8) {
     for (int v = threadIdx.x; v < 256; v += RS_TW * RS_ROWS) {
       if constexpr (F32) s_norm[v] = normalize_rgb_u8_f32(v, v, v, m0, m1, m2, s0, s1, s2);
       else s_norm[v] = normalize_rgb_u8(v, v, v, m0, m1, m2, s0, s1, s2);
@@ -323,7 +324,7 @@ __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kerne
   const long long pitch = (long long)im.src_w * 3;
   for (int r = ty; r < RS_TH; r += RS_ROWS) {
     const int oy = y0 + r, yp = oy + 3;
-    if (yp >= HP) break;
+    if (U8 ? oy >= im.dst_h : yp >= HP) break;
     Pix v;
     if constexpr (F32) v = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
     else v = make_uint2(0u, 0u);
@@ -359,6 +360,12 @@ __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kerne
           for (int c = 0; c < 3; c++) acc[c] += (int)resample_clip8(h[c]) * kv;
         }
       }
+      if constexpr (U8) {
+        unsigned char *o = y + out_off[n] + ((long long)oy * im.dst_w + ox) * 3;
+#pragma unroll
+        for (int c = 0; c < 3; c++) o[c] = (unsigned char)resample_clip8(acc[c]);
+        continue;
+      }
       // the normalisation is per channel: take r from the red value's entry, g from the green one's, b from the blue one's
       if constexpr (F32)
         v = make_float4(s_norm[resample_clip8(acc[0])].x, s_norm[resample_clip8(acc[1])].y, s_norm[resample_clip8(acc[2])].z, 0.0f);
@@ -366,7 +373,8 @@ __global__ void __launch_bounds__(RS_TW * RS_ROWS, 3) preprocess_resize_u8_kerne
         v = make_uint2(__byte_perm(s_norm[resample_clip8(acc[0])].x, s_norm[resample_clip8(acc[1])].x, 0x7610),
                        s_norm[resample_clip8(acc[2])].y);
     }
-    if (xp < WP) y[((long long)n * HP + yp) * WP + xp] = v;
+    if constexpr (!U8)
+      if (xp < WP) y[((long long)n * HP + yp) * WP + xp] = v;
   }
 }
 
@@ -611,6 +619,32 @@ extern "C" long long odtk_preprocess_resize_u8_f32(const void *x, size_t x_bytes
                                                    const odtk_resize_image_t *images_dev, int n, int canvas_h, int canvas_w,
                                                    void *y, const float *mean, const float *std, odtk_stream_t stream_) {
   return preprocess_resize<true>(x, x_bytes, images, images_dev, n, canvas_h, canvas_w, y, mean, std, stream_);
+}
+
+extern "C" long long odtk_resize_u8_packed(const void *x, size_t x_bytes, const odtk_resize_image_t *images,
+                                           const odtk_resize_image_t *images_dev, const long long *out_off,
+                                           const long long *out_off_dev, int n, void *y, size_t y_bytes,
+                                           odtk_stream_t stream_) {
+  if (!images || !out_off || n <= 0 || n > 65535) return ODTK_E_INVALID;
+  long long packed = 0;
+  int max_h = 0, max_w = 0;
+  for (int i = 0; i < n; i++) {
+    const odtk_resize_image_t &im = images[i];
+    if (im.src_h <= 0 || im.src_w <= 0 || im.dst_h <= 0 || im.dst_w <= 0) return ODTK_E_INVALID;
+    if (im.offset < 0 || (unsigned long long)im.offset + (unsigned long long)im.src_h * im.src_w * 3 > x_bytes) return ODTK_E_INVALID;
+    const long long out = (long long)im.dst_h * im.dst_w * 3;
+    if (y && (out_off[i] < 0 || (unsigned long long)out_off[i] + (unsigned long long)out > y_bytes)) return ODTK_E_INVALID;
+    packed += out;
+    max_h = max(max_h, im.dst_h);
+    max_w = max(max_w, im.dst_w);
+  }
+  if (!y) return packed;
+  if (!x || !images_dev || !out_off_dev) return ODTK_E_INVALID;
+  const dim3 grid((max_w + RS_TW - 1) / RS_TW, (max_h + RS_TH - 1) / RS_TH, n);
+  OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+  preprocess_resize_u8_kernel<false, true><<<grid, RS_TW * RS_ROWS, 0, (cudaStream_t)stream_>>>(
+      (const unsigned char *)x, images_dev, (unsigned char *)y, 0, 0, 0.f, 0.f, 0.f, 1.f, 1.f, 1.f, out_off_dev);
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
 
 extern "C" int odtk_pad_input_f32(const void *x, void *y, int n, int h, int w, odtk_stream_t stream_) {

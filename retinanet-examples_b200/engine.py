@@ -520,6 +520,45 @@ def decode_jpeg(datas, device=None):
     return [y[t.offset:t.offset + h * w * 3].view(h, w, 3) for t, (h, w) in zip(outs, batch.shapes)], status
 
 
+def resize_u8_launch(x_dev, x_bytes, table, table_dev, out_off, out_off_dev, y):
+    """odtk_resize_u8_packed over already staged bytes: Pillow's uint8 BILINEAR result of image i, dst_h x dst_w x 3,
+    written at y[out_off[i]:] (y a uint8 CUDA tensor).  table: _lib.ResizeImage[n] (host) and table_dev its device copy;
+    out_off: host int64 tensor [n] and out_off_dev its device copy.  y=None returns the packed bytes the images need."""
+    L = _lib.lib()
+    off = ctypes.c_void_p(out_off.data_ptr())
+    if y is None:
+        return _lib.check(L.odtk_resize_u8_packed(None, x_bytes, ctypes.byref(table), None, off, None, len(table), None, 0,
+                                                  None), "resize_u8_packed")
+    _lib.check(L.odtk_resize_u8_packed(ctypes.c_void_p(x_dev.data_ptr()), x_bytes, ctypes.byref(table),
+                                       ctypes.c_void_p(table_dev.data_ptr()), off, ctypes.c_void_p(out_off_dev.data_ptr()),
+                                       len(table), ctypes.c_void_p(y.data_ptr()), y.numel(), _stream()), "resize_u8_packed")
+    STATS["launches"] += 1
+    return y
+
+
+def augment_launch(x, table, table_dev, canvas, out=None, workspace=None, mean=IMAGENET_MEAN, std=IMAGENET_STD):
+    """odtk_augment_u8: the rotation, flip, colour adjustments and normalisation of CocoDataset.__getitem__ on the uint8
+    images in x (uint8 CUDA tensor, each at table[i].offset), collated into fp32 [n, canvas_h, canvas_w, 3] (returned as
+    the [n, 3, canvas_h, canvas_w] channels_last view).  table: _lib.AugmentImage[n] (host); table_dev: its device copy."""
+    ch, cw = canvas
+    n = len(table)
+    L = _lib.lib()
+    need = _lib.check(L.odtk_augment_u8(None, x.numel(), ctypes.byref(table), None, n, ch, cw, None, 0, None, None, None,
+                                        None), "augment_u8")
+    if workspace is None or workspace.numel() < need:
+        workspace = torch.empty(need, dtype=torch.uint8, device=x.device)
+    if out is None:
+        out = torch.empty((n, ch, cw, 3), dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == (n, ch, cw, 3)
+    m = (ctypes.c_float * 3)(*mean)
+    s = (ctypes.c_float * 3)(*std)
+    _lib.check(L.odtk_augment_u8(ctypes.c_void_p(x.data_ptr()), x.numel(), ctypes.byref(table),
+                                 ctypes.c_void_p(table_dev.data_ptr()), n, ch, cw, ctypes.c_void_p(workspace.data_ptr()),
+                                 workspace.numel(), ctypes.c_void_p(out.data_ptr()), m, s, _stream()), "augment_u8")
+    STATS["launches"] += 2
+    return out.permute(0, 3, 1, 2)
+
+
 class _DevPtr:
     """A raw device address with the two tensor attributes resize_launch reads."""
 

@@ -279,16 +279,19 @@ class JpegBatch:
     and `blocks` (totals), `resize_off` (byte offset of the odtk_resize_image_t table in the staging buffer).
     ValueError names the image and the reason."""
 
-    def __init__(self, datas):
+    def __init__(self, datas, infos=None):
         if len(datas) == 0:
             raise ValueError("no images")
         self.datas = [d if isinstance(d, (bytes, bytearray)) else bytes(d) for d in datas]
-        self.infos = []
-        for i, d in enumerate(self.datas):
-            try:
-                self.infos.append(parse(d))
-            except ValueError as e:
-                raise ValueError("image %d: %s" % (i, e)) from None
+        if infos is not None:             # headers the caller already parsed with parse()
+            self.infos = list(infos)
+        else:
+            self.infos = []
+            for i, d in enumerate(self.datas):
+                try:
+                    self.infos.append(parse(d))
+                except ValueError as e:
+                    raise ValueError("image %d: %s" % (i, e)) from None
         n = self.n = len(self.datas)
         self.shapes = [(f.height, f.width) for f in self.infos]
         self.resize_off = _align(n * ctypes.sizeof(_lib.JpegImage), ALIGN)
