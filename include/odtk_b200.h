@@ -329,8 +329,13 @@ long long odtk_conv_wgrad(const odtk_wgrad_t *desc, void *workspace, size_t work
  *       the level's tiles and in the channels >= cout (the other levels' rows may hold anything)
  *   x   NHWC fp16 [n, x_h, x_width, cin], cin % 128 == 0; the level is (x_h - 1) / s + 1 rows from g_row0 by
  *       (x_width - 1) / s + 1 columns
- *   tile_tab / tab_tiles   the level's tiles of the atlas tile table of odtk_conv_t (a contiguous slice of it)
- * Any other (ksize, stride) returns ODTK_E_UNSUPPORTED.  Deterministic and with the workspace query of odtk_conv_wgrad. */
+ *   tile_tab / tab_tiles   the level's tiles of the atlas tile table of odtk_conv_t (a contiguous slice of it), or NULL:
+ *       g is the convolution's dense output [n, (x_h - 1) / s + 1, (x_width - 1) / s + 1, cout_pad] (g_rows / g_width those
+ *       sizes, g_row0 0; tab_tiles ignored).  1x1 stride 2 (a ResNet downsample) is accepted only so.
+ *   row_scale   fp32 [cout] or NULL: dw[co] is multiplied by row_scale[co] (a BatchNorm-folded weight w * gamma / sqrt(var +
+ *       eps) gives d/dw with row_scale = gamma / sqrt(var + eps)); db is not scaled
+ * cin and cout up to 2048 (ResNet stages 3-4).  Any other (ksize, stride) returns ODTK_E_UNSUPPORTED.  Deterministic and
+ * with the workspace query of odtk_conv_wgrad.                                                                        */
 typedef struct {
   const void *g;
   const void *x;
@@ -341,6 +346,7 @@ typedef struct {
   int ksize, stride;
   const void *tile_tab;
   int tab_tiles;
+  const float *row_scale;
 } odtk_wgrad_ex_t;
 long long odtk_conv_wgrad_ex(const odtk_wgrad_ex_t *desc, void *workspace, size_t workspace_size, odtk_stream_t stream);
 
@@ -351,11 +357,17 @@ long long odtk_conv_wgrad_ex(const odtk_wgrad_ex_t *desc, void *workspace, size_
  *                       fp16_rn((float)dst + ((s00 + s01) + (s10 + s11))); source pixels past the src level count as 0.
  *                       src == dst is allowed when the two levels' rows are disjoint.
  *   odtk_dilate_f16     dst[dst_row0 + 2y, 2x] = src[src_row0 + y, x] for the src_h x src_w level; nothing else of dst is
- *                       written, so a zeroed dst keeps zeros at the odd positions                                       */
+ *                       written, so a zeroed dst keeps zeros at the odd positions
+ *   odtk_dilate_ex_f16  the same into a destination of its own geometry [n, dst_rows, dst_width, c] with stride 1 or 2:
+ *                       dst[dst_row0 + s y, s x] = src[src_row0 + y, x] (src [n, src_rows, src_width, c]; src != dst).
+ *                       Stride 1 copies an atlas level into a dense tensor (the FPN's C4 / C5 input gradients); stride 2
+ *                       scatters a dense gradient into a stride-2 layer's input geometry for the stride-1 dgrad.       */
 int odtk_pool_add_f16(const void *src, void *dst, int n, int rows, int width, int c, int src_row0, int src_h, int src_w,
                       int dst_row0, int dst_h, int dst_w, int pool, odtk_stream_t stream);
 int odtk_dilate_f16(const void *src, void *dst, int n, int rows, int width, int c, int src_row0, int src_h, int src_w,
                     int dst_row0, odtk_stream_t stream);
+int odtk_dilate_ex_f16(const void *src, void *dst, int n, int c, int src_rows, int src_width, int src_row0, int src_h,
+                       int src_w, int dst_rows, int dst_width, int dst_row0, int stride, odtk_stream_t stream);
 
 /* Loss gradients -> fp16 gradient atlas: level l's fp32 NCHW gradient [batch, channels, height, width] times *scale (a
  * DEVICE fp32 scalar, NULL for 1: the upstream autograd factor, e.g. a GradScaler scale, read without a host sync) lands at rows [row0, row0 + height) x columns [0, width) of the NHWC
@@ -373,7 +385,10 @@ int odtk_grad_to_atlas(int batch, int num_levels, const odtk_grad_level_t *level
  * the output gradient g, w = the weights rotated by 180 degrees with cin / cout swapped, out_mode ODTK_OUT_NHWC_F16, no
  * bias, no ReLU; residual adds a second gradient, e.g. the other head tower's), then every output element whose `mask`
  * element is not > 0 becomes 0.  mask: NHWC fp16 [n, h, width, cout] (the layer input saved by the forward pass; the
- * tile table's geometry when base.tile_tab is set), or NULL for no mask.  fp16 overflow gives +-inf.                  */
+ * tile table's geometry when base.tile_tab is set), or NULL for no mask.  fp16 overflow gives +-inf.
+ * base.ksize 1: the same for a 1x1 convolution (w = the transposed weights [cout, cin]) over dense tensors, with a mask
+ * and cout % 128 == 0 (the input channels of a layer whose weight gradient odtk_conv_wgrad_ex takes).  Stride-2 layers:
+ * scatter g with odtk_dilate_ex_f16 into the input geometry, then the stride-1 call.                                  */
 typedef struct {
   odtk_conv_t base;
   const void *mask;

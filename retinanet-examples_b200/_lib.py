@@ -60,6 +60,7 @@ SIGNATURES = {
     "odtk_conv_wgrad_ex": (ctypes.c_longlong, [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_size_t, ctypes.c_void_p]),
     "odtk_pool_add_f16": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 11 + [ctypes.c_void_p]),
     "odtk_dilate_f16": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 8 + [ctypes.c_void_p]),
+    "odtk_dilate_ex_f16": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p] + [ctypes.c_int] * 11 + [ctypes.c_void_p]),
     "odtk_grad_to_atlas": (ctypes.c_int, [ctypes.c_int, ctypes.c_int, ctypes.c_void_p, ctypes.c_int, ctypes.c_void_p,
                                           ctypes.c_void_p, ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_void_p]),
     "odtk_conv2d_dgrad": (ctypes.c_int, [ctypes.c_void_p, ctypes.c_void_p]),

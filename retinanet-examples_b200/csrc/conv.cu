@@ -906,8 +906,8 @@ constexpr OpSpec kSpecF32 = {kOpTF32x3, 4, ODTK_OUT_NHWC_F32, 2, 2, 8, false};
 
 // The fields of odtk_conv_t, odtk_conv_s8_ex_t and odtk_conv_f32_t in one place, plus the fp16-only extras: a second
 // operand pair (mode 0) added to the same accumulator, y = x * w^T + x2 * w2^T with x2 [M, c2in], w2 [cout, c2in] (the
-// projected identity of a bottleneck block), and the input-gradient launch (odtk_conv2d_dgrad: the masked instance; a
-// tile-table launch may then take a residual, a whole atlas like y).
+// projected identity of a bottleneck block), and the input-gradient launch (odtk_conv2d_dgrad: the masked instance, 3x3 or
+// dense 1x1; a tile-table launch may then take a residual, a whole atlas like y).
 struct ConvArgs {
   const void *x, *w, *w_lo, *residual, *upsample, *x2, *w2, *mask, *tile_tab;
   const float *bias, *alpha;
@@ -925,8 +925,11 @@ struct ConvArgs {
 // or a nearest-upsampled addend, and may land in a level view of an atlas.  Every argument is checked before any CUDA call.
 int conv_run(const ConvArgs &a, const OpSpec &s, cudaStream_t stream) {
   if (!a.x || !a.w || (s.op == kOpS8 && !a.alpha) || (s.op == kOpTF32x3 && !a.w_lo)) return ODTK_E_INVALID;
-  if (a.dgrad && (a.ksize != 3 || a.stride > 1 || a.out_mode != ODTK_OUT_NHWC_F16 || a.relu || a.groups > 1 || a.upsample ||
-                  a.x_rows > 0 || a.x_width > 0 || a.y_rows > 0 || a.y_width > 0 || a.y_row_off > 0))
+  // dgrad: 3x3, or 1x1 (mode 0, dense) masked, into the input channels of a layer odtk_conv_wgrad_ex takes
+  const bool dgrad_1x1 = a.ksize == 1 && a.mask && a.cout % 128 == 0 && !a.tile_tab;
+  if (a.dgrad && ((a.ksize != 3 && !dgrad_1x1) || a.stride > 1 || a.out_mode != ODTK_OUT_NHWC_F16 || a.relu ||
+                  a.groups > 1 || a.upsample || a.x_rows > 0 || a.x_width > 0 || a.y_rows > 0 || a.y_width > 0 ||
+                  a.y_row_off > 0))
     return ODTK_E_UNSUPPORTED;
   if (a.mask && ((uintptr_t)a.mask & 3)) return ODTK_E_INVALID;
   if (a.out_mode == ODTK_OUT_CANDIDATES ? !a.sink : !a.y) return ODTK_E_INVALID;

@@ -1,5 +1,6 @@
-// wgrad.cu -- backward of the head and FPN convolutions (sm_90a): the weight-gradient GEMM over the gradient atlas, the
-// bias gradient, the packing of the loss gradients into the fp16 gradient atlas, and the FPN's top-down pathway backward.
+// wgrad.cu -- backward of the head, FPN and ResNet stage 3-4 convolutions (sm_90a): the weight-gradient GEMM over the
+// gradient atlas or a dense gradient, the bias gradient, the packing of the loss gradients into the fp16 gradient atlas,
+// the FPN's top-down pathway backward and the scatter of a gradient into a strided layer's input geometry.
 // The input gradient runs on conv_gemm_kernel (odtk_conv2d_dgrad, conv.cu).
 //
 //   dW[co, tap, ci] = sum over images and pixels (r, c) of  G[r, c, co] * X[s * (r - g_row0) + ky - p, s * c + kx - p, ci]
@@ -14,15 +15,19 @@
 //                   dimension of the NHWC boxes): 128B-swizzled MN-major descriptors + the transpose immediates.
 // Each CTA writes its fp32 partial tile; one reduce kernel sums the partials in split order and writes the [Cout, Cin, k, k]
 // parameter layout, so the result is bit-identical run to run.  The bias gradient is a fixed-order column sum of G's level.
+// A backbone convolution runs BatchNorm-folded (w' = w * gamma / sqrt(var + eps) per output channel); the reduce kernel's
+// optional per-row scale turns d/dw' into d/dw without another pass over dw.
 //
 // Both entry points run the same launch routine:
 //   odtk_conv_wgrad     (head layers) 3x3 stride 1: G and X are whole atlases of one geometry (g_row0 0) and the tile table
 //                       lists every level's tiles, or both are dense tensors; the atlas's zero gap rows / columns and the
 //                       hardware zero fill are the padding, exactly as in the forward pass.
-//   odtk_conv_wgrad_ex  (FPN layers) 1x1, 3x3 stride 1 or 3x3 stride 2: G is one level of the gradient atlas (the level's
-//                       slice of the tile table, first row g_row0), X a dense tensor.  G is zero outside the level (gap
-//                       rows, columns right of a narrow level), so the in-bounds X values under it contribute nothing; the
-//                       hardware zero fill outside X is the padding.
+//   odtk_conv_wgrad_ex  (FPN and backbone layers) 1x1, 3x3 stride 1 or 3x3 stride 2: G is one level of the gradient atlas
+//                       (the level's slice of the tile table, first row g_row0), X a dense tensor.  G is zero outside the
+//                       level (gap rows, columns right of a narrow level), so the in-bounds X values under it contribute
+//                       nothing; the hardware zero fill outside X is the padding.  Without a tile table G is the dense
+//                       output itself (the dense 8 x 16 tiles, g_row0 0; the TMA zero fill past its edge), which also
+//                       admits 1x1 stride 2 (the ResNet downsample).  Up to 2048 channels on either side.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <string.h>
@@ -182,10 +187,12 @@ __global__ void bgrad_level_partial_kernel(const __half *g, long long px, long l
   }
 }
 
-// dw[co, ci, tap] = sum over splits (in order) of ws[split, co, tap * cin + ci]; db[co] = sum over blocks of part[b, co]
-template <int kTaps>
+// dw[co, ci, tap] = sum over splits (in order) of ws[split, co, tap * cin + ci] (kScale: times row_scale[co], one rounding
+// after the sum); db[co] = sum over blocks of part[b, co].  row_scale comes last so that the unscaled instances keep their
+// parameter offsets.
+template <int kTaps, bool kScale>
 __global__ void wgrad_reduce_kernel(const float *ws, int splits, int cout, int cout_pad, int cin, float *dw,
-                                    const float *part, int nparts, float *db) {
+                                    const float *part, int nparts, float *db, const float *row_scale) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long N = (long long)kTaps * cin;
   if (i < (long long)cout * cin) {
@@ -194,6 +201,7 @@ __global__ void wgrad_reduce_kernel(const float *ws, int splits, int cout, int c
       const float *src = ws + (long long)co * N + (long long)t * cin + ci;
       float s = 0.0f;
       for (int k = 0; k < splits; k++) s += src[(long long)k * cout_pad * N];
+      if constexpr (kScale) s *= __ldg(row_scale + co);
       dw[i * kTaps + t] = s;
     }
   }
@@ -333,10 +341,9 @@ long long wgrad_run(const odtk_wgrad_ex_t &d, void *workspace, size_t workspace_
           (long long)lh * d.g_width, (long long)d.g_rows * d.g_width * d.cout_pad, d.cout_pad, part);
     const long long elems = (long long)d.cout * d.cin;
     const unsigned blocks = (unsigned)((elems + 255) / 256);
-    if (taps == 1)
-      wgrad_reduce_kernel<1><<<blocks, 256, 0, stream>>>(p.ws, splits, d.cout, d.cout_pad, d.cin, d.dw, part, kBiasBlocks, d.db);
-    else
-      wgrad_reduce_kernel<9><<<blocks, 256, 0, stream>>>(p.ws, splits, d.cout, d.cout_pad, d.cin, d.dw, part, kBiasBlocks, d.db);
+    auto reduce = taps == 1 ? (d.row_scale ? wgrad_reduce_kernel<1, true> : wgrad_reduce_kernel<1, false>)
+                            : (d.row_scale ? wgrad_reduce_kernel<9, true> : wgrad_reduce_kernel<9, false>);
+    reduce<<<blocks, 256, 0, stream>>>(p.ws, splits, d.cout, d.cout_pad, d.cin, d.dw, part, kBiasBlocks, d.db, d.row_scale);
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }
@@ -394,23 +401,30 @@ extern "C" int odtk_grad_to_atlas(int batch, int num_levels, const odtk_grad_lev
 }
 
 extern "C" long long odtk_conv_wgrad_ex(const odtk_wgrad_ex_t *d, void *workspace, size_t workspace_size, odtk_stream_t stream_) {
-  if (!d || !d->g || !d->x || !d->dw || !d->tile_tab) return ODTK_E_INVALID;
-  const bool mode_ok = (d->ksize == 1 && d->stride == 1) || (d->ksize == 3 && (d->stride == 1 || d->stride == 2));
+  if (!d || !d->g || !d->x || !d->dw) return ODTK_E_INVALID;
+  const bool dense = !d->tile_tab;   // G is the convolution's whole dense output
+  // 1x1 stride 2 (the ResNet downsample) only over a dense G: no FPN layer has that shape
+  const bool mode_ok = (d->ksize == 1 && d->stride == 1) || (d->ksize == 3 && (d->stride == 1 || d->stride == 2)) ||
+                       (d->ksize == 1 && d->stride == 2 && dense);
+  if (dense && d->g_row0 != 0) return ODTK_E_INVALID;
   if (!mode_ok) return ODTK_E_UNSUPPORTED;
   if (d->n <= 0 || d->g_rows <= 0 || d->g_width <= 0 || d->g_row0 < 0 || d->x_h <= 0 || d->x_width <= 0 || d->cin <= 0 ||
-      d->cout <= 0 || d->cout_pad <= 0 || d->tab_tiles <= 0)
+      d->cout <= 0 || d->cout_pad <= 0 || (!dense && d->tab_tiles <= 0))
     return ODTK_E_INVALID;
   if (d->cout > d->cout_pad) return ODTK_E_INVALID;
   if (d->cin % 128 || d->cout_pad % 64) return ODTK_E_UNSUPPORTED;   // 128-wide N tiles inside one tap; 64-channel G boxes
-  // the level is the convolution's output: (x - 1) / s + 1 rows and columns from row g_row0 of the atlas
+  // the level is the convolution's output: (x - 1) / s + 1 rows and columns from row g_row0 of the atlas (dense: all of G)
   const int lh = (d->x_h - 1) / d->stride + 1, lw = (d->x_width - 1) / d->stride + 1;
   if ((long long)d->g_row0 + lh > d->g_rows || lw > d->g_width) return ODTK_E_INVALID;
+  if (dense && (lh != d->g_rows || lw != d->g_width)) return ODTK_E_INVALID;
   if ((long long)d->n * d->g_rows * d->g_width >= (1ll << 31) || (long long)d->n * d->x_h * d->x_width >= (1ll << 31))
     return ODTK_E_UNSUPPORTED;
-  if (((uintptr_t)d->g | (uintptr_t)d->x | (uintptr_t)d->tile_tab) & 15) return ODTK_E_INVALID;
-  const long long ktiles = (long long)d->n * d->tab_tiles;
+  if ((((uintptr_t)d->g | (uintptr_t)d->x | (uintptr_t)d->tile_tab) & 15) || ((uintptr_t)d->row_scale & 3)) return ODTK_E_INVALID;
+  odtk_wgrad_ex_t e = *d;
+  if (dense) e.tab_tiles = ((lh + 7) / 8) * ((lw + 15) / 16);   // wgrad_run's dense 8 x 16 tiles
+  const long long ktiles = (long long)e.n * e.tab_tiles;
   if (ktiles >= (1ll << 31)) return ODTK_E_UNSUPPORTED;
-  return wgrad_run(*d, workspace, workspace_size, stream_);
+  return wgrad_run(e, workspace, workspace_size, stream_);
 }
 
 // ---- the FPN's top-down pathway and pyramid7's input gradient: two small HBM-bound kernels over fp16 NHWC atlases -------
@@ -455,8 +469,12 @@ __global__ void pool_add_kernel(const __half *src, __half *dst, int n, int rows,
   *reinterpret_cast<uint4 *>(o) = v;
 }
 
-// dst[dr0 + 2y, 2x] = src[sr0 + y, x] over the h x w source level; nothing else of dst is written
-__global__ void dilate_kernel(const __half *src, __half *dst, int n, int rows, int width, int c8, int sr0, int h, int w, int dr0) {
+// dst[dr0 + s y, s x] = src[sr0 + y, x] over the h x w source level; nothing else of dst is written.  kGeom false: dst has
+// the source's geometry and s = 2 (the FPN's P7 -> P6 scatter); true: dst is [n, d_rows, d_width, c] and s is 1 or 2 (an
+// atlas level into a dense tensor, a dense gradient into the even positions of a strided layer's input).
+template <bool kGeom>
+__global__ void dilate_kernel(const __half *src, __half *dst, int n, int rows, int width, int c8, int sr0, int h, int w, int dr0,
+                              int d_rows, int d_width, int s) {
   const long long total = (long long)n * h * w * c8;
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
@@ -465,9 +483,15 @@ __global__ void dilate_kernel(const __half *src, __half *dst, int n, int rows, i
   const int x = (int)(t % w);
   t /= w;
   const int y = (int)(t % h);
-  const long long img0 = (t / h) * rows;
-  *reinterpret_cast<uint4 *>(dst + (((img0 + dr0 + 2 * y) * width + 2 * x) * c8 + ch) * 8) =
-      *reinterpret_cast<const uint4 *>(src + (((img0 + sr0 + y) * width + x) * c8 + ch) * 8);
+  if constexpr (kGeom) {
+    const long long img = t / h;
+    *reinterpret_cast<uint4 *>(dst + (((img * d_rows + dr0 + s * y) * d_width + s * x) * c8 + ch) * 8) =
+        *reinterpret_cast<const uint4 *>(src + (((img * rows + sr0 + y) * width + x) * c8 + ch) * 8);
+  } else {
+    const long long img0 = (t / h) * rows;
+    *reinterpret_cast<uint4 *>(dst + (((img0 + dr0 + 2 * y) * width + 2 * x) * c8 + ch) * 8) =
+        *reinterpret_cast<const uint4 *>(src + (((img0 + sr0 + y) * width + x) * c8 + ch) * 8);
+  }
 }
 
 }  // namespace
@@ -503,8 +527,32 @@ extern "C" int odtk_dilate_f16(const void *src, void *dst, int n, int rows, int 
   if ((long long)n * rows * width * c >= (1ll << 40)) return ODTK_E_UNSUPPORTED;
   {
     OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
-    dilate_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(
-        (const __half *)src, (__half *)dst, n, rows, width, c / 8, src_row0, src_h, src_w, dst_row0);
+    dilate_kernel<false><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(
+        (const __half *)src, (__half *)dst, n, rows, width, c / 8, src_row0, src_h, src_w, dst_row0, 0, 0, 2);
+  }
+  return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
+}
+
+extern "C" int odtk_dilate_ex_f16(const void *src, void *dst, int n, int c, int src_rows, int src_width, int src_row0,
+                                  int src_h, int src_w, int dst_rows, int dst_width, int dst_row0, int stride,
+                                  odtk_stream_t stream_) {
+  if (!src || !dst || n <= 0 || c <= 0 || (c % 8) || src_rows <= 0 || src_width <= 0 || dst_rows <= 0 || dst_width <= 0)
+    return ODTK_E_INVALID;
+  if (stride != 1 && stride != 2) return ODTK_E_UNSUPPORTED;
+  if (src_row0 < 0 || src_h <= 0 || src_w <= 0 || dst_row0 < 0) return ODTK_E_INVALID;
+  if ((long long)src_row0 + src_h > src_rows || src_w > src_width || (long long)stride * (src_w - 1) >= dst_width ||
+      (long long)dst_row0 + (long long)stride * (src_h - 1) >= dst_rows)
+    return ODTK_E_INVALID;
+  if (src == dst) return ODTK_E_INVALID;
+  if (((uintptr_t)src | (uintptr_t)dst) & 15) return ODTK_E_INVALID;
+  const long long total = (long long)n * src_h * src_w * (c / 8);
+  if ((long long)n * src_rows * src_width * c >= (1ll << 40) || (long long)n * dst_rows * dst_width * c >= (1ll << 40))
+    return ODTK_E_UNSUPPORTED;
+  {
+    OdtkProfScope prof(ODTK_PROF_LAYER, (cudaStream_t)stream_);
+    dilate_kernel<true><<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream_>>>(
+        (const __half *)src, (__half *)dst, n, src_rows, src_width, c / 8, src_row0, src_h, src_w, dst_row0, dst_rows,
+        dst_width, stride);
   }
   return cudaGetLastError() == cudaSuccess ? ODTK_OK : ODTK_E_CUDA;
 }

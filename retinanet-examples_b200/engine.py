@@ -73,8 +73,14 @@ def last_plan():
 def fold_bn(weight, bn_weight, bn_bias, running_mean, running_var, eps=1e-5):
     """conv (no bias) followed by eval-mode BatchNorm == conv with scaled weights + a bias
     (torchvision BasicBlock/Bottleneck, odtk/backbones/layers.py:5-15).  fp32 in, fp32 out."""
+    scale, bias = bn_affine(bn_weight, bn_bias, running_mean, running_var, eps)
+    return weight.float() * scale.view(-1, 1, 1, 1), bias
+
+
+def bn_affine(bn_weight, bn_bias, running_mean, running_var, eps=1e-5):
+    """Eval-mode BatchNorm as y = x * scale + bias per channel (fp32): the factor fold_bn scales the weights by."""
     scale = bn_weight.float() / torch.sqrt(running_var.float() + eps)
-    return weight.float() * scale.view(-1, 1, 1, 1), bn_bias.float() - running_mean.float() * scale
+    return scale, bn_bias.float() - running_mean.float() * scale
 
 
 def pack_weight(weight, kpad=None):
@@ -851,11 +857,11 @@ def _tab_px(n, h, w, tile_tab):
 
 
 def pack_weight_dgrad(weight, cout_pad=None):
-    """Weights of the input gradient of a 3x3 stride-1 convolution: [Cout, Cin, 3, 3] -> the forward convolution with Cin
-    outputs over Cout_pad inputs (pad_out zero-padded to a multiple of 64), rotated by 180 degrees:
-    w'[ci, co, ky, kx] = w[co, ci, 2 - ky, 2 - kx], packed like pack_weight ([Cin, 9 * Cout_pad] fp16)."""
+    """Weights of the input gradient of a 3x3 (or 1x1) stride-1 convolution: [Cout, Cin, k, k] -> the forward convolution
+    with Cin outputs over Cout_pad inputs (pad_out zero-padded to a multiple of 64), rotated by 180 degrees:
+    w'[ci, co, ky, kx] = w[co, ci, k - 1 - ky, k - 1 - kx], packed like pack_weight ([Cin, k * k * Cout_pad] fp16)."""
     cout, cin, kh, kw = weight.shape
-    assert kh == 3 and kw == 3
+    assert kh == kw and kh in (1, 3)
     cout_pad = pad64(cout) if cout_pad is None else cout_pad
     w = weight.detach().float()
     if cout_pad > cout:
@@ -906,25 +912,31 @@ class WgradExDesc(ctypes.Structure):
     _fields_ = [("g", ctypes.c_void_p), ("x", ctypes.c_void_p), ("dw", ctypes.c_void_p), ("db", ctypes.c_void_p)] + \
                [(f, ctypes.c_int) for f in ("n", "g_rows", "g_width", "g_row0", "cout_pad", "x_h", "x_width", "cin", "cout",
                                             "ksize", "stride")] + \
-               [("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int)]
+               [("tile_tab", ctypes.c_void_p), ("tab_tiles", ctypes.c_int), ("row_scale", ctypes.c_void_p)]
 
 
-def conv_wgrad_ex(g, x, cout, ksize, stride, tile_tab, g_row0, bias=True):
-    """Weight (and bias) gradient of an FPN convolution (odtk_conv_wgrad_ex): 1x1 stride 1, 3x3 stride 1 or 3x3 stride 2
-    (pad ksize // 2).  g: the NHWC fp16 gradient atlas [N, rows, width, Cout_pad] whose level at row g_row0 is the
-    convolution's output ((H - 1) // stride + 1 rows and columns; zero in its tiles outside the level and in the channels
-    >= cout), tile_tab: that level's slice of the atlas tile table, x: the dense NHWC fp16 input [N, H, W, Cin].  Returns
+def conv_wgrad_ex(g, x, cout, ksize, stride, tile_tab, g_row0, bias=True, row_scale=None):
+    """Weight (and bias) gradient of an FPN or backbone convolution (odtk_conv_wgrad_ex): 1x1 stride 1, 3x3 stride 1 or 3x3
+    stride 2 (pad ksize // 2), and with a dense g 1x1 stride 2.  g: the NHWC fp16 gradient atlas [N, rows, width,
+    Cout_pad] whose level at row g_row0 is the convolution's output ((H - 1) // stride + 1 rows and columns; zero in its
+    tiles outside the level and in the channels >= cout), tile_tab: that level's slice of the atlas tile table; or, with
+    tile_tab None (g_row0 0), g is that dense output itself.  x: the dense NHWC fp16 input [N, H, W, Cin].  row_scale:
+    fp32 [cout] on the device or None, multiplies dw's rows (d/dw of a BatchNorm-folded weight w * row_scale).  Returns
     fp32 (dw [cout, Cin, k, k], db [cout] or None: the level's rows only), bit-identical run to run."""
     assert g.is_cuda and g.dtype == torch.float16 and g.is_contiguous()
     assert x.is_cuda and x.dtype == torch.float16 and x.is_contiguous() and x.device == g.device
-    assert tile_tab is not None and tile_tab.is_contiguous() and tile_tab.device == g.device
+    assert tile_tab is None or (tile_tab.is_contiguous() and tile_tab.device == g.device)
+    assert row_scale is None or (row_scale.device == g.device and row_scale.dtype == torch.float32 and
+                                 row_scale.is_contiguous() and row_scale.numel() == cout)
     n, rows, aw, cpad = g.shape
     xn, xh, xw, cin = x.shape
     assert xn == n
     d = WgradExDesc()
     d.n, d.g_rows, d.g_width, d.g_row0, d.cout_pad = n, rows, aw, int(g_row0), cpad
     d.x_h, d.x_width, d.cin, d.cout, d.ksize, d.stride = xh, xw, cin, cout, ksize, stride
-    d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    if tile_tab is not None:
+        d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
+    d.row_scale = row_scale.data_ptr() if row_scale is not None else None
     dw, db, size = _wgrad_launch("conv_wgrad_ex", d, g, x, cout, ksize, bias)
     if STATS["trace"] is not None:
         px = n * ((xh - 1) // stride + 1) * ((xw - 1) // stride + 1)
@@ -973,6 +985,23 @@ def dilate(src, dst, src_level, dst_row0):
     return dst
 
 
+def dilate_into(src, src_level, dst, stride, dst_row0=0):
+    """dst[:, dst_row0 + s y, s x] = src level (row0, h, w) [y, x] (odtk_dilate_ex_f16): NHWC fp16 tensors of their own
+    geometries (a dense tensor is one level at row 0).  Stride 1 copies an atlas level into a dense tensor; stride 2
+    scatters a gradient into a stride-2 layer's input geometry (a zeroed dst keeps zeros at the odd positions)."""
+    for t in (src, dst):
+        assert t.is_cuda and t.dtype == torch.float16 and t.is_contiguous()
+    n, rows, aw, c = src.shape
+    assert dst.shape[0] == n and dst.shape[3] == c and dst.device == src.device
+    args = [n, c, rows, aw] + [int(v) for v in src_level] + [dst.shape[1], dst.shape[2], int(dst_row0), int(stride)]
+    _lib.check(_lib.lib().odtk_dilate_ex_f16(ctypes.c_void_p(src.data_ptr()), ctypes.c_void_p(dst.data_ptr()), *args,
+                                             _stream()), "dilate_ex_f16")
+    STATS["launches"] += 1
+    px = n * int(src_level[1]) * int(src_level[2])
+    _trace("dilate", 0, px * c * 4, n=n, h=int(src_level[1]), w=int(src_level[2]), cin=c, cout=c, stride=int(stride))
+    return dst
+
+
 def grad_to_atlas(grads, rows0, scale, atlas):
     """Per-level fp32 NCHW loss gradients [B, C, H_l, W_l] * scale (a number, or a one-element fp32 tensor on the atlas's
     device, read there without a host sync) -> the fp16 NHWC gradient atlas [B, rows, width, C_pad]
@@ -997,12 +1026,14 @@ def grad_to_atlas(grads, rows0, scale, atlas):
 
 
 def conv2d_dgrad(g, w, cout, mask=None, residual=None, tile_tab=None, out=None):
-    """Input gradient of a 3x3 stride-1 convolution (odtk_conv2d_dgrad): g NHWC fp16 [N, H, W, Cout_pad] convolved with
-    w = pack_weight_dgrad(weight) into NHWC fp16 [N, H, W, cout] (cout = the forward layer's Cin), + residual (same shape),
-    then zero wherever mask (NHWC fp16, same shape: the forward layer's input) is not > 0.  tile_tab: whole atlases, only
-    the listed tiles are written (`out` must then be zero outside them)."""
+    """Input gradient of a 3x3 or 1x1 stride-1 convolution (odtk_conv2d_dgrad): g NHWC fp16 [N, H, W, Cout_pad] convolved
+    with w = pack_weight_dgrad(weight) into NHWC fp16 [N, H, W, cout] (cout = the forward layer's Cin), + residual (same
+    shape), then zero wherever mask (NHWC fp16, same shape: the forward layer's input) is not > 0.  tile_tab: whole
+    atlases (3x3), only the listed tiles are written (`out` must then be zero outside them).  1x1 (w [cout, Cout_pad]):
+    dense, with a mask, cout % 128 == 0.  A stride-2 layer's input gradient is this call on g scattered by dilate_into."""
     assert g.is_cuda and g.dtype == torch.float16 and g.is_contiguous()
-    assert w.device == g.device and w.dtype == torch.float16 and w.is_contiguous() and w.shape[1] == 9 * g.shape[3]
+    ksize = 3 if w.shape[1] == 9 * g.shape[3] else 1
+    assert w.device == g.device and w.dtype == torch.float16 and w.is_contiguous() and w.shape[1] == ksize * ksize * g.shape[3]
     n, h, wd, cpad = g.shape
     if out is None:
         out = (torch.zeros if tile_tab is not None else torch.empty)((n, h, wd, cout), dtype=torch.float16, device=g.device)
@@ -1014,14 +1045,14 @@ def conv2d_dgrad(g, w, cout, mask=None, residual=None, tile_tab=None, out=None):
     d.residual = residual.data_ptr() if residual is not None else None
     if tile_tab is not None:
         d.tile_tab, d.tab_tiles = tile_tab.data_ptr(), tile_tab.shape[0]
-    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cpad, cout, 3
+    d.n, d.h, d.width, d.cin, d.cout, d.ksize = n, h, wd, cpad, cout, ksize
     d.out_mode = OUT_NHWC_F16
     e.mask = mask.data_ptr() if mask is not None else None
     _lib.check(_lib.lib().odtk_conv2d_dgrad(ctypes.byref(e), _stream()), "conv2d_dgrad")
     STATS["launches"] += 1
     if STATS["trace"] is not None:
         px = _tab_px(n, h, wd, tile_tab)
-        _trace("dgrad3x3", 2 * px * cout * 9 * cpad,
+        _trace("dgrad%dx%d" % (ksize, ksize), 2 * px * cout * ksize * ksize * cpad,
                px * cpad * 2 + w.numel() * 2 + px * cout * 2 * (1 + (mask is not None) + (residual is not None)),
                n=n, h=h, w=wd, cin=cpad, cout=cout, residual=residual is not None, mask=mask is not None)
     return out

@@ -300,6 +300,9 @@ class _ConvF32:
 
 
 FPN_LAYERS = ("lateral3", "lateral4", "lateral5", "pyramid6", "pyramid7", "smooth3", "smooth4", "smooth5")   # fpn.py:26-33
+# backbone training scopes -> the ResNet levels they train (network_walk's block "level": layer3 is 4 (C4), layer4 is 5)
+BACKBONE_SCOPES = {"layer4": (5,), "layer3": (4, 5)}
+TRAIN_SCOPES = ("heads", "fpn") + tuple(BACKBONE_SCOPES)
 
 
 class _HeadsTrain(torch.autograd.Function):
@@ -370,8 +373,10 @@ class Model:
         self._f32 = None              # full precision: split-TF32 weights of every layer (packed on first use)
         self._params = None           # trainable parameters by name (created by named_parameters / parameters)
         self._walk = network_walk(backbones)   # read by every training forward (_trainable_layers)
-        self.train_scope = "heads"    # "heads" or "fpn": which parameters named_parameters lists (set_train_scope)
+        self.train_scope = "heads"    # one of TRAIN_SCOPES: which parameters named_parameters lists (set_train_scope)
         self._param_versions = {}     # weight name -> the layer's (weight, bias) _version when its fp16 weights were packed
+        self._bn_fold = {}            # BatchNorm prefix -> (scale on the device, bias): a trained backbone weight's fold
+        self._bwd_zeros = {}          # (shape, device) -> zeroed fp16 buffer of the backbone backward's stride-2 scatters
         self._sd_versions = {}        # parameter name -> its _version when it was last copied into the state dict
         self._dgrad_w = {}            # weight name -> ((_version, id), pack_weight_dgrad weights)
         self._fwd_gen = 0             # counts forward passes: a backward must follow its own forward
@@ -441,6 +446,7 @@ class Model:
         self._sd = {k: v.detach().float().cpu() for k, v in sd.items() if torch.is_tensor(v)}
         self._packed = None
         self._f32 = None
+        self._bn_fold = {}
         if self._params is not None:       # as nn.Module: the existing parameter tensors take the new values in place
             with torch.no_grad():
                 for n, p in self._params.items():
@@ -456,42 +462,80 @@ class Model:
     def _fpn_param_names(self):
         return ["backbones.%s.%s.%s" % (self.backbone, l, k) for l in FPN_LAYERS for k in ("weight", "bias")]
 
+    def _backbone_blocks(self, scope=None):
+        """(index in network_walk's blocks, block) of the residual blocks the training scope trains, in forward order."""
+        levels = BACKBONE_SCOPES.get(self.train_scope if scope is None else scope, ())
+        return [(i, b) for i, b in enumerate(self._walk.get("blocks", ())) if b["level"] in levels]
+
+    @staticmethod
+    def _block_convs(blk):
+        """A block's convolutions in the reference's named_parameters() order: conv1, conv2(, conv3), downsample.0."""
+        return blk["convs"] + ([blk["down"]] if blk["down"] else [])
+
+    def _backbone_param_names(self):
+        return [c["conv"] + ".weight" for _, b in self._backbone_blocks() for c in self._block_convs(b)]
+
     def _param_names(self):
-        """The training scope's parameter names in the reference's named_parameters() order: the FPN's before the heads'."""
-        return (self._fpn_param_names() if self.train_scope == "fpn" else []) + self._head_param_names()
+        """The training scope's parameter names in the reference's named_parameters() order: the backbone stages' conv
+        weights, then the FPN's, then the heads'."""
+        fpn = self._fpn_param_names() if self.train_scope != "heads" else []
+        return self._backbone_param_names() + fpn + self._head_param_names()
 
     def _trainable_layers(self):
-        """(packed-layer key, index in a head list or None, stride, weight name, bias name) of every layer whose
-        parameters exist, the FPN's before the heads'."""
+        """(path into the packed layer set, network_walk convolution) of every layer whose parameters exist: the backbone
+        stages' (path ("blocks", i, "convs", k) or ("blocks", i, "down")), the FPN's, then the heads' (path (head, k))."""
         walk = self._walk
-        layers = [(l, None, walk[l]) for l in FPN_LAYERS if l in walk]
-        layers += [(head, k, c) for head in calib.HEADS for k, c in enumerate(walk[head])]
-        return [(key, k, c["stride"], c["conv"] + ".weight", c["conv"] + ".bias") for key, k, c in layers
-                if self._params is not None and c["conv"] + ".weight" in self._params]
+        layers = [(("blocks", i, "convs", k), c) for i, b in enumerate(walk.get("blocks", ())) for k, c in enumerate(b["convs"])]
+        layers += [(("blocks", i, "down"), b["down"]) for i, b in enumerate(walk.get("blocks", ())) if b["down"]]
+        layers += [((l,), walk[l]) for l in FPN_LAYERS if l in walk]
+        layers += [((head, k), c) for head in calib.HEADS for k, c in enumerate(walk[head])]
+        return [(path, c) for path, c in layers if self._params is not None and c["conv"] + ".weight" in self._params]
+
+    def _layer_params(self, c):
+        """(weight, bias or None) parameters of a convolution of network_walk: a BatchNorm-folded one has no bias."""
+        w = self._params[c["conv"] + ".weight"]
+        return w, (self._params[c["conv"] + ".bias"] if c["bn"] is None else None)
+
+    def _bn_scale_bias(self, c):
+        """(gamma / sqrt(var + eps) on the device, the folded bias) of a backbone convolution's frozen BatchNorm."""
+        f = self._bn_fold.get(c["bn"])
+        if f is None:
+            sd, bn = self._sd, c["bn"]
+            scale, bias = engine.bn_affine(sd[bn + ".weight"], sd[bn + ".bias"], sd[bn + ".running_mean"],
+                                           sd[bn + ".running_var"])
+            f = self._bn_fold[c["bn"]] = (scale.to(self.device), bias)
+        return f
 
     def set_train_scope(self, scope):
-        """What training updates: "heads" (default: the class and box heads, the backbone and the FPN frozen) or "fpn"
-        (the FPN's 16 tensors as well; ResNet18/34/50/101/152 and ResNeXt FPNs -- not MobileNetV2FPN, whose 64-channel
-        padded C3 does not fit the weight-gradient GEMM's 128-channel tiles).  named_parameters / parameters list the
-        scope's tensors, so build the optimizer after this call.  A parameter keeps its identity across scope changes.
+        """What training updates: "heads" (default: the class and box heads, the backbone and the FPN frozen), "fpn" (the
+        FPN's 16 tensors as well; ResNet18/34/50/101/152 and ResNeXt FPNs -- not MobileNetV2FPN, whose 64-channel padded
+        C3 does not fit the weight-gradient GEMM's 128-channel tiles), "layer4" (ResNet layer4's convolution weights, the
+        FPN and the heads) or "layer3" (layer3 and layer4, the FPN and the heads; both ResNet18/34/50/101/152 FPN only).
+        BatchNorms stay frozen, as the reference's FixedBatchNorm2d.  named_parameters / parameters list the scope's
+        tensors, so build the optimizer after this call.  A parameter keeps its identity across scope changes.
         Returns self."""
-        if scope not in ("heads", "fpn"):
-            raise ValueError("training scope must be 'heads' or 'fpn', got %r" % (scope,))
-        if scope == "fpn" and self.backbone in MOBILENET:
-            raise ValueError("the fpn training scope needs C3 with a multiple of 128 channels; %s's padded C3 has 64 channels"
-                             % self.backbone)
+        if scope not in TRAIN_SCOPES:
+            raise ValueError("training scope must be one of %s, got %r" % (", ".join(TRAIN_SCOPES), scope))
+        if scope != "heads" and self.backbone in MOBILENET:
+            raise ValueError("the %s training scope needs C3 with a multiple of 128 channels; %s's padded C3 has 64 channels"
+                             % (scope, self.backbone))
+        if scope in BACKBONE_SCOPES and self.backbone in RESNEXT:
+            raise ValueError("the %s training scope has no weight gradient for %s's grouped 3x3 convolutions (it would be "
+                             "block-diagonal); train scope 'fpn' or a plain ResNet" % (scope, self.backbone))
         self.train_scope = scope
         return self
 
     def named_parameters(self, prefix="", recurse=True):
         """(name, parameter) of the training scope (set_train_scope), with the reference's names, shapes and order: the
         default scope "heads" lists cls_head.{0,2,4,6,8}.{weight,bias}, then box_head.*; scope "fpn" lists
-        backbones.<backbone>.{lateral3,lateral4,lateral5,pyramid6,pyramid7,smooth3,smooth4,smooth5}.{weight,bias} first.
-        fp32 CUDA leaf tensors, created from the state dict on first request (after .cuda()).  The backbone is frozen: it
-        has no backward kernels here and is never listed.  Once the parameters exist, the training-mode forward returns
-        losses connected to them (the backward runs on the sm_90a kernels: odtk_conv_wgrad, odtk_conv_wgrad_ex,
-        odtk_conv2d_dgrad, odtk_pool_add_f16, odtk_dilate_f16), and every forward uses their current values (the fp16
-        weights are repacked when a parameter changed, e.g. after optimizer.step())."""
+        backbones.<backbone>.{lateral3,lateral4,lateral5,pyramid6,pyramid7,smooth3,smooth4,smooth5}.{weight,bias} first;
+        scopes "layer4" / "layer3" list before those the stages' convolution weights, per block conv1, conv2(, conv3),
+        downsample.0 (backbones.<backbone>.features.layer3.0.conv1.weight, ...).  BatchNorm values are never parameters.
+        fp32 CUDA leaf tensors, created from the state dict on first request (after .cuda()).  The stem, layer1 and layer2
+        are frozen.  Once the parameters exist, the training-mode forward returns losses connected to them (the backward
+        runs on the sm_90a kernels: odtk_conv_wgrad, odtk_conv_wgrad_ex, odtk_conv2d_dgrad, odtk_pool_add_f16,
+        odtk_dilate_f16, odtk_dilate_ex_f16), and every forward uses their current values (the fp16 weights are repacked,
+        BatchNorm folded, when a parameter changed, e.g. after optimizer.step())."""
         names = self._param_names()
         if self._params is None or any(n not in self._params for n in names):
             if self._packed is None or self.device is None:
@@ -502,9 +546,10 @@ class Model:
                 if n not in self._params:
                     self._params[n] = torch.nn.Parameter(self._sd[n].to(self.device, torch.float32).clone())
                     self._sd_versions[n] = self._params[n]._version
-            for _, _, _, wn, bn in self._trainable_layers():
-                if wn not in self._param_versions:      # the packed layer holds the state dict's values
-                    self._param_versions[wn] = (self._params[wn]._version, self._params[bn]._version)
+            for _, c in self._trainable_layers():
+                if c["conv"] + ".weight" not in self._param_versions:      # the packed layer holds the state dict's values
+                    self._param_versions[c["conv"] + ".weight"] = tuple(p._version if p is not None else None
+                                                                        for p in self._layer_params(c))
         for n in names:
             yield prefix + n, self._params[n]
 
@@ -529,22 +574,29 @@ class Model:
                     self._sd_versions[n] = p._version
 
     def _sync_params(self):
-        """Repack the fp16 weights of every head or FPN layer whose parameters changed since they were packed (then the
-        fp32 weights are dropped, the INT8 network is rebuilt and CUDA graphs are recaptured); counts the forward pass."""
+        """Repack the fp16 weights of every trainable layer whose parameters changed since they were packed -- a backbone
+        weight folded with its frozen BatchNorm (the fp32 product fold_bn computes, so the packing equals a fresh model's),
+        with _pack's geometry -- then the fp32 weights are dropped, the INT8 network is rebuilt and CUDA graphs are
+        recaptured; counts the forward pass."""
         self._fwd_gen += 1
         if self._params is None or self._packed is None:
             return
         P, changed = self._packed, False
-        for key, k, stride, wn, bn in self._trainable_layers():
-            w, b = self._params[wn], self._params[bn]
-            v = (w._version, b._version)
+        for path, c in self._trainable_layers():
+            w, b = self._layer_params(c)
+            v = (w._version, b._version if b is not None else None)
+            wn = c["conv"] + ".weight"
             if self._param_versions.get(wn) != v:
                 with torch.no_grad():
-                    conv = _Conv(w.detach(), b.detach().clone(), stride, self.device)
-                if k is None:
-                    P[key] = conv
-                else:
-                    P[key][k] = conv
+                    if b is None:
+                        scale, bias = self._bn_scale_bias(c)
+                        conv = _Conv(w.detach() * scale.view(-1, 1, 1, 1), bias, c["stride"], self.device, c["groups"])
+                    else:
+                        conv = _Conv(w.detach(), b.detach().clone(), c["stride"], self.device)
+                parent = P
+                for key in path[:-1]:
+                    parent = parent[key]
+                parent[path[-1]] = conv
                 self._param_versions[wn] = v
                 changed = True
         if changed:
@@ -574,8 +626,9 @@ class Model:
     def train(self, mode=True):
         """Training-mode forward (odtk/model.py:130-138): `model([images, targets])` returns (cls_loss, box_loss).  Once
         the parameters of the training scope exist (set_train_scope, then named_parameters / parameters), the losses are
-        connected to them and .backward() fills their .grad on the sm_90a backward kernels: the heads, and in scope "fpn"
-        the FPN too; the backbone is frozen (no backward kernels).  An INT8 network table calibrated before training
+        connected to them and .backward() fills their .grad on the sm_90a backward kernels: the heads, in scope "fpn"
+        the FPN too, in scopes "layer4" / "layer3" ResNet stage 4 (and 3) as well; the stem, layer1, layer2 and every
+        BatchNorm stay frozen.  An INT8 network table calibrated before training
         describes the old weights: recalibrate after training.
         Without them, the losses and -- `_compute_loss(..., with_grad=True)` -- their gradients w.r.t. the head outputs
         are what this provides.  The training forward runs in fp16 over the pyramid atlas whatever set_precision chose."""
@@ -862,9 +915,15 @@ class Model:
         blocks = P["blocks"]
         hook = self._calib_hook if self._calib_net else None     # network-scope calibration: layer3 / layer4 tensors
         z_next = None                 # conv1 of THIS block, already computed by the previous block's fused tail (GEMM3)
+        # backbone training scope: keep["blocks"][i] = (block input, post-ReLU conv outputs) of every trained block (they
+        # run conv by conv below: the fused block kernels take only 64 / 128-channel 3x3s, layer1 / layer2's)
+        kept = {i for i, _ in self._backbone_blocks()} if keep is not None else set()
+        if kept:
+            keep["blocks"] = {}
         for bi, blk in enumerate(blocks):
             cs = blk["convs"]
             dn = blk["down"]
+            x_in = x
             if isinstance(cs[0], _ConvS8) and x.dtype == torch.float16:
                 x = outs[3] = engine.quantize_f16_s8(x, P["inv_c3"])
             fp16 = isinstance(cs[0], _Conv)
@@ -908,11 +967,15 @@ class Model:
                     x = engine.bottleneck_tail(out, cs[1].w, cs[1].b, cs[2].w, cs[2].b, identity, relu=True)
             else:
                 out = z_in if z_in is not None else x
+                acts = []
                 for k, c in enumerate(cs[1:-1] if z_in is not None else cs[:-1]):
                     out = c(out, relu=True)
+                    acts.append(out)
                     if tap is not None:
                         tap("%s.conv%d" % (blk["name"], k + 1), out)
                 x = cs[-1](out, relu=True, residual=identity)
+                if bi in kept:
+                    keep["blocks"][bi] = (x_in, acts)
             if tap is not None:
                 tap(blk["name"], x)
             if blk["last"]:
@@ -1172,7 +1235,7 @@ class Model:
         and the state the backward needs."""
         if self._packed is None:
             raise RuntimeError("call .cuda() after loading weights: there is no CPU path")
-        keep = {} if self.train_scope == "fpn" else None
+        keep = {} if self.train_scope != "heads" else None
         views = self._features(self._stem(self._to_nhwc_half(x)), keep)
         P = self._packed
         atlas0 = views[0].atlas
@@ -1208,7 +1271,8 @@ class Model:
         P = self._packed
         names = state["names"]
         need = dict(zip(names, needs))
-        need_fpn = any(need.get(n, False) for n in self._fpn_param_names())
+        need_bb = state["fpn"] is not None and any(need.get(n, False) for n in names if ".features." in n)
+        need_fpn = need_bb or any(need.get(n, False) for n in self._fpn_param_names())
         got = {}
         atlas0 = state["views"][0].atlas
         gbuf = [self._atlas_zeros(at, "gbuf%d" % i) for i in range(4)]    # tower gradient ping-pong + d(atlas) (cls, sum)
@@ -1234,18 +1298,20 @@ class Model:
                     d_atlas = engine.conv2d_dgrad(G, wpk, 256, residual=d_atlas, tile_tab=tab,
                                                   out=gbuf[2] if d_atlas is None else gbuf[3])
         if need_fpn and d_atlas is not None:
-            self._fpn_backward(state, d_atlas, need, got)
+            self._fpn_backward(state, d_atlas, need, got, need_bb)
         self.last_atlas_grad = d_atlas if self.want_atlas_grad else None
         return [got.get(n) for n in names]
 
-    def _fpn_backward(self, state, d_atlas, need, got):
+    def _fpn_backward(self, state, d_atlas, need, got, need_bb=False):
         """The FPN's weight and bias gradients from d(atlas), the gradient w.r.t. the five FPN outputs, into `got`:
         pyramid7 (odtk_conv_wgrad_ex, stride 2 over relu(P6)); dP6 = d(atlas)'s P6 level + the input gradient of pyramid7 --
         dP7 dilated into P6's geometry (odtk_dilate_f16), the stride-1 masked dgrad over P6's tiles, then the plain add
         (odtk_pool_add_f16, pool 1: the dgrad's mask would also zero a residual addend); pyramid6 (stride 2 over C5);
         smooth3-5 (3x3 over the pre-smooth p3-p5); their unmasked input gradients into a pre-smooth gradient atlas, the
         top-down pathway's upsample-add backward (pool 2, level 0 -> 1, then 1 -> 2), then lateral3-5 (1x1 over C3-C5).
-        Only the launches whose results a needed gradient reads run; the backbone gets no gradient."""
+        Only the launches whose results a needed gradient reads run.  need_bb (a backbone parameter needs a gradient):
+        dP6 and the pre-lateral gradients of every level are formed whatever the FPN parameters need, and the backbone
+        backward (_backbone_backward) runs from them."""
         S, at, views = state["fpn"], state["at"], state["views"]
         pre = "backbones.%s." % self.backbone
         rows, tabs, atlas0 = at["rows"], at["tabs"], views[0].atlas
@@ -1258,7 +1324,8 @@ class Model:
             self._wgrad(need, got, pre + layer, engine.conv_wgrad_ex, g, x, 256, ksize, stride, tabs[l], rows[l])
 
         wgrad("pyramid7", d_atlas, S["r6"], 3, 2, 4)
-        if wants("pyramid6"):
+        dp6 = dpre = None
+        if wants("pyramid6") or need_bb:
             gd = engine.dilate(d_atlas, self._atlas_zeros(at, "fpn_dilated"), lv[4], rows[3])
             dp6 = engine.conv2d_dgrad(gd, self._dgrad_weights(pre + "pyramid7.weight", 256), 256, mask=atlas0,
                                       tile_tab=tabs[3], out=self._atlas_zeros(at, "fpn_dp6"))
@@ -1266,7 +1333,7 @@ class Model:
             wgrad("pyramid6", dp6, S["c5"], 3, 2, 3)
         for l in range(3):
             wgrad("smooth%d" % (l + 3), d_atlas, S["p%d" % (l + 3)], 3, 1, l)
-        top = max([l for l in range(3) if wants("lateral%d" % (l + 3))], default=-1)    # lateral l reads levels 0..l
+        top = max([l for l in range(3) if wants("lateral%d" % (l + 3)) or need_bb], default=-1)   # lateral l reads levels 0..l
         if top >= 0:
             dpre = self._atlas_zeros(at, "fpn_dpre")
             for l in range(top + 1):
@@ -1276,6 +1343,88 @@ class Model:
                 engine.pool_add(dpre, dpre, lv[l], lv[l + 1], pool=2)
             for l in range(top + 1):
                 wgrad("lateral%d" % (l + 3), dpre, S["c%d" % (l + 3)], 1, 1, l)
+        if need_bb:
+            self._backbone_backward(state, dpre, dp6, need, got)
+
+    def _backbone_backward(self, state, dpre, dp6, need, got):
+        """The trained ResNet stages' weight gradients into `got`, last block first, from the pre-lateral gradient atlas
+        dpre and dP6 (both atlases of the pyramid's geometry):
+          dC5 = mask(C5 > 0) (lateral5^T dpre[level 2] + pyramid6^T dP6): dP6 scattered to the even positions of C5's
+                geometry (odtk_dilate_ex_f16) through the stride-1 3x3 dgrad, then dpre's level copied out dense through the
+                masked 1x1 dgrad with that as its residual addend;
+          dC4 = mask(C4 > 0) (lateral4^T dpre[level 1] + layer4.0's input gradient) in scope "layer3";
+        then per block _block_backward.  Launches whose results no needed gradient reads are skipped: the lowest trained
+        block, and every block below the lowest one with a needed gradient, computes no input gradient."""
+        S, at, views = state["fpn"], state["at"], state["views"]
+        kept, walk = S["blocks"], self._walk["blocks"]
+        pre = "backbones.%s." % self.backbone
+        lv = [(r, v.h, v.w) for r, v in zip(at["rows"], views)]
+        order = sorted(kept)
+
+        def wants(b):
+            return any(need.get(c["conv"] + ".weight", False) for c in self._block_convs(walk[b]))
+
+        below, seen = {}, False        # below[b]: a block under b needs a gradient, so b's input gradient is needed
+        for b in order:
+            below[b], seen = seen, seen or wants(b)
+        if not seen:
+            return
+
+        def dense(l, like):            # dpre's level l as a dense tensor of C_l's geometry with 256 channels
+            return engine.dilate_into(dpre, lv[l], like.new_empty(like.shape[:3] + (256,)), 1)
+
+        c4, c5 = S["c4"], S["c5"]
+        gd = engine.dilate_into(dp6, lv[3], self._zeros_like(c5.shape[:3] + (256,), c5), 2)
+        t = engine.conv2d_dgrad(gd, self._dgrad_weights(pre + "pyramid6.weight", 256), c5.shape[3])
+        g = engine.conv2d_dgrad(dense(2, c5), self._dgrad_weights(pre + "lateral5.weight", 256), c5.shape[3], mask=c5,
+                                residual=t)
+        for b in reversed(order):
+            if not (wants(b) or below[b]):
+                break
+            blk = walk[b]
+            if blk["level"] == 4 and blk["last"]:      # C4: layer4.0's input gradient meets lateral4's
+                g = engine.conv2d_dgrad(dense(1, c4), self._dgrad_weights(pre + "lateral4.weight", 256), c4.shape[3],
+                                        mask=c4, residual=g)
+            g = self._block_backward(blk, kept[b], g, need, got, below[b])
+
+    def _block_backward(self, blk, saved, g, need, got, need_input):
+        """One residual block's weight gradients into `got` from g, the gradient w.r.t. its output before the final ReLU
+        (dense NHWC fp16); returns the same for the block below (its input gradient, masked by the block input > 0) when
+        need_input, else None.  `saved`: (block input x, post-ReLU outputs of the convolutions before the last).  From the
+        last convolution down: weight gradient (odtk_conv_wgrad_ex over the dense g, BatchNorm scale in its reduce), then
+        the input gradient masked by the convolution's input (odtk_conv2d_dgrad; stride 2 through odtk_dilate_ex_f16 and
+        the stride-1 call).  The downsample's weight gradient reads the block's g; the input gradient is
+        mask(x > 0) (conv1^T dy1 + g, or downsample^T g) -- the downsample's term as the masked residual addend."""
+        x, acts = saved
+        ins = [x] + list(acts)
+        convs, dn = blk["convs"], blk["down"]
+
+        def wgrad(c, gk, xk):
+            wn = c["conv"] + ".weight"
+            if need.get(wn, False):
+                w = self._params[wn]
+                got[wn] = engine.conv_wgrad_ex(gk, xk, w.shape[0], w.shape[2], c["stride"], None, 0, bias=False,
+                                               row_scale=self._bn_scale_bias(c)[0])[0]
+
+        def dgrad(c, gk, xk, residual=None):
+            wk = self._dgrad_weights(c["conv"] + ".weight", gk.shape[3], self._bn_scale_bias(c)[0])
+            if c["stride"] == 2:
+                gk = engine.dilate_into(gk, (0, gk.shape[1], gk.shape[2]), self._zeros_like(xk.shape[:3] + (gk.shape[3],), gk),
+                                        2)
+            return engine.conv2d_dgrad(gk, wk, xk.shape[3], mask=xk, residual=residual)
+
+        if dn is not None:
+            wgrad(dn, g, x)
+        gk = g
+        for k in range(len(convs) - 1, -1, -1):
+            wgrad(convs[k], gk, ins[k])
+            if k == 0 or not (need_input or any(need.get(c["conv"] + ".weight", False) for c in convs[:k])):
+                break
+            gk = dgrad(convs[k], gk, ins[k])
+        if not need_input:
+            return None
+        identity = g if dn is None else dgrad(dn, g, x)
+        return dgrad(convs[0], gk, x, residual=identity)
 
     @staticmethod
     def _wgrad(need, got, layer, launch, *args, **kwargs):
@@ -1289,13 +1438,24 @@ class Model:
             if need.get(bn, False):
                 got[bn] = db
 
-    def _dgrad_weights(self, name, cout_pad):
-        """engine.pack_weight_dgrad of parameter `name`, cached until the parameter changes."""
+    def _dgrad_weights(self, name, cout_pad, bn_scale=None):
+        """engine.pack_weight_dgrad of parameter `name` (times bn_scale per output channel: the BatchNorm-folded weight
+        the forward packed), cached until the parameter changes."""
         p = self._params[name]
         cached = self._dgrad_w.get(name)
         if cached is None or cached[0] != (p._version, id(p)):
-            cached = self._dgrad_w[name] = ((p._version, id(p)), engine.pack_weight_dgrad(p, cout_pad))
+            w = p if bn_scale is None else p.detach() * bn_scale.view(-1, 1, 1, 1)
+            cached = self._dgrad_w[name] = ((p._version, id(p)), engine.pack_weight_dgrad(w, cout_pad))
         return cached[1]
+
+    def _zeros_like(self, shape, like):
+        """A zero-initialised fp16 buffer of `shape` on like's device, one per shape: the stride-2 scatters write only its
+        even positions, so the rest stays zero (stream order: a launch has read it before the next scatter writes it)."""
+        key = (tuple(shape), str(like.device))
+        buf = self._bwd_zeros.get(key)
+        if buf is None:
+            buf = self._bwd_zeros[key] = torch.zeros(key[0], dtype=torch.float16, device=like.device)
+        return buf
 
     @staticmethod
     def _atlas_zeros(at, key, channels=256):

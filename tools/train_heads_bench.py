@@ -7,7 +7,11 @@ repeated launches, FLOPs = 2 * pixels of the levels * 256 * 9 * 256).
 backward (the same step with every FPN parameter frozen but d(atlas) computed) and FPN backward (the rest), and per
 launch the time and TFLOP/s of each FPN layer's weight gradient (odtk_conv_wgrad_ex) next to its forward launch (FLOPs =
 2 * output pixels * 256 * k^2 * Cin).
-    python tools/train_heads_bench.py [--batch 8] [--steps 10] [--scope heads|fpn]"""
+--scope layer4 / layer3 trains ResNet stage 4 (and 3) as well and adds the backbone backward to the split (the FPN
+backward is then measured with every backbone parameter frozen, the head backward with the FPN frozen too), and per
+launch each trained backbone convolution's forward, weight gradient (odtk_conv_wgrad_ex over its dense output gradient)
+and input gradient (odtk_conv2d_dgrad, stride 2 including its scatter) with FLOPs = 2 * output pixels * Cout * k^2 * Cin.
+    python tools/train_heads_bench.py [--batch 8] [--steps 10] [--scope heads|fpn|layer4|layer3]"""
 import argparse
 import json
 import os
@@ -38,7 +42,7 @@ def main():
     ap.add_argument("--batch", type=int, default=8)
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--classes", type=int, default=80)
-    ap.add_argument("--scope", choices=("heads", "fpn"), default="heads")
+    ap.add_argument("--scope", choices=("heads", "fpn", "layer4", "layer3"), default="heads")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "this benchmark needs a GPU"
     dev = "cuda:0"
@@ -102,20 +106,25 @@ def main():
         fn()
         ms = timed(fn, 20)
         per_launch[k] = {"ms": round(ms, 4), "tflops": round(flops / ms / 1e9, 1)}
-    head_bwd = None
-    if args.scope == "fpn":
+    head_bwd = fpn_bwd = None
+    if args.scope != "heads":
         params = dict(m.named_parameters())
-        fpn = m._fpn_param_names()
-        for k in fpn:                     # the heads' share: the same backward with d(atlas) but no FPN gradient
-            params[k].requires_grad_(False)
-        m.want_atlas_grad = True
-        split_h = []
-        for _ in range(args.steps):
-            step(split_h)
-        m.want_atlas_grad = False
-        for k in fpn:
-            params[k].requires_grad_(True)
-        head_bwd = sum(s[1] for s in split_h) / len(split_h)
+        fpn, bb = m._fpn_param_names(), m._backbone_param_names()
+
+        def backward_without(frozen):     # the backward of the same step with `frozen` parameters frozen
+            for k in frozen:
+                params[k].requires_grad_(False)
+            m.want_atlas_grad = True
+            split_f = []
+            for _ in range(args.steps):
+                step(split_f)
+            m.want_atlas_grad = False
+            for k in frozen:
+                params[k].requires_grad_(True)
+            return sum(s[1] for s in split_f) / len(split_f)
+
+        head_bwd = backward_without(fpn + bb)    # the heads' share: d(atlas) but no FPN or backbone gradient
+        fpn_bwd = backward_without(bb) - head_bwd if bb else None
         S, views = st["fpn"], st["views"]
         rows, tabs = at["rows"], at["tabs"]
         ga = (torch.randn(a0.shape, generator=g) * 0.01).half().to(dev)
@@ -138,6 +147,30 @@ def main():
                 fn()
                 ms = timed(fn, 20)
                 per_launch["%s_%s" % (name, key)] = {"ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}
+        for bi, blk in m._backbone_blocks():
+            xb, acts = S["blocks"][bi]
+            ins, pb = [xb] + list(acts), P["blocks"][bi]
+            for k, c in enumerate(m._block_convs(blk)):
+                conv, xin = (pb["convs"] + [pb["down"]])[k], ins[k] if k < len(blk["convs"]) else xb
+                w = params[c["conv"] + ".weight"]
+                scale = m._bn_scale_bias(c)[0]
+                oh, ow = (xin.shape[1] - 1) // c["stride"] + 1, (xin.shape[2] - 1) // c["stride"] + 1
+                gd = (torch.randn((args.batch, oh, ow, w.shape[0]), generator=g) * 0.01).half().to(dev)
+                wdg = m._dgrad_weights(c["conv"] + ".weight", w.shape[0], scale)
+                zbuf = torch.zeros(xin.shape[:3] + (w.shape[0],), dtype=torch.float16, device=dev)
+
+                def dg(gd=gd, wdg=wdg, zbuf=zbuf, xin=xin, s=c["stride"]):
+                    src = engine.dilate_into(gd, (0, gd.shape[1], gd.shape[2]), zbuf, 2) if s == 2 else gd
+                    engine.conv2d_dgrad(src, wdg, xin.shape[3], mask=xin)
+                fl = 2 * args.batch * oh * ow * w.shape[0] * w.shape[2] * w.shape[3] * w.shape[1]
+                name = c["conv"].split(".features.")[1]
+                for key, fn in (("forward", lambda conv=conv, xin=xin: conv(xin, relu=True)),
+                                ("wgrad", lambda gd=gd, xin=xin, w=w, c=c, scale=scale: engine.conv_wgrad_ex(
+                                    gd, xin, w.shape[0], w.shape[2], c["stride"], None, 0, bias=False, row_scale=scale)),
+                                ("dgrad", dg)):
+                    fn()
+                    ms = timed(fn, 20)
+                    per_launch["%s_%s" % (name, key)] = {"ms": round(ms, 4), "tflops": round(fl / ms / 1e9, 1)}
     try:
         gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
                              capture_output=True, text=True, timeout=20).stdout.strip()
@@ -148,9 +181,14 @@ def main():
            "loss_ms": round(loss_ms, 3), "backward_ms": round(bwd, 3), "tower_launches": per_launch,
            "tower_layer_gflop": round(flops / 1e9, 1)}
     if head_bwd is not None:
-        out["workload"] = out["workload"].replace("heads training", "FPN + heads training")
+        scope = {"fpn": "FPN", "layer4": "layer4 + FPN", "layer3": "layer3-4 + FPN"}[args.scope]
+        out["workload"] = out["workload"].replace("heads training", scope + " + heads training")
         out["head_backward_ms"] = round(head_bwd, 3)
-        out["fpn_backward_ms"] = round(bwd - head_bwd, 3)
+        if fpn_bwd is None:
+            out["fpn_backward_ms"] = round(bwd - head_bwd, 3)
+        else:
+            out["fpn_backward_ms"] = round(fpn_bwd, 3)
+            out["backbone_backward_ms"] = round(bwd - head_bwd - fpn_bwd, 3)
     print(json.dumps(out))
 
 
